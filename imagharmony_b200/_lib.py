@@ -72,6 +72,10 @@ SIGNATURES = {
                                      c_int, c_float, c_void_p]),
     "ih_conv2d_shortcut_f16": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_longlong, c_void_p, c_int, c_void_p, c_int,
                                        c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p]),
+    "ih_conv2d_down_f16": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int,
+                                   c_float, c_void_p]),
+    "ih_vae_posterior_noise_f16": (c_int, [c_void_p, c_longlong, c_void_p, c_int, c_void_p, c_void_p, c_int, c_int,
+                                           c_int, c_longlong, c_int, c_float, c_float, c_void_p]),
     "ih_gemm_set_trace": (None, [c_void_p]),
     "ih_gemm_prefetch_next": (None, [c_void_p, c_longlong]),
     "ih_conv2d_f16": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_longlong, c_void_p, c_void_p, c_int, c_int,

@@ -711,6 +711,48 @@ __global__ void nhwc_to_nchw_kernel(const __half* __restrict__ x, long long ldc,
   }
 }
 
+// ---------------------------------------------------------------------------------------------------------------
+// Image-to-image initial latents from the VAE encoder's moments: posterior sample, scaling and the scheduler's
+// add_noise in one pass.  Rounding points of [3P] diffusers==0.30.0 StableDiffusionXLImg2ImgPipeline.prepare_latents
+// (latents fp16) -> DiagonalGaussianDistribution.sample -> EulerDiscreteScheduler.add_noise:
+//   eps fp32 (force_upcast: the posterior is fp32):
+//     lv = clamp(logvar, -30, 20);  z = mean + exp(0.5 lv) * eps          (fp32, mul and add rounded separately)
+//   eps fp16 (no upcast: every posterior op rounds to fp16):
+//     lv = clamp(logvar, -30, 20);  sd = fp16(exp(fp16(0.5 lv)));  z = fp16(mean + fp16(sd * eps))
+//   then  z = fp16(z);  z = fp16(scaling_factor * z);  x = fp16(z + fp16(noise * fp16(sigma)))
+// moments: NHWC [Bm, HW, ldc], mean = channels [0, C), logvar = [C, 2C) (the padded conv_out of the encoder).
+// Output image b uses moments[b % Bm] and eps[b % Be] (diffusers tiles a batch of encoded latents with torch.cat).
+// eps, noise and out are NCHW; noise and out hold B images.
+// ---------------------------------------------------------------------------------------------------------------
+__global__ void vae_posterior_noise_kernel(const __half* __restrict__ moments, long long ldc, const void* __restrict__ eps,
+                                           int eps_f32, const __half* __restrict__ noise, __half* __restrict__ out, int B,
+                                           int Bm, int Be, long long HW, int C, float scaling_factor, float sigma) {
+  pdl_launch_dependents();
+  pdl_wait();
+  const long long total = (long long)B * C * HW;
+  const float sig16 = __half2float(__float2half_rn(sigma));
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+    const long long p = i % HW;
+    const int c = (int)((i / HW) % C);
+    const int b = (int)(i / (HW * C));
+    const __half* mrow = moments + ((long long)(b % Bm) * HW + p) * ldc;
+    const float mean = __half2float(mrow[c]);
+    const float lv = fminf(fmaxf(__half2float(mrow[C + c]), -30.f), 20.f);
+    const long long ei = ((long long)(b % Be) * C + c) * HW + p;
+    float z;
+    if (eps_f32) {
+      z = __fadd_rn(mean, __fmul_rn(expf(0.5f * lv), static_cast<const float*>(eps)[ei]));
+    } else {
+      const float sd = __half2float(__float2half_rn(expf(__half2float(__float2half_rn(0.5f * lv)))));
+      const float e = __half2float(static_cast<const __half*>(eps)[ei]);
+      z = __half2float(__float2half_rn(mean + __half2float(__float2half_rn(sd * e))));
+    }
+    const float zs = __half2float(__float2half_rn(__fmul_rn(scaling_factor, __half2float(__float2half_rn(z)))));
+    const float ns = __half2float(__float2half_rn(__half2float(noise[i]) * sig16));   // exact product of two fp16
+    out[i] = __float2half_rn(zs + ns);
+  }
+}
+
 static int grid_for(long long total, int threads) {
   long long b = (total + threads - 1) / threads;
   const long long cap = (long long)num_sms() * 16;
@@ -942,5 +984,23 @@ extern "C" int ih_nhwc_to_nchw_f16(const void* x, long long ldc, void* out, int 
   const long long total = (long long)B * C * HW;
   IH_CUDA(launch_kernel(nhwc_to_nchw_kernel, dim3(grid_for(total, 256)), dim3(256), (size_t)0, (cudaStream_t)stream,
                         (const __half*)x, ldc, (__half*)out, B, HW, C));
+  return 0;
+}
+
+extern "C" int ih_vae_posterior_noise_f16(const void* moments, long long ldc, const void* eps, int eps_f32,
+                                          const void* noise, void* out, int B, int B_moments, int B_eps, long long HW,
+                                          int C, float scaling_factor, float sigma, void* stream) {
+  IH_CHECK(moments && eps && noise && out, IH_ERR_ARG, "ih_vae_posterior_noise_f16: null pointer");
+  IH_CHECK(B >= 1 && B_moments >= 1 && B_eps >= 1 && HW >= 1 && C >= 1, IH_ERR_SHAPE,
+           "ih_vae_posterior_noise_f16: empty shape (B=%d, B_moments=%d, B_eps=%d, C=%d)", B, B_moments, B_eps, C);
+  IH_CHECK(B % B_moments == 0 && B % B_eps == 0, IH_ERR_SHAPE,
+           "ih_vae_posterior_noise_f16: B=%d must be a multiple of B_moments=%d and B_eps=%d", B, B_moments, B_eps);
+  IH_CHECK(ldc >= 2 * C, IH_ERR_SHAPE, "ih_vae_posterior_noise_f16: ldc=%lld cannot hold mean and logvar of %d channels",
+           ldc, C);
+  IH_CHECK(eps_f32 == 0 || eps_f32 == 1, IH_ERR_ARG, "ih_vae_posterior_noise_f16: eps_f32 must be 0 or 1");
+  const long long total = (long long)B * C * HW;
+  IH_CUDA(launch_kernel(vae_posterior_noise_kernel, dim3(grid_for(total, 256)), dim3(256), (size_t)0, (cudaStream_t)stream,
+                        (const __half*)moments, ldc, eps, eps_f32, (const __half*)noise, (__half*)out, B, B_moments, B_eps,
+                        HW, C, scaling_factor, sigma));
   return 0;
 }

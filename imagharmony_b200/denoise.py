@@ -92,7 +92,7 @@ class DenoiseEngine:
             control_guidance_start: float = 0.0, control_guidance_end: float = 1.0, stop_after: Optional[int] = None,
             start_step: int = 0, guidance_rescale: float = 0.0, num_loop_steps: Optional[int] = None,
             callback: Optional[Callable] = None, callback_steps: int = 1,
-            negative_time_ids: Optional[torch.Tensor] = None) -> torch.Tensor:
+            negative_time_ids: Optional[torch.Tensor] = None, begin_step: int = 0) -> torch.Tensor:
         """latents [n,4,h,w] (already scaled by init_noise_sigma; host or device); embeds host or device tensors.
         Returns the latents after the last executed step as a new device tensor.
 
@@ -100,7 +100,13 @@ class DenoiseEngine:
         are the output of a `stop_after=k` call with the same schedule (two-phase PNS: preview all candidates,
         continue only the winner).  `num_loop_steps` = k truncates the timestep list to its first k entries the way
         `denoising_end` does (custom_pipelines.py:307-316: the gating fractions of :326 then use k, the sigma table
-        stays the full schedule's).  `guidance_scale <= 1` runs the UNet on the positive branch only (:223)."""
+        stays the full schedule's).  `guidance_scale <= 1` runs the UNet on the positive branch only (:223).
+
+        `begin_step` = k is image-to-image ([3P] StableDiffusionXLImg2ImgPipeline): the loop runs over the schedule's
+        entries [k, num_loop_steps) starting from `latents` that already carry the noise of sigma[k]; the device step
+        counter starts at k, and the gating fractions and callback indices count from k, i.e. they see the truncated
+        list.  It resumes nothing, so it cannot be combined with `start_step` / `stop_after` (IHError).  The step graphs
+        do not depend on k: image-to-image replays the text-to-image graphs of the same shape."""
         use_cfg = guidance_scale > 1.0                                            # :223
         if use_cfg and (negative_prompt_embeds is None or negative_pooled is None):
             raise IHError("classifier-free guidance needs negative_prompt_embeds / negative_pooled")
@@ -129,14 +135,22 @@ class DenoiseEngine:
             st["time_ids"].copy_(time_ids, non_blocking=True)
         if not 0 <= start_step <= loop_T:
             raise IHError(f"start_step {start_step} outside the {loop_T}-step loop")
+        if begin_step:
+            if start_step or stop_after is not None:
+                raise IHError("begin_step (image-to-image) cannot be combined with start_step / stop_after")
+            if not 0 < begin_step < loop_T:
+                raise IHError(f"begin_step {begin_step} leaves no step of the {loop_T}-step loop")
+            start_step = begin_step
         st["step"].fill_(start_step)
         self.unet.prepare_conditioning(st["ehs"], st["text_embeds"], st["time_ids"])
         ops.scale_model_input(st["latents"], st["model_in"], sigmas, st["step"], duplicate=use_cfg)   # :332-334
 
         steps = loop_T if stop_after is None else min(stop_after, loop_T)
 
+        b0, n_loop = begin_step, loop_T - begin_step                         # the (truncated) list the loop sees
+
         def scale_at(i: int) -> float:
-            off = (i / loop_T < control_guidance_start) or ((i + 1) / loop_T > control_guidance_end)   # :326-329
+            off = ((i - b0) / n_loop < control_guidance_start) or ((i - b0 + 1) / n_loop > control_guidance_end)  # :326-329
             return 0.0 if off else float(ip_scale)
 
         def gkey(scale: float):
@@ -172,8 +186,8 @@ class DenoiseEngine:
             else:
                 self.set_scale(sc)
                 self._step(st, timesteps, sigmas, guidance_scale, use_cfg, rescale)
-            if callback is not None and i % callback_steps == 0:                  # :359-363 (Euler: order 1, no warm-up)
-                callback(i, timesteps[i], st["latents"])
+            if callback is not None and (i - b0) % callback_steps == 0:           # :359-363 (Euler: order 1, no warm-up)
+                callback(i - b0, timesteps[i], st["latents"])
         self.set_scale(ip_scale)
         return st["latents"].clone()
 

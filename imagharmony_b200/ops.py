@@ -176,6 +176,49 @@ def conv3x3(x: torch.Tensor, w_packed: torch.Tensor, bias: Optional[torch.Tensor
     return out
 
 
+def conv3x3_down(x: torch.Tensor, w_packed: torch.Tensor, bias: Optional[torch.Tensor] = None, *,
+                 out: Optional[torch.Tensor] = None, tile_n: int = 0, alpha: float = 1.0) -> torch.Tensor:
+    """alpha * conv3x3(F.pad(x, (0, 1, 0, 1)), stride 2, pad 0) + bias: the VAE encoder's Downsample2D.  x NHWC
+    [B, H, W, Cin] with H, W even; w_packed [Cout, 9*Cin]; returns [B, H/2, W/2, Cout]."""
+    lib = _lib.load()
+    _req(x, "x"); _req(w_packed, "w")
+    B, H, W, Cin = x.shape
+    Cout = w_packed.shape[0]
+    if not x.is_contiguous() or not w_packed.is_contiguous() or w_packed.shape[1] != 9 * Cin:
+        raise IHError("conv3x3_down: x must be contiguous NHWC and w_packed [Cout, 9*Cin]")
+    if out is None:
+        out = torch.empty((B, H // 2, W // 2, Cout), dtype=torch.float16, device=x.device)
+    rc = lib.ih_conv2d_down_f16(x.data_ptr(), w_packed.data_ptr(), _p(bias), out.data_ptr(), B, H, W, Cin, Cout, tile_n,
+                                float(alpha), _stream())
+    check(rc, "ih_conv2d_down_f16")
+    return out
+
+
+def vae_posterior_noise(moments: torch.Tensor, eps: torch.Tensor, noise: torch.Tensor, channels: int,
+                        scaling_factor: float, sigma: float, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """Image-to-image initial latents (ih_vae_posterior_noise_f16): moments NHWC [Bm, h, w, >= 2*channels] fp16, eps
+    NCHW [Be, channels, h, w] fp32 or fp16, noise NCHW [B, channels, h, w] fp16 -> NCHW fp16 [B, channels, h, w];
+    image b uses moments[b % Bm] and eps[b % Be]."""
+    lib = _lib.load()
+    _req(moments, "moments"); _req(noise, "noise")
+    if eps.dtype not in (torch.float32, torch.float16):
+        raise IHError(f"vae_posterior_noise: eps must be float32 or float16, got {eps.dtype}")
+    _req(eps, "eps", eps.dtype)
+    Bm, h, w, ldc = moments.shape
+    B = noise.shape[0]
+    if (not (moments.is_contiguous() and eps.is_contiguous() and noise.is_contiguous())
+            or tuple(noise.shape) != (B, channels, h, w) or tuple(eps.shape[1:]) != (channels, h, w)):
+        raise IHError(f"vae_posterior_noise: contiguous eps [*, {channels}, {h}, {w}] and noise [B, {channels}, {h}, {w}] "
+                      "required")
+    if out is None:
+        out = torch.empty((B, channels, h, w), dtype=torch.float16, device=moments.device)
+    rc = lib.ih_vae_posterior_noise_f16(moments.data_ptr(), ldc, eps.data_ptr(), int(eps.dtype == torch.float32),
+                                        noise.data_ptr(), out.data_ptr(), B, Bm, eps.shape[0], h * w, channels,
+                                        float(scaling_factor), float(sigma), _stream())
+    check(rc, "ih_vae_posterior_noise_f16")
+    return out
+
+
 def pack_conv3x3_weight(w_oihw: torch.Tensor) -> torch.Tensor:
     """[Cout, Cin, 3, 3] (nn.Conv2d) -> [Cout, 9*Cin] tap-major, the layout ih_conv2d_f16 expects."""
     Cout, Cin, kh, kw = w_oihw.shape

@@ -42,6 +42,17 @@ class EulerDiscreteScheduler:
         self.schedule = EulerSchedule(ts.astype(np.float32), sigmas, float((sigmas.max() ** 2 + 1) ** 0.5))
         return self.schedule
 
+    @staticmethod
+    def img2img_begin_index(num_inference_steps: int, strength: float) -> int:
+        """[3P] StableDiffusionXLImg2ImgPipeline.get_timesteps: an image-to-image run of `strength` skips the first
+        t_start entries of the schedule and denoises over timesteps[t_start:] (the scheduler's begin index)."""
+        init_timestep = min(int(num_inference_steps * strength), num_inference_steps)
+        return max(num_inference_steps - init_timestep, 0)
+
+    def add_noise_sigma(self, begin_index: int) -> float:
+        """The sigma EulerDiscreteScheduler.add_noise scales the noise with before the first image-to-image step."""
+        return float(self.sigmas[begin_index])
+
     @property
     def timesteps(self):
         return self.schedule.timesteps

@@ -22,6 +22,17 @@ so each consumer normalises the scaled stream directly; every conv / linear that
 accumulator and bias by s in the GEMM epilogue (`alpha`), shortcuts / upsampler convs are linear in the stream and only
 scale their bias.  In real arithmetic this is exact; in fp16 it moves the representable range from 6.5e4 to 8.4e6 while
 the weights stay untouched.  `force_upcast = False` configurations (the fp16-fix checkpoint) run with s = 1.
+
+`AutoencoderKLEncoder` is the other half (image-to-image: [3P] StableDiffusionXLImg2ImgPipeline.prepare_latents ->
+`vae.encode(image)`), with diffusers' `encoder.*` / `quant_conv.*` keys and the same scaled residual stream:
+
+* `encoder.conv_in` (3x3, 3->C): `ih_im2col3x3_nchw_f16` [B*H*W, 27 -> 64] + one scaled GEMM (alpha = s);
+* DownEncoderBlock2D: ResnetBlock2D as in the decoder, then Downsample2D(padding=0) = zero pad of one row / column at
+  the bottom and right + 3x3 conv stride 2 (`ih_conv2d_down_f16`, linear in the stream: only its bias is scaled);
+* the mid block of the decoder (ResBlock, single-head attention, ResBlock);
+* GroupNorm+SiLU, then `conv_out` (3x3, C->8) with `quant_conv` (1x1, 8->8) folded into it,
+  W'[:, :, tap] = W_q W_out[:, :, tap], b' = W_q b_out + b_q, Cout padded 8 -> 16.  Its output are the moments
+  (mean = channels 0-3, logvar = 4-7) in fp16, where the reference's upcast VAE has them in fp32.
 """
 from __future__ import annotations
 
@@ -325,6 +336,199 @@ class AutoencoderKLDecoder(nn.Module):
         x = ops.groupnorm(x, dec.conv_norm_out.weight, dec.conv_norm_out.bias, groups=g, eps=1e-6 * s * s, silu=True)
         x = ops.conv3x3(x, self._w_out, self._b_out)
         return ops.nhwc_to_nchw(x, self.config.out_channels)
+
+
+class VAEDownsample(nn.Module):
+    """[3P] Downsample2D(use_conv=True, padding=0): F.pad(x, (0, 1, 0, 1)) then a 3x3 conv with stride 2."""
+
+    def __init__(self, ch: int):
+        super().__init__()
+        self.conv = nn.Conv2d(ch, ch, 3, stride=2, padding=0)
+        self._w = None
+
+    def finalize(self, s: float = 1.0):
+        self._w = ops.pack_conv3x3_weight(self.conv.weight.detach())
+        self._b = _scaled(self.conv.bias, s)
+
+    def forward(self, x):
+        return ops.conv3x3_down(x, self._w, self._b)                 # linear in the scaled stream: only the bias scales
+
+
+class VAEDownBlock(nn.Module):
+    """[3P] DownEncoderBlock2D."""
+
+    def __init__(self, cin: int, cout: int, n_res: int, groups: int, add_down: bool):
+        super().__init__()
+        self.resnets = nn.ModuleList([VAEResnetBlock(cin if j == 0 else cout, cout, groups) for j in range(n_res)])
+        if add_down:
+            self.downsamplers = nn.ModuleList([VAEDownsample(cout)])
+        self.has_down = add_down
+
+    def forward(self, x):
+        for r in self.resnets:
+            x = r(x)
+        return self.downsamplers[0](x) if self.has_down else x
+
+
+class Encoder(nn.Module):
+    def __init__(self, cfg: VAEConfig):
+        super().__init__()
+        ch = cfg.block_out_channels
+        g = cfg.norm_num_groups
+        self.conv_in = nn.Conv2d(cfg.out_channels, ch[0], 3, padding=1)
+        downs: List[nn.Module] = []
+        prev = ch[0]
+        for i, c in enumerate(ch):
+            downs.append(VAEDownBlock(prev, c, cfg.layers_per_block, g, add_down=i < len(ch) - 1))
+            prev = c
+        self.down_blocks = nn.ModuleList(downs)
+        self.mid_block = VAEMidBlock(ch[-1], g)
+        self.conv_norm_out = nn.GroupNorm(g, ch[-1], eps=1e-6)
+        self.conv_out = nn.Conv2d(ch[-1], 2 * cfg.latent_channels, 3, padding=1)
+
+
+class AutoencoderKLEncoder(nn.Module):
+    """`encode(image)` = diffusers `quant_conv(vae.encoder(image))`, the moments of the latent posterior."""
+
+    MOMENT_PAD = 16                       # conv_out's Cout (2 * latent_channels) padded for the conv kernel's tiles
+
+    def __init__(self, cfg: VAEConfig = SDXL_VAE):
+        super().__init__()
+        self.config = cfg
+        self.encoder = Encoder(cfg)
+        self.quant_conv = nn.Conv2d(2 * cfg.latent_channels, 2 * cfg.latent_channels, 1)
+        self._w_in = self._w_out = self._b_out = None
+        self.use_tiling = False
+        self.stream_scale = 2.0 ** -7 if getattr(cfg, "force_upcast", True) else 1.0      # as AutoencoderKLDecoder
+
+    # ---- construction ------------------------------------------------------------------------------------------
+    @classmethod
+    def from_state_dict(cls, cfg: VAEConfig, sd: Dict[str, torch.Tensor], device="cuda",
+                        stream_scale: Optional[float] = None) -> "AutoencoderKLEncoder":
+        """`sd` may be a whole `vae/diffusion_pytorch_model*.safetensors`: only `encoder.*` / `quant_conv.*` are read."""
+        with torch.device("meta"):
+            m = cls(cfg)
+        if stream_scale is not None:
+            if stream_scale <= 0 or math.log2(stream_scale) != int(math.log2(stream_scale)):
+                raise IHError("stream_scale must be a power of two")
+            m.stream_scale = float(stream_scale)
+        m = m.to_empty(device=device)
+        own = m.state_dict()
+        missing = [k for k in own if k not in sd]
+        if missing:
+            raise KeyError(f"VAE checkpoint lacks {len(missing)} encoder keys, e.g. {missing[:3]}")
+        m.load_state_dict({k: sd[k].to(device=device, dtype=torch.float16).reshape(own[k].shape) for k in own})
+        m = m.half().eval()
+        m.finalize()
+        return m
+
+    def finalize(self) -> None:
+        s = self.stream_scale
+        for mod in self.modules():
+            if isinstance(mod, (VAEResnetBlock, VAEAttention, VAEDownsample)):
+                mod.finalize(s)
+        enc = self.encoder
+        ci = enc.conv_in
+        c0, cin = ci.weight.shape[0], ci.weight.shape[1]
+        w = torch.zeros((c0, 64), dtype=ci.weight.dtype, device=ci.weight.device)
+        w[:, :cin * 9] = ci.weight.detach().reshape(c0, cin * 9)                     # k = ci*9 + ky*3 + kx
+        self._w_in = w.contiguous()
+        self._b_in = _scaled(ci.bias, s)
+        w_out, b_out = self.folded_conv_out()
+        cpad = self.MOMENT_PAD
+        wp = torch.zeros((cpad,) + tuple(w_out.shape[1:]), dtype=torch.float32, device=w_out.device)
+        wp[:w_out.shape[0]] = w_out
+        bp = torch.zeros((cpad,), dtype=torch.float32, device=w_out.device)
+        bp[:w_out.shape[0]] = b_out
+        dt = enc.conv_out.weight.dtype
+        self._w_out = ops.pack_conv3x3_weight(wp.to(dt))
+        self._b_out = bp.to(dt).contiguous()
+
+    def folded_conv_out(self):
+        """quant_conv o conv_out as ONE 3x3 conv, in fp32: W'[o, c, tap] = sum_m W_q[o, m] W_out[m, c, tap],
+        b' = W_q b_out + b_q."""
+        co, q = self.encoder.conv_out, self.quant_conv
+        m = q.weight.shape[0]
+        wq = q.weight.detach().float().reshape(m, m)
+        w = torch.einsum("om,mcyx->ocyx", wq, co.weight.detach().float())
+        b = wq @ co.bias.detach().float() + q.bias.detach().float()
+        return w, b
+
+    # ---- forward -----------------------------------------------------------------------------------------------
+    @torch.no_grad()
+    def encode(self, image: torch.Tensor) -> torch.Tensor:
+        """image [B, 3, H, W] in [-1, 1] (H, W multiples of 8) -> moments [B, 2 * latent_channels, H/8, W/8]
+        (mean, then logvar), fp16.  With `use_tiling` and an image larger than `sample_size` pixels it is encoded
+        tile by tile, [3P] diffusers `AutoencoderKL.tiled_encode`."""
+        m = self.encode_moments_nhwc(image)
+        return ops.nhwc_to_nchw(m, 2 * self.config.latent_channels)
+
+    @torch.no_grad()
+    def encode_moments_nhwc(self, image: torch.Tensor) -> torch.Tensor:
+        """The moments as the encoder's conv_out writes them: NHWC [B, H/8, W/8, 16], channels [0, 8) valid (the input
+        of ops.vae_posterior_noise)."""
+        if self._w_in is None:
+            raise IHError("AutoencoderKLEncoder.finalize() has not run (use from_state_dict)")
+        if image.dim() != 4 or image.shape[1] != self.config.out_channels or image.shape[2] % 8 or image.shape[3] % 8:
+            raise IHError(f"encode: expected [B, {self.config.out_channels}, H, W] with H, W multiples of 8, got "
+                          f"{tuple(image.shape)}")
+        t = self.config.sample_size
+        if self.use_tiling and (image.shape[-1] > t or image.shape[-2] > t):
+            return self._tiled_encode(image)
+        return self._encode_tile(image)
+
+    def _tiled_encode(self, x: torch.Tensor) -> torch.Tensor:
+        """[3P] tiled_encode: image tiles of `sample_size` pixels every 3/4 tile, each encoded on its own (so tile
+        borders see zero padding, as in diffusers); the tiles' MOMENTS are cross-faded over the overlap with the tile
+        above and the tile to the left and cropped to the stride.  The cross-fade is elementwise torch glue (NHWC)."""
+        cfg = self.config
+        ts = cfg.sample_size
+        tl = cfg.tile_latent_min_size
+        overlap = int(ts * (1 - cfg.tile_overlap_factor))
+        blend = int(tl * cfg.tile_overlap_factor)
+        limit = tl - blend
+        rows = []
+        for i in range(0, x.shape[2], overlap):
+            rows.append([self._encode_tile(x[:, :, i:i + ts, j:j + ts].contiguous()).float()
+                         for j in range(0, x.shape[3], overlap)])
+
+        def blend_v(a, b, ext):
+            ext = min(a.shape[1], b.shape[1], ext)
+            wgt = (torch.arange(ext, device=b.device, dtype=torch.float32) / ext).view(1, ext, 1, 1)
+            b[:, :ext] = a[:, -ext:] * (1 - wgt) + b[:, :ext] * wgt
+            return b
+
+        def blend_h(a, b, ext):
+            ext = min(a.shape[2], b.shape[2], ext)
+            wgt = (torch.arange(ext, device=b.device, dtype=torch.float32) / ext).view(1, 1, ext, 1)
+            b[:, :, :ext] = a[:, :, -ext:] * (1 - wgt) + b[:, :, :ext] * wgt
+            return b
+
+        out_rows = []
+        for i, row in enumerate(rows):
+            out_row = []
+            for j, tile in enumerate(row):
+                if i > 0:
+                    tile = blend_v(rows[i - 1][j], tile, blend)
+                if j > 0:
+                    tile = blend_h(row[j - 1], tile, blend)
+                out_row.append(tile[:, :limit, :limit])
+            out_rows.append(torch.cat(out_row, dim=2))
+        return torch.cat(out_rows, dim=1).to(self._w_in.dtype).contiguous()
+
+    def _encode_tile(self, image: torch.Tensor) -> torch.Tensor:
+        B, _, H, W = image.shape
+        enc = self.encoder
+        dt = self._w_in.dtype                                     # fp16 on the GPU (fp32 only in the CPU wiring test)
+        a = ops.im2col3x3_nchw(image.to(dt).contiguous(), self._w_in.shape[1])
+        s = self.stream_scale
+        x = ops.linear(a, self._w_in, self._b_in, alpha=s).reshape(B, H, W, -1)          # s * conv_in
+        for blk in enc.down_blocks:
+            x = blk(x)
+        x = enc.mid_block(x)
+        g = self.config.norm_num_groups
+        x = ops.groupnorm(x, enc.conv_norm_out.weight, enc.conv_norm_out.bias, groups=g, eps=1e-6 * s * s, silu=True)
+        return ops.conv3x3(x, self._w_out, self._b_out)              # quant_conv o conv_out, unscaled moments
 
 
 def postprocess(image: torch.Tensor, output_type: str = "pil"):

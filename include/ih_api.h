@@ -89,6 +89,13 @@ int ih_conv2d_shortcut_f16(const void* x, const void* w, const void* bias, const
 int ih_conv2d_scaled_f16(const void* x, const void* w, const void* bias, const void* residual, void* out, int B, int Hin,
                          int Win, int Cin, int Cout, int stride, float alpha, void* stream);
 
+/* out = alpha * conv(x) + bias: 3x3 conv, stride 2, padded by one zero row / column at the BOTTOM and RIGHT only
+ * (Ho = Hin / 2, Wo = Win / 2; Hin, Win even).  Replaces [3P] diffusers Downsample2D(padding=0) of the VAE encoder
+ * (`F.pad(x, (0, 1, 0, 1))` then Conv2d(stride 2, padding 0)); alpha serves the encoder's scaled residual stream.
+ * Same weight layout and tile_n values as ih_conv2d_f16. */
+int ih_conv2d_down_f16(const void* x, const void* w, const void* bias, void* out, int B, int Hin, int Win, int Cin,
+                       int Cout, int tile_n, float alpha, void* stream);
+
 /* Multi-head attention, head_dim 64, softmax scale 1/8, no mask.
  *   q: [B, Nq, *] rows with ldq elements per row, head h at columns [h*64, h*64+64) (same for k, v, out).
  *   Self attention (n_ip == 0): out = softmax(q k^T / 8) v over Nk keys.
@@ -186,6 +193,17 @@ int ih_conv_out_f16(const void* x, const void* w, const void* bias, void* out_nc
 int ih_im2col3x3_nchw_f16(const void* x_nchw, void* out, int B, int Cin, int H, int W, int Kpad, void* stream);
 /* conv_out on ih_conv2d_f16 with Cout padded to 16: gather NHWC [B, HW, ldc] channels [0, C) into NCHW [B, C, HW]. */
 int ih_nhwc_to_nchw_f16(const void* x, long long ldc, void* out, int B, long long HW, int C, void* stream);
+
+/* Image-to-image initial latents ([3P] diffusers StableDiffusionXLImg2ImgPipeline.prepare_latents with fp16 latents):
+ *   z = posterior sample of the VAE encoder's moments (mean + exp(0.5 clamp(logvar, -30, 20)) * eps),
+ *   out = fp16(fp16(scaling_factor * fp16(z)) + fp16(noise * fp16(sigma)))   (EulerDiscreteScheduler.add_noise).
+ * moments: NHWC fp16 [B_moments, HW, ldc] (mean = channels [0, C), logvar = [C, 2C)); eps: NCHW [B_eps, C, HW], fp32
+ * (eps_f32 = 1: the fp32 posterior of an upcast VAE) or fp16 (eps_f32 = 0: fp16 posterior, fp16 rounding after every
+ * op); noise, out: NCHW fp16 [B, C, HW].  Image b reads moments[b % B_moments] and eps[b % B_eps] (the torch.cat tiling
+ * of encoded latents); B must be a multiple of both.  eps and noise are drawn by the caller from its generators. */
+int ih_vae_posterior_noise_f16(const void* moments, long long ldc, const void* eps, int eps_f32, const void* noise,
+                               void* out, int B, int B_moments, int B_eps, long long HW, int C, float scaling_factor,
+                               float sigma, void* stream);
 
 /* One scheduler transition (custom_pipelines.py:332-334,348-357):
  *   eps = u + g (c - u)  (fp16 tensor arithmetic, rounded like the reference's);

@@ -20,6 +20,7 @@ from typing import Any, Callable, Dict, List, Optional, Tuple, Union
 
 import torch
 
+from imagharmony_b200 import ops
 from imagharmony_b200._lib import IHError
 from imagharmony_b200.config import SDXL_BASE, UNetConfig
 from imagharmony_b200.denoise import DenoiseEngine
@@ -95,6 +96,12 @@ class StableDiffusionXLCustomPipeline:
                         cfg: UNetConfig = SDXL_BASE, vae_cfg=None, **kwargs):
         """test.py:68-72.  Loads `<path>/unet/diffusion_pytorch_model.safetensors` (diffusers key names are the native
         UNet's key names, so no key map is needed)."""
+        unet, enc, vae, _, _ = cls._load_pretrained(path, torch_dtype, device, cfg, vae_cfg)
+        return cls(unet, prompt_encoder=enc, vae=vae)
+
+    @staticmethod
+    def _load_pretrained(path: str, torch_dtype, device, cfg: UNetConfig, vae_cfg):
+        """-> (unet, prompt encoder or None, VAE decoder or None, VAE state dict or None, VAE config or None)."""
         from safetensors.torch import load_file
         f = os.path.join(path, "unet", "diffusion_pytorch_model.safetensors")
         if not os.path.exists(f):
@@ -102,7 +109,7 @@ class StableDiffusionXLCustomPipeline:
         if not os.path.exists(f):
             raise FileNotFoundError(f"no SDXL UNet weights under {path}/unet (safetensors)")
         unet = UNet2DConditionModel.from_state_dict(cfg, load_file(f), device=device)
-        vae = None
+        vae = vsd = vcfg = None
         for name in ("diffusion_pytorch_model.fp16.safetensors", "diffusion_pytorch_model.safetensors"):
             vf = os.path.join(path, "vae", name)
             if os.path.exists(vf):
@@ -118,13 +125,14 @@ class StableDiffusionXLCustomPipeline:
                     meta = json.load(open(cj))
                     vcfg = dataclasses.replace(vcfg, force_upcast=bool(meta.get("force_upcast", True)),
                                                scaling_factor=float(meta.get("scaling_factor", vcfg.scaling_factor)))
-                vae = AutoencoderKLDecoder.from_state_dict(vcfg, load_file(vf), device=device)  # decoder keys only
+                vsd = load_file(vf)
+                vae = AutoencoderKLDecoder.from_state_dict(vcfg, vsd, device=device)  # decoder keys only
                 break
         enc = None
         from .encoders import ClipPromptEncoder
         if ClipPromptEncoder.available(path):
             enc = ClipPromptEncoder.from_pretrained(path, device=device, dtype=torch_dtype)
-        return cls(unet, prompt_encoder=enc, vae=vae)
+        return unet, enc, vae, vsd, vcfg
 
     def to(self, device=None, *args, **kwargs):
         """Weights live on the device the UNet was built on (from_random / from_pretrained take `device=`); moving 5 GB
@@ -252,6 +260,10 @@ class StableDiffusionXLCustomPipeline:
         else:
             out = lat.to(self.device)
         self.set_scale(conditioning_scale)
+        return self._output(out, output_type, return_dict)
+
+    def _output(self, out: torch.Tensor, output_type: Optional[str], return_dict: bool):
+        """Final latents -> images (:365-386) in the requested output type."""
         if output_type == "latent":
             image = out
         else:
@@ -266,3 +278,195 @@ class StableDiffusionXLCustomPipeline:
         if not return_dict:
             return (image,)
         return StableDiffusionXLPipelineOutput(images=image)
+
+
+def preprocess_image(image, vae_scale_factor: int = 8) -> torch.Tensor:
+    """[3P] diffusers VaeImageProcessor.preprocess (SDXL defaults: resize with Lanczos, normalise): PIL image(s) ->
+    float32 [B, 3, H, W] in [-1, 1] with H, W floored to multiples of `vae_scale_factor` (every image takes the first
+    one's size).  A [B, 3, H, W] / [3, H, W] tensor is taken as it is, resized (nearest) when its size is not a multiple
+    of the factor; as in diffusers it is expected in [-1, 1], and one without negative values is taken as [0, 1] and
+    normalised."""
+    import numpy as np
+    from PIL import Image
+    if isinstance(image, Image.Image) or (isinstance(image, (list, tuple)) and image and isinstance(image[0], Image.Image)):
+        images = [image] if isinstance(image, Image.Image) else list(image)
+        w, h = (x - x % vae_scale_factor for x in images[0].size)
+        if w <= 0 or h <= 0:
+            raise ValueError(f"image of size {images[0].size} is smaller than {vae_scale_factor} pixels")
+        images = [im.convert("RGB") if im.mode != "RGB" else im for im in images]
+        images = [im if im.size == (w, h) else im.resize((w, h), resample=Image.LANCZOS) for im in images]
+        arr = np.stack([np.array(im).astype(np.float32) / 255.0 for im in images])
+        return torch.from_numpy(arr).permute(0, 3, 1, 2).contiguous() * 2.0 - 1.0
+    if isinstance(image, torch.Tensor):
+        x = image.unsqueeze(0) if image.dim() == 3 else image
+        if x.dim() != 4 or x.shape[1] != 3:
+            raise ValueError(f"image tensor must be [B, 3, H, W] or [3, H, W], got {tuple(image.shape)}")
+        x = x.float()
+        h, w = (v - v % vae_scale_factor for v in x.shape[2:])
+        if h <= 0 or w <= 0:
+            raise ValueError(f"image of size {tuple(x.shape[2:])} is smaller than {vae_scale_factor} pixels")
+        if (h, w) != tuple(x.shape[2:]):
+            x = torch.nn.functional.interpolate(x, size=(h, w))
+        if x.min() >= 0:
+            x = x * 2.0 - 1.0
+        return x.contiguous()
+    raise ValueError(f"`image` must be a PIL image, a list of them or a tensor, got {type(image).__name__}")
+
+
+class StableDiffusionXLImg2ImgPipeline(StableDiffusionXLCustomPipeline):
+    """Image-to-image with the call surface of [3P] diffusers `StableDiffusionXLImg2ImgPipeline`, so that
+    `IPAdapterXL(img2img_pipe, ...).generate(pil_image=..., image=init, strength=s)` works as it does on the
+    reference built over that pipeline.  The init image is encoded by the native VAE encoder
+    (imagharmony_b200.vae.AutoencoderKLEncoder), its posterior sampled and noised to sigma[t_start] by one kernel
+    (ops.vae_posterior_noise), and the denoise loop runs over timesteps[t_start:] on the same engine and graphs as
+    text-to-image (DenoiseEngine.run(begin_step=t_start)).
+
+    Batch expansion follows diffusers: with one generator the encoded latents of the image batch are tiled to the
+    prompt batch with torch.cat (prompt slot b gets image b % n_images, while num_images_per_prompt repeats prompts
+    in place), with a list of generators each slot encodes image b % n_images with its own generator.
+    The SDXL-base configuration has requires_aesthetics_score = False: `aesthetic_score` / `negative_aesthetic_score`
+    are accepted and unused."""
+
+    # diffusers arguments that change the result and have no native implementation: refused, never ignored
+    UNSUPPORTED = ("denoising_start", "timesteps", "sigmas", "latents", "ip_adapter_image", "ip_adapter_image_embeds",
+                   "clip_skip", "callback_on_step_end")
+
+    def __init__(self, unet: UNet2DConditionModel, prompt_encoder: Optional[Callable] = None,
+                 vae_decode: Optional[Callable] = None, scheduler: Optional[EulerDiscreteScheduler] = None,
+                 vae=None, vae_encoder=None):
+        super().__init__(unet, prompt_encoder=prompt_encoder, vae_decode=vae_decode, scheduler=scheduler, vae=vae)
+        self.vae_encoder = vae_encoder      # imagharmony_b200.vae.AutoencoderKLEncoder or None
+
+    @classmethod
+    def from_random(cls, cfg: UNetConfig = SDXL_BASE, seed: int = 0, device="cuda", vae_cfg=None):
+        """Random-init weights; with `vae_cfg` also a random VAE decoder and encoder."""
+        pipe = super().from_random(cfg, seed=seed, device=device, vae_cfg=vae_cfg)
+        if vae_cfg is not None:
+            from imagharmony_b200.vae import AutoencoderKLEncoder
+            from imagharmony_b200.weights import random_state_dict, shapes_of
+            with torch.device("meta"):
+                shapes = shapes_of(AutoencoderKLEncoder(vae_cfg))
+            gen_dev = device if str(device).startswith("cuda") else "cpu"
+            pipe.vae_encoder = AutoencoderKLEncoder.from_state_dict(vae_cfg, random_state_dict(shapes, seed + 19,
+                                                                                               device=gen_dev),
+                                                                    device=device)
+        return pipe
+
+    @classmethod
+    def from_pretrained(cls, path: str, torch_dtype=torch.float16, add_watermarker: bool = False, device="cuda",
+                        cfg: UNetConfig = SDXL_BASE, vae_cfg=None, **kwargs):
+        """As StableDiffusionXLCustomPipeline.from_pretrained; the VAE checkpoint also provides the encoder."""
+        unet, enc, vae, vsd, vcfg = cls._load_pretrained(path, torch_dtype, device, cfg, vae_cfg)
+        vae_encoder = None
+        if vsd is not None:
+            from imagharmony_b200.vae import AutoencoderKLEncoder
+            vae_encoder = AutoencoderKLEncoder.from_state_dict(vcfg, vsd, device=device)
+        return cls(unet, prompt_encoder=enc, vae=vae, vae_encoder=vae_encoder)
+
+    def enable_vae_tiling(self):
+        super().enable_vae_tiling()
+        if self.vae_encoder is not None:
+            self.vae_encoder.use_tiling = True
+
+    def prepare_img2img_latents(self, image: torch.Tensor, batch_size: int, generator, sigma: float) -> torch.Tensor:
+        """[3P] StableDiffusionXLImg2ImgPipeline.prepare_latents (fp16 latents): encode, sample the posterior, scale,
+        add_noise(sigma).  eps (fp32 when the VAE config asks for the upcast, else fp16) and the fp16 noise are drawn
+        here from the caller's generator(s) in diffusers' order; the arithmetic is one kernel."""
+        venc = self.vae_encoder
+        n_img = image.shape[0]
+        if batch_size % n_img:
+            raise ValueError(f"cannot duplicate an image batch of {n_img} to a prompt batch of {batch_size}")
+        moments = venc.encode_moments_nhwc(image.to(self.device, torch.float16))      # [n_img, h, w, 16]
+        L = venc.config.latent_channels
+        h, w = moments.shape[1], moments.shape[2]
+        eps_dtype = torch.float32 if getattr(venc.config, "force_upcast", True) else torch.float16
+
+        def draw(shape, g, dtype):
+            return torch.randn(shape, generator=g, device=g.device if g is not None else "cpu", dtype=dtype)
+        if isinstance(generator, list):
+            if len(generator) != batch_size:
+                raise ValueError(f"got {len(generator)} generators for a batch of {batch_size}")
+            eps = torch.cat([draw((1, L, h, w), g, eps_dtype).to(self.device) for g in generator])
+            noise = torch.cat([draw((1, L, h, w), g, torch.float16).to(self.device) for g in generator])
+        else:
+            eps = draw((n_img, L, h, w), generator, eps_dtype).to(self.device)
+            noise = draw((batch_size, L, h, w), generator, torch.float16).to(self.device)
+        return ops.vae_posterior_noise(moments, eps.contiguous(), noise.contiguous(), L, venc.config.scaling_factor,
+                                       sigma)
+
+    @torch.no_grad()
+    def __call__(self, prompt: Optional[Union[str, List[str]]] = None, prompt_2=None, image=None, strength: float = 0.3,
+                 num_inference_steps: int = 50, denoising_end: Optional[float] = None, guidance_scale: float = 5.0,
+                 negative_prompt=None, negative_prompt_2=None, num_images_per_prompt: Optional[int] = 1,
+                 eta: float = 0.0, generator=None, prompt_embeds: Optional[torch.Tensor] = None,
+                 negative_prompt_embeds: Optional[torch.Tensor] = None,
+                 pooled_prompt_embeds: Optional[torch.Tensor] = None,
+                 negative_pooled_prompt_embeds: Optional[torch.Tensor] = None, output_type: Optional[str] = "pil",
+                 return_dict: bool = True, callback=None, callback_steps: int = 1,
+                 cross_attention_kwargs: Optional[Dict[str, Any]] = None, guidance_rescale: float = 0.0,
+                 original_size: Optional[Tuple[int, int]] = None, crops_coords_top_left: Tuple[int, int] = (0, 0),
+                 target_size: Optional[Tuple[int, int]] = None, negative_original_size=None,
+                 negative_crops_coords_top_left=(0, 0), negative_target_size=None, aesthetic_score: float = 6.0,
+                 negative_aesthetic_score: float = 2.5, control_guidance_start: float = 0.0,
+                 control_guidance_end: float = 1.0, **kwargs):
+        """The text-to-image parameter list without height / width, plus `image` (PIL image(s) or a [B, 3, H, W]
+        tensor in [-1, 1]) and `strength`.  Unknown keywords are ignored as in the text-to-image pipeline, except the
+        diffusers arguments in UNSUPPORTED, which raise IHError."""
+        refused = [k for k in self.UNSUPPORTED if kwargs.get(k) is not None]
+        if refused:
+            raise IHError(f"StableDiffusionXLImg2ImgPipeline does not implement {refused}")
+        if not 0.0 <= strength <= 1.0:
+            raise ValueError(f"The value of strength should in [0.0, 1.0] but is {strength}")          # [3P] check_inputs
+        if callback is not None and (not isinstance(callback_steps, int) or callback_steps <= 0):
+            raise ValueError(f"`callback_steps` has to be a positive integer but is {callback_steps}")
+        if image is None:
+            raise ValueError("`image` input cannot be undefined")
+        if self.vae_encoder is None:
+            raise IHError("this pipeline has no VAE encoder: build it with from_random(vae_cfg=...) or from_pretrained "
+                          "with a vae/ folder")
+        pixels = preprocess_image(image, self.vae_scale_factor)
+        height, width = pixels.shape[2], pixels.shape[3]
+        original_size = original_size or (height, width)
+        target_size = target_size or (height, width)
+        do_classifier_free_guidance = guidance_scale > 1.0
+        (prompt_embeds, negative_prompt_embeds, pooled_prompt_embeds, negative_pooled_prompt_embeds) = \
+            self.encode_prompt(prompt, prompt_2, None, num_images_per_prompt, do_classifier_free_guidance,
+                               negative_prompt, negative_prompt_2, prompt_embeds, negative_prompt_embeds,
+                               pooled_prompt_embeds, negative_pooled_prompt_embeds)
+        batch = prompt_embeds.shape[0]
+        self.scheduler.set_timesteps(num_inference_steps)
+        t_start = self.scheduler.img2img_begin_index(num_inference_steps, strength)
+        if num_inference_steps - t_start < 1:
+            raise ValueError(f"After adjusting the num_inference_steps by strength parameter: {strength}, the number of "
+                             f"pipeline steps is {num_inference_steps - t_start} which is < 1 and not appropriate for "
+                             "this pipeline.")
+        lat = self.prepare_img2img_latents(pixels, batch, generator, self.scheduler.add_noise_sigma(t_start))
+
+        def time_ids(size, crop, target):
+            return torch.tensor([list(size) + list(crop) + list(target)], dtype=torch.float32).repeat(batch, 1)
+        add_time_ids = time_ids(original_size, crops_coords_top_left, target_size)
+        negative_add_time_ids = None
+        if negative_original_size is not None and negative_target_size is not None:
+            negative_add_time_ids = time_ids(negative_original_size, negative_crops_coords_top_left, negative_target_size)
+        loop_end = num_inference_steps
+        if denoising_end is not None and isinstance(denoising_end, float) and 0 < denoising_end < 1:
+            n_train = self.scheduler.num_train_timesteps
+            cutoff = int(round(n_train - denoising_end * n_train))
+            loop_end = t_start + int(sum(1 for t in self.scheduler.timesteps[t_start:] if t >= cutoff))
+        conditioning_scale = 1.0
+        for attn_processor in self.unet.attn_processors.values():
+            if isinstance(attn_processor, IPAttnProcessor):
+                conditioning_scale = attn_processor.scale
+                break
+        if loop_end > t_start:
+            out = self.engine.run(lat, prompt_embeds, negative_prompt_embeds, pooled_prompt_embeds,
+                                  negative_pooled_prompt_embeds, add_time_ids, num_inference_steps,
+                                  guidance_scale=guidance_scale, ip_scale=conditioning_scale,
+                                  control_guidance_start=control_guidance_start,
+                                  control_guidance_end=control_guidance_end, guidance_rescale=guidance_rescale,
+                                  num_loop_steps=loop_end, callback=callback, callback_steps=callback_steps,
+                                  negative_time_ids=negative_add_time_ids, begin_step=t_start)
+        else:
+            out = lat
+        self.set_scale(conditioning_scale)
+        return self._output(out, output_type, return_dict)
