@@ -351,6 +351,128 @@ __global__ void __launch_bounds__(1024) euler_ex_kernel(const __half* __restrict
   }
 }
 
+// ---------------------------------------------------------------------------------------------------------------
+// Inpainting step ([3P] diffusers==0.30.0 StableDiffusionXLInpaintPipeline, 4-channel UNet): the transition of
+// euler_cfg_kernel / euler_ex_kernel (same rounding points), then, before the next step's input is formed, the blend
+//   proper = i + 1 < blend_end ? fp16(img + fp16(noise * fp16(sigma[i+1]))) : img     (add_noise after step())
+//   x      = fp16(fp16(fp16(1 - m) * proper) + fp16(m * x_euler))                      (fp16 tensor arithmetic)
+// with m = mask[b, pixel] broadcast over the 4 latent channels.  The last step of the loop blends with the clean
+// image latents even when sigma[blend_end] is not 0 (denoising_end).  image_latents / noise: [n,4,h,w], mask [n,1,h,w].
+// ---------------------------------------------------------------------------------------------------------------
+struct InpaintArgs {
+  const __half* image_latents;
+  const __half* noise;
+  const __half* mask;
+  long long hw;          // pixels per image: n_per_image / 4
+  bool renoise;          // i + 1 < blend_end
+  float sig_next16;      // fp16(sigma[i+1])
+};
+
+// One element: Euler update of the guided prediction `eps`, mask blend, latents and next-step input written.
+__device__ __forceinline__ void euler_inpaint_elem(long long idx, float eps, float sigma, float sigma_next, float den_next,
+                                                   const InpaintArgs& ia, long long per_image, long long total, int cfg,
+                                                   __half* __restrict__ latents, __half* __restrict__ model_in) {
+  const float x = __half2float(latents[idx]);
+  const float x0 = x - __half2float(__float2half_rn(sigma * eps));
+  const float deriv = (x - x0) / sigma;
+  const float xn = x + deriv * (sigma_next - sigma);
+  const float xe = __half2float(__float2half_rn(xn));
+  const long long b = idx / per_image;
+  const float m = __half2float(ia.mask[b * ia.hw + (idx - b * per_image) % ia.hw]);
+  float proper = __half2float(ia.image_latents[idx]);
+  if (ia.renoise) proper = __half2float(__float2half_rn(proper + __half2float(__float2half_rn(__half2float(ia.noise[idx]) * ia.sig_next16))));
+  const float keep = __half2float(__float2half_rn(__half2float(__float2half_rn(1.f - m)) * proper));
+  const float gen = __half2float(__float2half_rn(m * xe));
+  const __half xh = __float2half_rn(keep + gen);
+  latents[idx] = xh;
+  const __half mi = __float2half_rn(__half2float(xh) / den_next);
+  model_in[idx] = mi;
+  if (cfg) model_in[total + idx] = mi;
+}
+
+// Without guidance_rescale: grid-stride over all elements.  With it: one block per image (blockIdx.x = image), the
+// per-image std ratio first, reduced in the order of euler_ex_kernel so both forms give the same factor.
+__global__ void __launch_bounds__(1024) euler_inpaint_kernel(const __half* __restrict__ noise, __half* __restrict__ latents,
+                                                             __half* __restrict__ model_in, const float* __restrict__ sigmas,
+                                                             const int* __restrict__ step, float guidance, float rescale,
+                                                             long long per_image, int n_images, int cfg,
+                                                             const __half* __restrict__ image_latents,
+                                                             const __half* __restrict__ blend_noise,
+                                                             const __half* __restrict__ mask,
+                                                             const int* __restrict__ blend_end) {
+  pdl_launch_dependents();
+  pdl_wait();
+  const int i = *step;
+  const float sigma = sigmas[i], sigma_next = sigmas[i + 1];
+  const float den_next = sqrtf(sigma_next * sigma_next + 1.f);
+  const long long total = per_image * n_images;
+  const InpaintArgs ia{image_latents, blend_noise, mask, per_image / 4, i + 1 < *blend_end,
+                       __half2float(__float2half_rn(sigma_next))};
+  auto guided = [&](long long idx, float& c_out) -> float {
+    if (!cfg) {
+      c_out = __half2float(noise[idx]);
+      return c_out;
+    }
+    const float u = __half2float(noise[idx]);
+    const float c = __half2float(noise[total + idx]);
+    c_out = c;
+    const float d1 = __half2float(__float2half_rn(c - u));
+    const float d2 = __half2float(__float2half_rn(guidance * d1));
+    return __half2float(__float2half_rn(u + d2));
+  };
+  const bool resc = cfg && rescale > 0.f;
+  if (!resc) {
+    for (long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x; idx < total;
+         idx += (long long)gridDim.x * blockDim.x) {
+      float c;
+      euler_inpaint_elem(idx, guided(idx, c), sigma, sigma_next, den_next, ia, per_image, total, cfg, latents, model_in);
+    }
+    return;
+  }
+  const long long base = (long long)blockIdx.x * per_image;
+  double s_t = 0.0, q_t = 0.0, s_g = 0.0, q_g = 0.0;
+  for (long long e = threadIdx.x; e < per_image; e += blockDim.x) {
+    float c;
+    const float g = guided(base + e, c);
+    s_t += c;
+    q_t += (double)c * c;
+    s_g += g;
+    q_g += (double)g * g;
+  }
+  __shared__ double red[4][32];
+  __shared__ float s_factor;
+  double v[4] = {s_t, q_t, s_g, q_g};
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    for (int o = 16; o > 0; o >>= 1) v[k] += __shfl_xor_sync(0xffffffffu, v[k], o);
+    if ((threadIdx.x & 31) == 0) red[k][threadIdx.x >> 5] = v[k];
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double t[4] = {0, 0, 0, 0};
+    const int nw = (blockDim.x + 31) >> 5;
+    for (int k = 0; k < 4; ++k)
+      for (int w = 0; w < nw; ++w) t[k] += red[k][w];
+    const double n = (double)per_image;
+    const double var_t = fmax((t[1] - t[0] * t[0] / n) / (n - 1.0), 0.0);
+    const double var_g = fmax((t[3] - t[2] * t[2] / n) / (n - 1.0), 0.0);
+    const float std_t = __half2float(__float2half_rn((float)sqrt(var_t)));
+    const float std_g = __half2float(__float2half_rn((float)sqrt(var_g)));
+    s_factor = __half2float(__float2half_rn(std_t / std_g));
+  }
+  __syncthreads();
+  const float factor = s_factor;
+  for (long long e = threadIdx.x; e < per_image; e += blockDim.x) {
+    float c;
+    const float eps = guided(base + e, c);
+    const float r = __half2float(__float2half_rn(eps * factor));
+    const float a = __half2float(__float2half_rn(rescale * r));
+    const float b = __half2float(__float2half_rn((1.f - rescale) * eps));
+    euler_inpaint_elem(base + e, __half2float(__float2half_rn(a + b)), sigma, sigma_next, den_next, ia, per_image, total,
+                       cfg, latents, model_in);
+  }
+}
+
 __global__ void step_inc_kernel(int* step) {
   pdl_launch_dependents();
   pdl_wait();
@@ -853,6 +975,28 @@ extern "C" int ih_euler_step_ex(const void* noise_pred, void* latents, void* mod
   IH_CUDA(launch_kernel(euler_ex_kernel, dim3(n_images), dim3(1024), (size_t)(0), stream, (const __half*)noise_pred,
                         (__half*)latents, (__half*)model_in, (const float*)sigmas, (const int*)step, guidance,
                         guidance_rescale, n_per_image, n_images, use_cfg ? 1 : 0));
+  IH_CUDA(launch_kernel(step_inc_kernel, dim3(1), dim3(1), (size_t)(0), stream, (int*)step));
+  return 0;
+}
+
+extern "C" int ih_euler_inpaint_step(const void* noise_pred, void* latents, void* model_in, const void* sigmas, void* step,
+                                     float guidance, float guidance_rescale, long long n_per_image, int n_images,
+                                     int use_cfg, const void* image_latents, const void* noise, const void* mask,
+                                     const void* blend_end, void* stream_) {
+  cudaStream_t stream = (cudaStream_t)stream_;
+  IH_CHECK(noise_pred && latents && model_in && sigmas && step && image_latents && noise && mask && blend_end, IH_ERR_ARG,
+           "ih_euler_inpaint_step: null pointer");
+  IH_CHECK(n_per_image > 1 && n_per_image % 4 == 0 && n_images > 0, IH_ERR_SHAPE,
+           "ih_euler_inpaint_step: n_per_image=%lld must be 4 latent channels x pixels", n_per_image);
+  IH_CHECK(guidance_rescale >= 0.f && guidance_rescale <= 1.f, IH_ERR_ARG,
+           "ih_euler_inpaint_step: guidance_rescale outside [0, 1]");
+  const int cfg = use_cfg ? 1 : 0;
+  const bool per_image = cfg && guidance_rescale > 0.f;
+  const long long total = n_per_image * n_images;
+  IH_CUDA(launch_kernel(euler_inpaint_kernel, dim3(per_image ? n_images : grid_for(total, 256)), dim3(per_image ? 1024 : 256),
+                        (size_t)(0), stream, (const __half*)noise_pred, (__half*)latents, (__half*)model_in,
+                        (const float*)sigmas, (const int*)step, guidance, guidance_rescale, n_per_image, n_images, cfg,
+                        (const __half*)image_latents, (const __half*)noise, (const __half*)mask, (const int*)blend_end));
   IH_CUDA(launch_kernel(step_inc_kernel, dim3(1), dim3(1), (size_t)(0), stream, (int*)step));
   return 0;
 }

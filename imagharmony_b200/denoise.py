@@ -11,10 +11,11 @@ not the graph): classifier-free guidance on or off (`guidance_scale <= 1`, :223,
 `control_guidance_start/end` IP-scale gating (:326-329), negative micro-conditioning time ids (:286-300).
 
 Graph lifetime: a captured graph holds raw pointers.  Everything it reads lives in buffers that are owned per shape
-and never freed while the graph exists -- the engine's static inputs (`_static`), the processors' K/V buffers and the
-UNet's add-embedding buffer (per-shape dicts inside those objects), and the library's grow-only scratch buffers whose
-re-allocation bumps `ops.workspace_generation()`.  A graph is replayed only if it was captured under the current UNet
-`graph_epoch` (weights / processors unchanged) and the current workspace generation; otherwise it is re-captured.
+and never freed while the graph exists -- the engine's static inputs (`_static`, `_inpaint_static`), the processors'
+K/V buffers and the UNet's add-embedding buffer (per-shape dicts inside those objects), and the library's grow-only
+scratch buffers whose re-allocation bumps `ops.workspace_generation()`.  A graph is replayed only if it was captured
+under the current UNet `graph_epoch` (weights / processors unchanged) and the current workspace generation; otherwise
+it is re-captured.
 """
 from __future__ import annotations
 
@@ -37,6 +38,7 @@ class DenoiseEngine:
         self.use_cuda_graph = use_cuda_graph and self.device.type == "cuda"
         self._graphs: Dict[Tuple, Tuple[torch.cuda.CUDAGraph, int]] = {}   # key -> (graph, workspace generation)
         self._static: Dict[Tuple, dict] = {}
+        self._inpaint_static: Dict[Tuple, dict] = {}
         self._tables: Dict[int, Tuple[torch.Tensor, torch.Tensor, float]] = {}
         self._epoch = getattr(unet, "graph_epoch", 0)
         self.last_launches_per_step = 0
@@ -79,10 +81,28 @@ class DenoiseEngine:
             self._static[key] = st
         return st
 
-    def _step(self, st, timesteps, sigmas, guidance, use_cfg=True, rescale=0.0):
+    def _inpaint_buffers(self, n: int, h: int, w: int):
+        """Static inputs of the inpainting step, per (n, h, w) and never freed (the graph-lifetime rule above)."""
+        key = (n, h, w)
+        ib = self._inpaint_static.get(key)
+        if ib is None:
+            dev = self.device
+            ib = {"image_latents": torch.empty((n, 4, h, w), dtype=torch.float16, device=dev),
+                  "noise": torch.empty((n, 4, h, w), dtype=torch.float16, device=dev),
+                  "mask": torch.empty((n, 1, h, w), dtype=torch.float16, device=dev),
+                  "blend_end": torch.zeros((1,), dtype=torch.int32, device=dev)}
+            self._inpaint_static[key] = ib
+        return ib
+
+    def _step(self, st, timesteps, sigmas, guidance, use_cfg=True, rescale=0.0, ib=None):
         noise = self.unet(st["model_in"], timesteps, st["ehs"], st["text_embeds"], st["time_ids"], step=st["step"])
-        ops.euler_step(noise, st["latents"], st["model_in"], sigmas, st["step"], guidance, use_cfg=use_cfg,
-                       guidance_rescale=rescale)
+        if ib is None:
+            ops.euler_step(noise, st["latents"], st["model_in"], sigmas, st["step"], guidance, use_cfg=use_cfg,
+                           guidance_rescale=rescale)
+        else:
+            ops.euler_inpaint_step(noise, st["latents"], st["model_in"], sigmas, st["step"], guidance,
+                                   ib["image_latents"], ib["noise"], ib["mask"], ib["blend_end"], use_cfg=use_cfg,
+                                   guidance_rescale=rescale)
 
     # ------------------------------------------------------------------------------------------------------------
     @torch.no_grad()
@@ -92,7 +112,8 @@ class DenoiseEngine:
             control_guidance_start: float = 0.0, control_guidance_end: float = 1.0, stop_after: Optional[int] = None,
             start_step: int = 0, guidance_rescale: float = 0.0, num_loop_steps: Optional[int] = None,
             callback: Optional[Callable] = None, callback_steps: int = 1,
-            negative_time_ids: Optional[torch.Tensor] = None, begin_step: int = 0) -> torch.Tensor:
+            negative_time_ids: Optional[torch.Tensor] = None, begin_step: int = 0,
+            inpaint: Optional[Tuple[torch.Tensor, torch.Tensor, torch.Tensor]] = None) -> torch.Tensor:
         """latents [n,4,h,w] (already scaled by init_noise_sigma; host or device); embeds host or device tensors.
         Returns the latents after the last executed step as a new device tensor.
 
@@ -106,7 +127,14 @@ class DenoiseEngine:
         entries [k, num_loop_steps) starting from `latents` that already carry the noise of sigma[k]; the device step
         counter starts at k, and the gating fractions and callback indices count from k, i.e. they see the truncated
         list.  It resumes nothing, so it cannot be combined with `start_step` / `stop_after` (IHError).  The step graphs
-        do not depend on k: image-to-image replays the text-to-image graphs of the same shape."""
+        do not depend on k: image-to-image replays the text-to-image graphs of the same shape.
+
+        `inpaint` = (image_latents [n,4,h,w], noise [n,4,h,w], mask [n,1,h,w]) is inpainting with a 4-channel UNet
+        ([3P] StableDiffusionXLInpaintPipeline): after every step the latents outside the mask are replaced by the
+        image latents re-noised to the next sigma, and by the clean image latents after the last step of the loop
+        (ops.euler_inpaint_step).  It composes with begin_step, num_loop_steps and the other loop options, not with
+        start_step / stop_after (IHError).  Its step graphs are captured once per shape next to the text-to-image
+        ones; the loop end is a device value, so they serve every num_loop_steps."""
         use_cfg = guidance_scale > 1.0                                            # :223
         if use_cfg and (negative_prompt_embeds is None or negative_pooled is None):
             raise IHError("classifier-free guidance needs negative_prompt_embeds / negative_pooled")
@@ -133,6 +161,16 @@ class DenoiseEngine:
             st["ehs"].copy_(prompt_embeds, non_blocking=True)
             st["text_embeds"].copy_(pooled, non_blocking=True)
             st["time_ids"].copy_(time_ids, non_blocking=True)
+        ib = None
+        if inpaint is not None:
+            if start_step or stop_after is not None:
+                raise IHError("inpaint cannot be combined with start_step / stop_after")
+            ib = self._inpaint_buffers(n, h, w)
+            for name, t in zip(("image_latents", "noise", "mask"), inpaint):
+                if tuple(t.shape) != tuple(ib[name].shape):
+                    raise IHError(f"inpaint {name}: expected shape {tuple(ib[name].shape)}, got {tuple(t.shape)}")
+                ib[name].copy_(t, non_blocking=True)
+            ib["blend_end"].fill_(loop_T)
         if not 0 <= start_step <= loop_T:
             raise IHError(f"start_step {start_step} outside the {loop_T}-step loop")
         if begin_step:
@@ -154,7 +192,7 @@ class DenoiseEngine:
             return 0.0 if off else float(ip_scale)
 
         def gkey(scale: float):
-            return (n, h, w, L, T, use_cfg, float(guidance_scale), rescale, scale)
+            return (n, h, w, L, T, use_cfg, float(guidance_scale), rescale, scale, ib is not None)
 
         if self.use_cuda_graph:
             if self._epoch != getattr(self.unet, "graph_epoch", 0):       # weights / processors changed since capture
@@ -169,7 +207,7 @@ class DenoiseEngine:
                     break
                 for sc in missing:
                     self.set_scale(sc)
-                    g = self._capture(st, timesteps, sigmas, guidance_scale, use_cfg, rescale)
+                    g = self._capture(st, timesteps, sigmas, guidance_scale, use_cfg, rescale, ib)
                     self._graphs[gkey(sc)] = (g, ops.workspace_generation())
                     captured = True
             else:
@@ -185,27 +223,27 @@ class DenoiseEngine:
                 self._graphs[gkey(sc)][0].replay()
             else:
                 self.set_scale(sc)
-                self._step(st, timesteps, sigmas, guidance_scale, use_cfg, rescale)
+                self._step(st, timesteps, sigmas, guidance_scale, use_cfg, rescale, ib)
             if callback is not None and (i - b0) % callback_steps == 0:           # :359-363 (Euler: order 1, no warm-up)
                 callback(i - b0, timesteps[i], st["latents"])
         self.set_scale(ip_scale)
         return st["latents"].clone()
 
-    def _capture(self, st, timesteps, sigmas, guidance, use_cfg=True, rescale=0.0):
+    def _capture(self, st, timesteps, sigmas, guidance, use_cfg=True, rescale=0.0, ib=None):
         # warm-up on a side stream (sets kernel attributes, fills the TMA descriptor cache, sizes the allocator and
         # the library's scratch buffers)
         side = torch.cuda.Stream(device=self.device)
         side.wait_stream(torch.cuda.current_stream())
         with torch.cuda.stream(side):
             st["step"].zero_()
-            self._step(st, timesteps, sigmas, guidance, use_cfg, rescale)
+            self._step(st, timesteps, sigmas, guidance, use_cfg, rescale, ib)
         torch.cuda.current_stream().wait_stream(side)
         torch.cuda.synchronize()
         st["step"].zero_()
         g = torch.cuda.CUDAGraph()
         before = ops.launch_count()
         with torch.cuda.graph(g):
-            self._step(st, timesteps, sigmas, guidance, use_cfg, rescale)
+            self._step(st, timesteps, sigmas, guidance, use_cfg, rescale, ib)
         self.last_launches_per_step = ops.launch_count() - before
         self.graphs_captured += 1
         return g

@@ -609,6 +609,33 @@ def euler_step(noise_pred: torch.Tensor, latents: torch.Tensor, model_in: torch.
                                _stream()), "ih_euler_step_ex")
 
 
+def euler_inpaint_step(noise_pred: torch.Tensor, latents: torch.Tensor, model_in: torch.Tensor, sigmas: torch.Tensor,
+                       step: torch.Tensor, guidance: float, image_latents: torch.Tensor, noise: torch.Tensor,
+                       mask: torch.Tensor, blend_end: torch.Tensor, *, use_cfg: bool = True,
+                       guidance_rescale: float = 0.0) -> None:
+    """euler_step followed by the inpainting blend (ih_euler_inpaint_step): outside `mask` the latents are replaced by
+    `image_latents` re-noised to the next sigma, or by the clean `image_latents` after the step that ends the loop at
+    schedule index `blend_end` (device int32).  image_latents / noise [n,4,h,w] and mask [n,1,h,w], fp16."""
+    lib = _lib.load()
+    _req(noise_pred, "noise_pred"); _req(latents, "latents"); _req(model_in, "model_in")
+    _req(sigmas, "sigmas", torch.float32); _req(step, "step", torch.int32)
+    _req(image_latents, "image_latents"); _req(noise, "noise"); _req(mask, "mask"); _req(blend_end, "blend_end", torch.int32)
+    n, c, h, w = latents.shape
+    per = latents.numel() // n
+    want = (2 * n if use_cfg else n) * per
+    if noise_pred.numel() != want or model_in.numel() != want:
+        raise IHError(f"euler_inpaint_step: noise_pred / model_in must hold {want} elements (use_cfg={use_cfg})")
+    if (c != 4 or tuple(image_latents.shape) != (n, 4, h, w) or tuple(noise.shape) != (n, 4, h, w)
+            or tuple(mask.shape) != (n, 1, h, w)
+            or not all(t.is_contiguous() for t in (latents, image_latents, noise, mask))):
+        raise IHError(f"euler_inpaint_step: contiguous latents / image_latents / noise [{n}, 4, {h}, {w}] and mask "
+                      f"[{n}, 1, {h}, {w}] required")
+    check(lib.ih_euler_inpaint_step(noise_pred.data_ptr(), latents.data_ptr(), model_in.data_ptr(), sigmas.data_ptr(),
+                                    step.data_ptr(), float(guidance), float(guidance_rescale), per, n, int(use_cfg),
+                                    image_latents.data_ptr(), noise.data_ptr(), mask.data_ptr(), blend_end.data_ptr(),
+                                    _stream()), "ih_euler_inpaint_step")
+
+
 def scale_model_input(latents: torch.Tensor, model_in: torch.Tensor, sigmas: torch.Tensor, step: torch.Tensor,
                       duplicate: bool = True) -> None:
     lib = _lib.load()

@@ -244,6 +244,20 @@ int ih_euler_step_ex(const void* noise_pred, void* latents, void* model_in, cons
                      float guidance, float guidance_rescale, long long n_per_image, int n_images, int use_cfg,
                      void* stream);
 
+/* Inpainting transition ([3P] diffusers StableDiffusionXLInpaintPipeline, 4-channel UNet): the transition of
+ * ih_euler_step_ex (same use_cfg / guidance_rescale options and rounding points), then, on the fp16 Euler result x of
+ * step i = *step, the blend with the image outside the mask before latents and model_in are written:
+ *   proper = fp16(img + fp16(noise * fp16(sigma[i+1])))  if i + 1 < *blend_end,  else img;
+ *   x <- fp16(fp16(fp16(1 - m) * proper) + fp16(m * x)),  m = mask[b, pixel] over the 4 channels;
+ *   model_in <- x / sqrt(sigma[i+1]^2 + 1) (duplicated with CFG); step counter i += 1.
+ * image_latents, noise: [n,4,H,W] fp16 (tiled to the batch), mask: [n,1,H,W] fp16, n_per_image = 4*H*W; blend_end:
+ * device int32, the absolute schedule index where the loop ends (read at every step, so one graph serves every
+ * denoising_end). */
+int ih_euler_inpaint_step(const void* noise_pred, void* latents, void* model_in, const void* sigmas, void* step,
+                          float guidance, float guidance_rescale, long long n_per_image, int n_images, int use_cfg,
+                          const void* image_latents, const void* noise, const void* mask, const void* blend_end,
+                          void* stream);
+
 /* model_in = cat([latents, latents]) / sqrt(sigma[*step]^2 + 1)   (custom_pipelines.py:332-334, first step). */
 int ih_scale_model_input(const void* latents, void* model_in, const void* sigmas, const void* step, long long total,
                          void* stream);

@@ -1,7 +1,8 @@
 """Drop-in import surface of the reference package (ip_adapter/__init__.py:1-11).  SD1.5-only classes
 (IPAdapter.generate, IPAdapterPlus, IPAdapterFull) are outside the SDXL hot path and are not provided."""
-from .custom_pipelines import StableDiffusionXLCustomPipeline, StableDiffusionXLImg2ImgPipeline
+from .custom_pipelines import (StableDiffusionXLCustomPipeline, StableDiffusionXLImg2ImgPipeline,
+                               StableDiffusionXLInpaintPipeline)
 from .ip_adapter import IPAdapter, IPAdapterPlusXL, IPAdapterXL
 
 __all__ = ["IPAdapter", "IPAdapterPlusXL", "IPAdapterXL", "StableDiffusionXLCustomPipeline",
-           "StableDiffusionXLImg2ImgPipeline"]
+           "StableDiffusionXLImg2ImgPipeline", "StableDiffusionXLInpaintPipeline"]

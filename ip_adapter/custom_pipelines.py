@@ -280,17 +280,20 @@ class StableDiffusionXLCustomPipeline:
         return StableDiffusionXLPipelineOutput(images=image)
 
 
-def preprocess_image(image, vae_scale_factor: int = 8) -> torch.Tensor:
+def preprocess_image(image, vae_scale_factor: int = 8, height: Optional[int] = None,
+                     width: Optional[int] = None) -> torch.Tensor:
     """[3P] diffusers VaeImageProcessor.preprocess (SDXL defaults: resize with Lanczos, normalise): PIL image(s) ->
     float32 [B, 3, H, W] in [-1, 1] with H, W floored to multiples of `vae_scale_factor` (every image takes the first
-    one's size).  A [B, 3, H, W] / [3, H, W] tensor is taken as it is, resized (nearest) when its size is not a multiple
-    of the factor; as in diffusers it is expected in [-1, 1], and one without negative values is taken as [0, 1] and
-    normalised."""
+    one's size), or the requested `height` x `width` when both are given.  A [B, 3, H, W] / [3, H, W] tensor is taken
+    as it is, resized (nearest) when its size is not a multiple of the factor or not the requested one; as in diffusers
+    it is expected in [-1, 1], and one without negative values is taken as [0, 1] and normalised."""
     import numpy as np
     from PIL import Image
     if isinstance(image, Image.Image) or (isinstance(image, (list, tuple)) and image and isinstance(image[0], Image.Image)):
         images = [image] if isinstance(image, Image.Image) else list(image)
         w, h = (x - x % vae_scale_factor for x in images[0].size)
+        if height is not None and width is not None:
+            h, w = height, width
         if w <= 0 or h <= 0:
             raise ValueError(f"image of size {images[0].size} is smaller than {vae_scale_factor} pixels")
         images = [im.convert("RGB") if im.mode != "RGB" else im for im in images]
@@ -303,6 +306,8 @@ def preprocess_image(image, vae_scale_factor: int = 8) -> torch.Tensor:
             raise ValueError(f"image tensor must be [B, 3, H, W] or [3, H, W], got {tuple(image.shape)}")
         x = x.float()
         h, w = (v - v % vae_scale_factor for v in x.shape[2:])
+        if height is not None and width is not None:
+            h, w = height, width
         if h <= 0 or w <= 0:
             raise ValueError(f"image of size {tuple(x.shape[2:])} is smaller than {vae_scale_factor} pixels")
         if (h, w) != tuple(x.shape[2:]):
@@ -441,13 +446,28 @@ class StableDiffusionXLImg2ImgPipeline(StableDiffusionXLCustomPipeline):
                              f"pipeline steps is {num_inference_steps - t_start} which is < 1 and not appropriate for "
                              "this pipeline.")
         lat = self.prepare_img2img_latents(pixels, batch, generator, self.scheduler.add_noise_sigma(t_start))
+        embeds = (prompt_embeds, negative_prompt_embeds, pooled_prompt_embeds, negative_pooled_prompt_embeds)
+        sizes = (original_size, crops_coords_top_left, target_size, negative_original_size,
+                 negative_crops_coords_top_left, negative_target_size)
+        out = self._denoise_from(lat, t_start, num_inference_steps, denoising_end, embeds, sizes, guidance_scale,
+                                 guidance_rescale, control_guidance_start, control_guidance_end, callback, callback_steps)
+        return self._output(out, output_type, return_dict)
+
+    def _denoise_from(self, lat, t_start: int, num_inference_steps: int, denoising_end, embeds, sizes, guidance_scale,
+                      guidance_rescale, control_guidance_start, control_guidance_end, callback, callback_steps,
+                      inpaint=None) -> torch.Tensor:
+        """The loop over timesteps[t_start:], truncated by denoising_end, from the noised start latents `lat`; the
+        micro-conditioning time ids are formed from `sizes` (requires_aesthetics_score = False). -> final latents."""
+        batch = embeds[0].shape[0]
+        original_size, crops_coords_top_left, target_size, neg_original_size, neg_crops_coords_top_left, \
+            neg_target_size = sizes
 
         def time_ids(size, crop, target):
             return torch.tensor([list(size) + list(crop) + list(target)], dtype=torch.float32).repeat(batch, 1)
         add_time_ids = time_ids(original_size, crops_coords_top_left, target_size)
         negative_add_time_ids = None
-        if negative_original_size is not None and negative_target_size is not None:
-            negative_add_time_ids = time_ids(negative_original_size, negative_crops_coords_top_left, negative_target_size)
+        if neg_original_size is not None and neg_target_size is not None:
+            negative_add_time_ids = time_ids(neg_original_size, neg_crops_coords_top_left, neg_target_size)
         loop_end = num_inference_steps
         if denoising_end is not None and isinstance(denoising_end, float) and 0 < denoising_end < 1:
             n_train = self.scheduler.num_train_timesteps
@@ -459,14 +479,157 @@ class StableDiffusionXLImg2ImgPipeline(StableDiffusionXLCustomPipeline):
                 conditioning_scale = attn_processor.scale
                 break
         if loop_end > t_start:
-            out = self.engine.run(lat, prompt_embeds, negative_prompt_embeds, pooled_prompt_embeds,
-                                  negative_pooled_prompt_embeds, add_time_ids, num_inference_steps,
+            out = self.engine.run(lat, *embeds, add_time_ids, num_inference_steps,
                                   guidance_scale=guidance_scale, ip_scale=conditioning_scale,
                                   control_guidance_start=control_guidance_start,
                                   control_guidance_end=control_guidance_end, guidance_rescale=guidance_rescale,
                                   num_loop_steps=loop_end, callback=callback, callback_steps=callback_steps,
-                                  negative_time_ids=negative_add_time_ids, begin_step=t_start)
+                                  negative_time_ids=negative_add_time_ids, begin_step=t_start, inpaint=inpaint)
         else:
             out = lat
         self.set_scale(conditioning_scale)
+        return out
+
+
+def preprocess_mask(mask, height: int, width: int) -> torch.Tensor:
+    """[3P] diffusers VaeImageProcessor(do_normalize=False, do_binarize=True, do_convert_grayscale=True).preprocess:
+    PIL mask(s) are converted to "L", resized to width x height with Lanczos and divided by 255; a [B, 1, H, W],
+    [B, H, W] or [H, W] tensor in [0, 1] is resized with nearest interpolation.  Then binarized (< 0.5 -> 0, else 1).
+    -> float32 [B, 1, height, width]."""
+    import numpy as np
+    from PIL import Image
+    if isinstance(mask, Image.Image) or (isinstance(mask, (list, tuple)) and mask and isinstance(mask[0], Image.Image)):
+        masks = [mask] if isinstance(mask, Image.Image) else list(mask)
+        masks = [m.convert("L").resize((width, height), resample=Image.LANCZOS) for m in masks]
+        x = torch.from_numpy(np.stack([np.array(m).astype(np.float32) / 255.0 for m in masks]))[:, None]
+    elif isinstance(mask, torch.Tensor):
+        x = mask.float()
+        if x.dim() == 2:
+            x = x[None, None]
+        elif x.dim() == 3:
+            x = x[:, None]
+        if x.dim() != 4 or x.shape[1] != 1:
+            raise ValueError(f"mask tensor must be [B, 1, H, W], [B, H, W] or [H, W], got {tuple(mask.shape)}")
+        x = torch.nn.functional.interpolate(x, size=(height, width))
+    else:
+        raise ValueError(f"`mask_image` must be a PIL image, a list of them or a tensor, got {type(mask).__name__}")
+    return (x >= 0.5).float().contiguous()
+
+
+class StableDiffusionXLInpaintPipeline(StableDiffusionXLImg2ImgPipeline):
+    """Inpainting with the call surface of [3P] diffusers `StableDiffusionXLInpaintPipeline` over the 4-channel SDXL-base
+    UNet, so that `IPAdapterXL(inpaint_pipe, ...).generate(pil_image=..., image=init, mask_image=mask, strength=s)`
+    works as it does on the reference built over that pipeline.  The region where the mask is 1 is regenerated; after
+    every step the rest is replaced by the image latents re-noised to the next sigma (the clean latents after the last
+    step), fused into the step kernel (ops.euler_inpaint_step, DenoiseEngine.run(inpaint=...)).
+
+    Differences from image-to-image follow diffusers: defaults strength = 0.9999 (the first step is skipped) and
+    guidance_scale = 7.5; height / width default to the UNet's sample size x 8, not to the image's size, and the image
+    and the mask are resized to them.  Image and mask batches are tiled to the prompt batch with `repeat` (slot b gets
+    image b % n_images and mask b % n_masks); with a list of generators only the first n_images encode (SURVEY C.19).
+    The 9-channel inpainting UNet and `padding_mask_crop` are not implemented and raise IHError."""
+
+    UNSUPPORTED = StableDiffusionXLImg2ImgPipeline.UNSUPPORTED + ("masked_image_latents",)
+
+    def prepare_inpaint_latents(self, image: torch.Tensor, batch_size: int, generator, t_start: int,
+                                is_strength_max: bool) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+        """[3P] StableDiffusionXLInpaintPipeline.prepare_latents (return_image_latents, fp16 latents) ->
+        (start latents, clean image latents, noise), each [batch_size, 4, h, w] fp16 on the device.  The posterior
+        kernel runs twice: with sigma 0 and zero noise it returns the clean latents exactly (fp16(zs + 0) = zs), with the
+        noise and sigma[t_start] the start latents (add_noise); at strength 1 the start is noise * init_noise_sigma."""
+        venc = self.vae_encoder
+        n_img = image.shape[0]
+        if batch_size % n_img:
+            raise ValueError(f"cannot duplicate an image batch of {n_img} to a prompt batch of {batch_size}")
+        moments = venc.encode_moments_nhwc(image.to(self.device, torch.float16))      # [n_img, h, w, 16]
+        L = venc.config.latent_channels
+        h, w = moments.shape[1], moments.shape[2]
+        eps_dtype = torch.float32 if getattr(venc.config, "force_upcast", True) else torch.float16
+
+        def draw(shape, g, dtype):
+            return torch.randn(shape, generator=g, device=g.device if g is not None else "cpu", dtype=dtype)
+        if isinstance(generator, list):
+            if len(generator) != batch_size:
+                raise ValueError(f"got {len(generator)} generators for a batch of {batch_size}")
+            # _encode_vae_image samples the n_img images with generator[i] before the batch is tiled
+            eps = torch.cat([draw((1, L, h, w), g, eps_dtype).to(self.device) for g in generator[:n_img]])
+            noise = torch.cat([draw((1, L, h, w), g, torch.float16).to(self.device) for g in generator])
+        else:
+            eps = draw((n_img, L, h, w), generator, eps_dtype).to(self.device)
+            noise = draw((batch_size, L, h, w), generator, torch.float16).to(self.device)
+        eps, noise = eps.contiguous(), noise.contiguous()
+        sf = venc.config.scaling_factor
+        image_latents = ops.vae_posterior_noise(moments, eps, torch.zeros_like(noise), L, sf, 0.0)
+        if is_strength_max:
+            latents = (noise.float() * self.scheduler.init_noise_sigma).half()
+        else:
+            latents = ops.vae_posterior_noise(moments, eps, noise, L, sf, self.scheduler.add_noise_sigma(t_start))
+        return latents, image_latents, noise
+
+    @torch.no_grad()
+    def __call__(self, prompt: Optional[Union[str, List[str]]] = None, prompt_2=None, image=None, mask_image=None,
+                 height: Optional[int] = None, width: Optional[int] = None, padding_mask_crop: Optional[int] = None,
+                 strength: float = 0.9999, num_inference_steps: int = 50, denoising_end: Optional[float] = None,
+                 guidance_scale: float = 7.5, negative_prompt=None, negative_prompt_2=None,
+                 num_images_per_prompt: Optional[int] = 1, eta: float = 0.0, generator=None,
+                 prompt_embeds: Optional[torch.Tensor] = None, negative_prompt_embeds: Optional[torch.Tensor] = None,
+                 pooled_prompt_embeds: Optional[torch.Tensor] = None,
+                 negative_pooled_prompt_embeds: Optional[torch.Tensor] = None, output_type: Optional[str] = "pil",
+                 return_dict: bool = True, callback=None, callback_steps: int = 1,
+                 cross_attention_kwargs: Optional[Dict[str, Any]] = None, guidance_rescale: float = 0.0,
+                 original_size: Optional[Tuple[int, int]] = None, crops_coords_top_left: Tuple[int, int] = (0, 0),
+                 target_size: Optional[Tuple[int, int]] = None, negative_original_size=None,
+                 negative_crops_coords_top_left=(0, 0), negative_target_size=None, aesthetic_score: float = 6.0,
+                 negative_aesthetic_score: float = 2.5, control_guidance_start: float = 0.0,
+                 control_guidance_end: float = 1.0, **kwargs):
+        """The image-to-image parameter list plus `mask_image` (PIL image(s) or a tensor in [0, 1]; 1 = regenerate),
+        `height`, `width` and `padding_mask_crop`.  Unknown keywords are ignored, except the diffusers arguments in
+        UNSUPPORTED and a `padding_mask_crop`, which raise IHError."""
+        refused = [k for k in self.UNSUPPORTED if kwargs.get(k) is not None]
+        if padding_mask_crop is not None:
+            refused.append("padding_mask_crop")
+        if refused:
+            raise IHError(f"StableDiffusionXLInpaintPipeline does not implement {refused}")
+        if self.unet.config.in_channels != 4:
+            raise IHError(f"StableDiffusionXLInpaintPipeline supports the 4-channel UNet only (this one has "
+                          f"{self.unet.config.in_channels} input channels)")
+        if not 0.0 <= strength <= 1.0:
+            raise ValueError(f"The value of strength should in [0.0, 1.0] but is {strength}")          # [3P] check_inputs
+        height = height or self.default_sample_size * self.vae_scale_factor
+        width = width or self.default_sample_size * self.vae_scale_factor
+        if height % 8 != 0 or width % 8 != 0:
+            raise ValueError(f"`height` and `width` have to be divisible by 8 but are {height} and {width}.")
+        if callback is not None and (not isinstance(callback_steps, int) or callback_steps <= 0):
+            raise ValueError(f"`callback_steps` has to be a positive integer but is {callback_steps}")
+        if image is None or mask_image is None:
+            raise ValueError("`image` and `mask_image` inputs cannot be undefined")
+        if self.vae_encoder is None:
+            raise IHError("this pipeline has no VAE encoder: build it with from_random(vae_cfg=...) or from_pretrained "
+                          "with a vae/ folder")
+        pixels = preprocess_image(image, self.vae_scale_factor, height, width)
+        mask = preprocess_mask(mask_image, height, width)
+        do_classifier_free_guidance = guidance_scale > 1.0
+        embeds = self.encode_prompt(prompt, prompt_2, None, num_images_per_prompt, do_classifier_free_guidance,
+                                    negative_prompt, negative_prompt_2, prompt_embeds, negative_prompt_embeds,
+                                    pooled_prompt_embeds, negative_pooled_prompt_embeds)
+        batch = embeds[0].shape[0]
+        self.scheduler.set_timesteps(num_inference_steps)
+        t_start = self.scheduler.img2img_begin_index(num_inference_steps, strength)
+        if num_inference_steps - t_start < 1:
+            raise ValueError(f"After adjusting the num_inference_steps by strength parameter: {strength}, the number of "
+                             f"pipeline steps is {num_inference_steps - t_start} which is < 1 and not appropriate for "
+                             "this pipeline.")
+        lat, image_latents, noise = self.prepare_inpaint_latents(pixels, batch, generator, t_start, strength == 1.0)
+        # the masked image's latents only feed a 9-channel UNet: with 4 channels diffusers encodes them unused.  That
+        # encode is skipped; its posterior draw comes after the noise, so no result of this call changes
+        mask_lat = torch.nn.functional.interpolate(mask, size=(height // self.vae_scale_factor,
+                                                               width // self.vae_scale_factor)).half()
+        if batch % mask_lat.shape[0]:
+            raise ValueError(f"cannot duplicate a mask batch of {mask_lat.shape[0]} to a prompt batch of {batch}")
+        mask_lat = mask_lat.repeat(batch // mask_lat.shape[0], 1, 1, 1).to(self.device)
+        sizes = (original_size or (height, width), crops_coords_top_left, target_size or (height, width),
+                 negative_original_size, negative_crops_coords_top_left, negative_target_size)
+        out = self._denoise_from(lat, t_start, num_inference_steps, denoising_end, embeds, sizes, guidance_scale,
+                                 guidance_rescale, control_guidance_start, control_guidance_end, callback, callback_steps,
+                                 inpaint=(image_latents, noise, mask_lat))
         return self._output(out, output_type, return_dict)
