@@ -65,9 +65,10 @@ struct GemmParams {
   // producer warp issues cp.async.bulk.prefetch.L2 for this CTA's slice while the main loop runs.
   const unsigned char* pf_ptr;
   unsigned long long pf_bytes;
-  // LayerNorm folding (plain GEMM mode only).  A producer GEMM writes, per output row and 64-column slab, the sum and
-  // the sum of squares of the fp16-rounded values it stores (stats_out [ceil(N/64), M, 2] fp32, one writer per slot:
-  // deterministic, nothing to zero).  The consumer GEMM multiplies the RAW rows with gamma-scaled, row-CENTRED weights
+  // LayerNorm folding (plain GEMM mode only).  A producer GEMM writes, per output row, the sum and the sum of squares
+  // of the fp16-rounded values it stores as partial sums whose total over slots is the row's (stats_out
+  // [ceil(N/64), M, 2] fp32, one writer per slot, every slot written: deterministic, nothing to zero).  The consumer
+  // GEMM multiplies the RAW rows with gamma-scaled, row-CENTRED weights
   // Wc[n,k] = W[n,k] gamma[k] - mean_k(W[n,:] gamma) -- so x Wc^T = (x - mean(x)) (W gamma)^T -- and applies
   //   out = rstd[m] * acc + c[n],  c = W beta + b (passed as `bias`)   (= LayerNorm(x) W^T + b in real arithmetic)
   // with rstd rebuilt from the producer's slabs (ln_stats [ln_slabs, M, 2]).
@@ -87,12 +88,16 @@ struct GemmSmem {
   static constexpr int BN_OUT = GEGLU ? BN / 2 : BN;
   static constexpr int SLABS = (BN_OUT + 63) / 64;   // 64-column output slabs per tile
   static constexpr int SLAB_BYTES = BM * 64 * 2;     // one 128-row x 64-column fp16 staging slab (TMA store source)
+  // BN_OUT = 64 k + 32 (the 160-column tile): the last slab is 32 columns wide, staged with 64-byte rows and stored
+  // through the 32-column tensor maps, so that it never writes the next tile's columns
+  static constexpr bool NARROW_LAST = (BN_OUT % 64) == 32;
+  static constexpr int ALL_SLAB_BYTES = SLABS * SLAB_BYTES - (NARROW_LAST ? SLAB_BYTES / 2 : 0);
   static constexpr int BAR_BYTES = 256;
   static constexpr int SMEM_LIMIT = 232448;          // 227 KiB per CTA
   // one staging slab per output slab when that fits (no buffer reuse inside a tile), else two (ping-pong)
   static constexpr int STG_SLABS =
-      (TILE_BYTES + SLABS * SLAB_BYTES + BAR_BYTES + 1024 <= SMEM_LIMIT) ? SLABS : (SLABS < 2 ? SLABS : 2);
-  static constexpr int STG_BYTES = STG_SLABS * SLAB_BYTES;
+      (TILE_BYTES + ALL_SLAB_BYTES + BAR_BYTES + 1024 <= SMEM_LIMIT) ? SLABS : (SLABS < 2 ? SLABS : 2);
+  static constexpr int STG_BYTES = STG_SLABS == SLABS ? ALL_SLAB_BYTES : STG_SLABS * SLAB_BYTES;
   static constexpr int TOTAL = TILE_BYTES + STG_BYTES + BAR_BYTES + 1024;  // + alignment slack
   static_assert(TOTAL <= SMEM_LIMIT, "GEMM shared-memory budget exceeded");
   static_assert(STG_SLABS <= 4, "residual barriers");
@@ -108,6 +113,8 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_f16_kernel(const __grid_
                                                                     const __grid_constant__ CUtensorMap bmap,
                                                                     const __grid_constant__ CUtensorMap omap,
                                                                     const __grid_constant__ CUtensorMap rmap,
+                                                                    const __grid_constant__ CUtensorMap omap32,
+                                                                    const __grid_constant__ CUtensorMap rmap32,
                                                                     const GemmParams p) {
   using S = GemmSmem<BN, STAGES, GEGLU>;
   extern __shared__ uint8_t smem_raw[];
@@ -135,6 +142,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_f16_kernel(const __grid_
     tma_prefetch_desc(&amaps.m[0]);
     tma_prefetch_desc(&bmap);
     tma_prefetch_desc(&omap);
+    if (S::NARROW_LAST) tma_prefetch_desc(&omap32);
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full_bar[s], 1);
       mbar_init(&empty_bar[s], GEMM_MMA_THREADS / 32);   // lane 0 of every MMA warp
@@ -227,6 +235,20 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_f16_kernel(const __grid_
     int stage = 0;
     uint32_t phase = 0;
     float acc[BN / 2];
+    // slab sl of the tile: 64 columns in a 128 B-row staging buffer, or (the last slab of a 160-column tile) 32
+    // columns in 64 B rows, fetched and stored through the 32-column tensor maps
+    auto narrow = [](int sl) { return S::NARROW_LAST && sl == SLABS - 1; };
+    auto load_residual = [&](int sl, uint8_t* dst, uint64_t* bar, int col0, int m_tile, int x0, int y0, int img) {
+      const CUtensorMap* m = narrow(sl) ? &rmap32 : &rmap;
+      mbar_arrive_expect_tx(bar, narrow(sl) ? BM * 64 : BM * 128);
+      if (p.mode == 0) tma_load_2d(dst, m, bar, col0, m_tile * BM);
+      else tma_load_4d(dst, m, bar, col0, x0, y0, img);
+    };
+    // byte offset of the 16-byte chunk c of row r inside a staging slab (the TMA swizzle of the slab's tensor map)
+    auto stg_off = [&](int sl, int r, int c) {
+      return narrow(sl) ? r * 64 + ((c ^ ((r >> 1) & 3)) << 4) : r * 128 + ((c ^ (r & 7)) << 4);
+    };
+    float carry_sum = 0.f, carry_sq = 0.f;            // row statistics of slab 0 of an odd 160-column tile
     int it = 0;
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
       const int n_tile = tile % n_tiles;
@@ -243,12 +265,11 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_f16_kernel(const __grid_
       // residual slabs of the first NBUF slabs are fetched now, behind the main loop (the staging buffers are free:
       // the previous tile ended after its stores had read them)
       if (issuer && p.residual) {
+#pragma unroll
         for (int sl = 0; sl < SLABS && sl < NBUF; ++sl) {
           const int col0 = n0 + sl * 64;
           if (col0 >= p.N) break;
-          mbar_arrive_expect_tx(&res_bar[sl], BM * 128);
-          if (p.mode == 0) tma_load_2d(stg + sl * S::SLAB_BYTES, &rmap, &res_bar[sl], col0, m_tile * BM);
-          else tma_load_4d(stg + sl * S::SLAB_BYTES, &rmap, &res_bar[sl], col0, x0, y0, img);
+          load_residual(sl, stg + sl * S::SLAB_BYTES, &res_bar[sl], col0, m_tile, x0, y0, img);
         }
       }
 
@@ -336,11 +357,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_f16_kernel(const __grid_
             // is fetched into it
             if (issuer) {
               tma_store_wait_read<(NBUF > 1 ? NBUF - 1 : 0)>();
-              if (p.residual) {
-                mbar_arrive_expect_tx(&res_bar[buf], BM * 128);
-                if (p.mode == 0) tma_load_2d(sbuf, &rmap, &res_bar[buf], col0, m_tile * BM);
-                else tma_load_4d(sbuf, &rmap, &res_bar[buf], col0, x0, y0, img);
-              }
+              if (p.residual) load_residual(sl, sbuf, &res_bar[buf], col0, m_tile, x0, y0, img);
             }
             named_bar_sync(1, GEMM_MMA_THREADS);
           }
@@ -349,7 +366,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_f16_kernel(const __grid_
             res_par ^= 1u << buf;
           }
 #pragma unroll
-          for (int j = 0; j < 8; ++j) {
+          for (int j = 0; j < (narrow(sl) ? 4 : 8); ++j) {
             const int i = sl * 8 + j;                // accumulator 8-column group (GEGLU: value half)
             const int lc = sl * 64 + j * 8 + cq;     // tile-local output column of my pair
             const int col = n0 + lc;
@@ -384,7 +401,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_f16_kernel(const __grid_
                 x0v = __fdividef(x0v, 1.f + __expf(-1.702f * x0v));
                 x1v = __fdividef(x1v, 1.f + __expf(-1.702f * x1v));
               }
-              uint32_t* slot = reinterpret_cast<uint32_t*>(sbuf + r * 128 + ((j ^ (r & 7)) << 4) + cq * 2);
+              uint32_t* slot = reinterpret_cast<uint32_t*>(sbuf + stg_off(sl, r, j) + cq * 2);
               if (p.residual) {
                 const float2 f = unpack_half2(*slot);
                 x0v += f.x;
@@ -396,22 +413,25 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_f16_kernel(const __grid_
           fence_proxy_async_smem();
           named_bar_sync(2, GEMM_MMA_THREADS);      // the slab is complete in shared memory
           if (issuer) {
-            if (p.mode == 0) tma_store_2d(&omap, sbuf, col0, m_tile * BM);
-            else tma_store_4d(&omap, sbuf, col0, x0, y0, img);
+            const CUtensorMap* m = narrow(sl) ? &omap32 : &omap;
+            if (p.mode == 0) tma_store_2d(m, sbuf, col0, m_tile * BM);
+            else tma_store_4d(m, sbuf, col0, x0, y0, img);
             tma_store_commit();
           }
           // row statistics of exactly the fp16 values a later LayerNorm would read: one warpgroup per slab, one row
-          // per thread, re-read from the staging buffer; one writer per (slab, row) slot
+          // per thread, re-read from the staging buffer; one writer per (slot, row).  Each slot holds a partial sum
+          // of the row's statistics and the total over all slots is the row's: 64-column tiles write slot col0 / 64; a pair
+          // of 160-column tiles covers the 5 slots of its 320 columns -- the even tile writes its three slabs into the
+          // first three, the odd tile its slabs 0 + 2 (96 columns) into the fourth and slab 1 into the fifth.
           if (p.stats_out && wg == (sl & 1)) {
             const int r = ct & 127;
             const long long srow = (long long)m_tile * BM + r;
             if (srow < p.M) {
-              const uint8_t* row_ptr = sbuf + r * 128;
               float st_sum = 0.f, st_sq = 0.f;
 #pragma unroll
-              for (int c = 0; c < 8; ++c) {
+              for (int c = 0; c < (narrow(sl) ? 4 : 8); ++c) {
                 if (col0 + c * 8 < p.N) {
-                  const uint4 o = *reinterpret_cast<const uint4*>(row_ptr + ((c ^ (r & 7)) << 4));
+                  const uint4 o = *reinterpret_cast<const uint4*>(sbuf + stg_off(sl, r, c));
                   const uint32_t ow[4] = {o.x, o.y, o.z, o.w};
 #pragma unroll
                   for (int e = 0; e < 4; ++e) {
@@ -421,7 +441,26 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_f16_kernel(const __grid_
                   }
                 }
               }
-              reinterpret_cast<float2*>(p.stats_out)[(long long)(col0 >> 6) * p.M + srow] = make_float2(st_sum, st_sq);
+              int slot = col0 >> 6;
+              bool write = true;
+              if (BN_OUT == 160) {
+                const int base = (n_tile >> 1) * 5;
+                if ((n_tile & 1) == 0) {
+                  slot = base + sl;
+                } else if (sl == 0) {
+                  carry_sum = st_sum;
+                  carry_sq = st_sq;
+                  write = false;
+                } else {
+                  slot = base + (sl == 1 ? 4 : 3);
+                  if (sl == 2) {
+                    st_sum += carry_sum;
+                    st_sq += carry_sq;
+                  }
+                }
+              }
+              if (write)
+                reinterpret_cast<float2*>(p.stats_out)[(long long)slot * p.M + srow] = make_float2(st_sum, st_sq);
             }
           }
         }
@@ -439,9 +478,39 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_f16_kernel(const __grid_
 // ------------------------------------------------------------------------------------------------
 // host side
 // ------------------------------------------------------------------------------------------------
+// The output (and residual) tensor as the epilogue's TMA stores and loads see it: 64-column slabs with a 128-byte
+// swizzle, and, for the 160-column tile, its 32-column last slab with a 64-byte swizzle.
+struct OutMaps {
+  CUtensorMap o, r, o32, r32;
+};
+struct OutView {
+  void* out;
+  const void* residual;
+  int rank;
+  uint64_t dims[4];
+  uint64_t ostr[3], rstr[3];
+  uint32_t box[4];   // box[0] (the column count) is set per slab width
+};
+
+static int out_maps(const OutView& v, bool narrow_slab, OutMaps& m) {
+  uint32_t box[4] = {64u, v.box[1], v.box[2], v.box[3]};
+  int rc = get_tmap_f16(&m.o, v.out, v.rank, v.dims, v.ostr, box);
+  if (rc) return rc;
+  m.r = m.o;
+  if (v.residual && (rc = get_tmap_f16(&m.r, v.residual, v.rank, v.dims, v.rstr, box))) return rc;
+  m.o32 = m.o;
+  m.r32 = m.r;
+  if (narrow_slab) {
+    box[0] = 32u;
+    if ((rc = get_tmap_f16(&m.o32, v.out, v.rank, v.dims, v.ostr, box, 64))) return rc;
+    if (v.residual && (rc = get_tmap_f16(&m.r32, v.residual, v.rank, v.dims, v.rstr, box, 64))) return rc;
+  }
+  return 0;
+}
+
 template <int BN, int STAGES, bool GEGLU>
-static int launch_gemm(const TmapSet4& amaps, const CUtensorMap& bmap, const CUtensorMap& omap,
-                       const CUtensorMap& rmap, GemmParams& p, int m_tiles, cudaStream_t stream) {
+static int launch_gemm(const TmapSet4& amaps, const CUtensorMap& bmap, const OutMaps& om, GemmParams& p, int m_tiles,
+                       cudaStream_t stream) {
   using S = GemmSmem<BN, STAGES, GEGLU>;
   static bool configured = false;
   auto kern = gemm_f16_kernel<BN, STAGES, GEGLU>;
@@ -454,15 +523,16 @@ static int launch_gemm(const TmapSet4& amaps, const CUtensorMap& bmap, const CUt
   const long long n_tiles = (p.N + BN_OUT - 1) / BN_OUT;
   const long long tiles = n_tiles * m_tiles;
   const int grid = (int)(tiles < num_sms() ? tiles : num_sms());
-  IH_CUDA(launch_kernel(kern, dim3(grid), dim3(GEMM_THREADS), (size_t)(S::TOTAL), stream, amaps, bmap, omap, rmap, p));
+  IH_CUDA(launch_kernel(kern, dim3(grid), dim3(GEMM_THREADS), (size_t)(S::TOTAL), stream, amaps, bmap, om.o, om.r,
+                        om.o32, om.r32, p));
   return 0;
 }
 
-// Cost model for the persistent kernel (one CTA per SM): the main loop streams A + B operand bytes through L2 per
-// 64-deep k-block -- 48 KiB for a 128x256 tile, 40 KiB for 128x192, 32 KiB for 128x128 -- so the per-tile cost is
-// taken proportional to those bytes (a model, not a measurement), plus a fixed per-round epilogue cost.  Padded
-// columns of a partially filled last N tile cost as much as real ones.
-static int pick_bn(long long m_tiles, int N) {
+// Cost model for the persistent kernel (one CTA per SM): a launch takes `rounds` tiles per SM one after the other,
+// each costing num_kb k-blocks of main loop plus a fixed part (pipeline fill, epilogue, store drain).  Padded columns of
+// a partially filled last N tile cost as much as real ones.  160-column tiles need N % 320 == 0 when the launch writes
+// row statistics (see the epilogue).
+static int pick_bn(long long m_tiles, int N, int num_kb, bool allow160) {
   if (N <= 64) return 64;
   const int sms = num_sms();
   // 128x64 tiles for launches that cannot fill the SMs with wider ones (e.g. the 1280-channel level of a 512^2 edit,
@@ -472,15 +542,22 @@ static int pick_bn(long long m_tiles, int N) {
     return e ? atoi(e) : 1;
   }();
   if (bn64 && m_tiles * ((N + 63) / 64) <= sms) return 64;
+  // Measured with tools/ab_probe.py tile (M = 2048, 128 tiles in one round, K = 1280 vs 5120) on an NVIDIA H100 80GB
+  // HBM3 at a 400 W power limit: per k-block 0.583 / 0.706 / 0.877 / 1.161 us and fixed 3.3 / 3.7 / 3.9 / 8.8 us for
+  // the 128 / 160 / 192 / 256-column tiles, here in units of the 128-column tile's k-block.  The main loop is
+  // MMA-bound (cost ~ BN), not L2-bound; the 256-column tile's fixed part is larger because its epilogue ping-pongs
+  // two staging slabs.
   double best = 1e30;
   int best_bn = 256;
-  const int cands[3] = {256, 192, 128};
-  const double tile_cost[3] = {1.5, 1.25, 1.0};
-  for (int i = 0; i < 3; ++i) {
+  const int cands[4] = {256, 192, 160, 128};
+  const double kb_cost[4] = {1.99, 1.50, 1.21, 1.0};
+  const double fixed_cost[4] = {15.1, 6.7, 6.3, 5.7};
+  for (int i = 0; i < 4; ++i) {
     const int bn = cands[i];
+    if (bn == 160 && !allow160) continue;
     const long long tiles = m_tiles * ((N + bn - 1) / bn);
     const long long rounds = (tiles + sms - 1) / sms;
-    const double t = (double)rounds * (tile_cost[i] + 0.15);
+    const double t = (double)rounds * (kb_cost[i] * num_kb + fixed_cost[i]);
     if (t < best - 1e-9) {
       best = t;
       best_bn = bn;
@@ -489,25 +566,30 @@ static int pick_bn(long long m_tiles, int N) {
   return best_bn;
 }
 
-static int dispatch(const TmapSet4& amaps, const CUtensorMap& omap, const CUtensorMap& rmap, const void* w, int ldw_rows,
-                    long long K, GemmParams& p, int m_tiles, int geglu, int force_bn, cudaStream_t stream) {
-  // tile_n: 0 = the cost model's choice, 64 / 128 / 192 / 256 force that tile width; 512 and 384 (the widest tiles a
-  // caller may ask for) are the 256- and 192-column tiles
+static int dispatch(const TmapSet4& amaps, const OutView& ov, const void* w, int ldw_rows, long long K, GemmParams& p,
+                    int m_tiles, int geglu, int force_bn, cudaStream_t stream) {
+  // tile_n: 0 = the cost model's choice, 64 / 128 / 160 / 192 / 256 force that tile width; 512 and 384 (the widest
+  // tiles a caller may ask for) are the 256- and 192-column tiles
   if (force_bn == 512) force_bn = 256;
   if (force_bn == 384) force_bn = 192;
-  const int bn = geglu ? 256 : (force_bn > 0 ? force_bn : pick_bn(m_tiles, p.N));
+  const bool allow160 = !p.stats_out || p.N % 320 == 0;
+  const int bn = geglu ? 256 : (force_bn > 0 ? force_bn : pick_bn(m_tiles, p.N, p.num_kb, allow160));
+  IH_CHECK(bn != 160 || allow160, IH_ERR_SHAPE, "ih_gemm_ln_f16: 160-column tiles with stats_out need N %% 320 == 0");
   CUtensorMap bmap;
   const uint64_t bdims[2] = {(uint64_t)K, (uint64_t)ldw_rows};
   const uint64_t bstr[1] = {(uint64_t)K * 2};
   const uint32_t bbox[2] = {(uint32_t)BK, (uint32_t)(geglu ? 128 : bn)};
   int rc = get_tmap_f16(&bmap, w, 2, bdims, bstr, bbox);
   if (rc) return rc;
-  if (geglu) return launch_gemm<256, 4, true>(amaps, bmap, omap, rmap, p, m_tiles, stream);
+  OutMaps om;
+  if ((rc = out_maps(ov, !geglu && bn == 160, om))) return rc;
+  if (geglu) return launch_gemm<256, 4, true>(amaps, bmap, om, p, m_tiles, stream);
   switch (bn) {
-    case 256: return launch_gemm<256, 4, false>(amaps, bmap, omap, rmap, p, m_tiles, stream);
-    case 192: return launch_gemm<192, 4, false>(amaps, bmap, omap, rmap, p, m_tiles, stream);
-    case 128: return launch_gemm<128, 6, false>(amaps, bmap, omap, rmap, p, m_tiles, stream);
-    case 64: return launch_gemm<64, 8, false>(amaps, bmap, omap, rmap, p, m_tiles, stream);
+    case 256: return launch_gemm<256, 4, false>(amaps, bmap, om, p, m_tiles, stream);
+    case 192: return launch_gemm<192, 4, false>(amaps, bmap, om, p, m_tiles, stream);
+    case 160: return launch_gemm<160, 5, false>(amaps, bmap, om, p, m_tiles, stream);
+    case 128: return launch_gemm<128, 6, false>(amaps, bmap, om, p, m_tiles, stream);
+    case 64: return launch_gemm<64, 8, false>(amaps, bmap, om, p, m_tiles, stream);
     default: return set_error(IH_ERR_ARG, "unsupported BN %d", bn);
   }
 }
@@ -619,21 +701,9 @@ static int gemm_impl(const void* a, long long lda, const void* w, const void* bi
   p.ln_eps = ln_eps;
   p.alpha = alpha;
   const int m_tiles = (M + BM - 1) / BM;
-  CUtensorMap omap, rmap;
-  {
-    const uint64_t odims[2] = {(uint64_t)p.N, (uint64_t)M};
-    const uint32_t obox[2] = {64u, (uint32_t)BM};
-    const uint64_t ostr[1] = {(uint64_t)ldo * 2};
-    rc = get_tmap_f16(&omap, out, 2, odims, ostr, obox);
-    if (rc) return rc;
-    rmap = omap;
-    if (residual) {
-      const uint64_t rstr[1] = {(uint64_t)ldr * 2};
-      rc = get_tmap_f16(&rmap, residual, 2, odims, rstr, obox);
-      if (rc) return rc;
-    }
-  }
-  return dispatch(amaps, omap, rmap, w, N, K, p, m_tiles, geglu, tile_n, (cudaStream_t)stream);
+  const OutView ov{out, residual, 2, {(uint64_t)p.N, (uint64_t)M}, {(uint64_t)ldo * 2}, {(uint64_t)ldr * 2},
+                   {64u, (uint32_t)BM}};
+  return dispatch(amaps, ov, w, N, K, p, m_tiles, geglu, tile_n, (cudaStream_t)stream);
 }
 
 static int conv_impl(const void* x, const void* w, const void* bias, const void* rowbias, long long ld_rowbias,
@@ -775,18 +845,8 @@ static int conv_impl(const void* x, const void* w, const void* bias, const void*
   const int m_tiles = B * p.tiles_x * p.tiles_y;
   // weight is [Cout, 9*Cin] tap-major; when Cin is not a multiple of 64 each tap's K range is padded by TMA zero fill
   IH_CHECK(Cin % BK == 0, IH_ERR_SHAPE, "ih_conv2d_f16: Cin must be a multiple of 64 (got %d)", Cin);
-  CUtensorMap omap, rmap;
-  {
-    const uint64_t odims[4] = {(uint64_t)Cout, (uint64_t)Wo, (uint64_t)Ho, (uint64_t)B};
-    const uint64_t ostr[3] = {(uint64_t)Cout * 2, (uint64_t)Wo * Cout * 2, (uint64_t)Ho * Wo * Cout * 2};
-    const uint32_t obox[4] = {64u, (uint32_t)p.bw, (uint32_t)p.bh, 1u};
-    int rc = get_tmap_f16(&omap, out, 4, odims, ostr, obox);
-    if (rc) return rc;
-    rmap = omap;
-    if (residual) {
-      rc = get_tmap_f16(&rmap, residual, 4, odims, ostr, obox);
-      if (rc) return rc;
-    }
-  }
-  return dispatch(amaps, omap, rmap, w, Cout, (long long)9 * Cin + Csc0 + Csc1, p, m_tiles, 0, tile_n, (cudaStream_t)stream);
+  const uint64_t ostr[3] = {(uint64_t)Cout * 2, (uint64_t)Wo * Cout * 2, (uint64_t)Ho * Wo * Cout * 2};
+  const OutView ov{out, residual, 4, {(uint64_t)Cout, (uint64_t)Wo, (uint64_t)Ho, (uint64_t)B}, {ostr[0], ostr[1], ostr[2]},
+                   {ostr[0], ostr[1], ostr[2]}, {64u, (uint32_t)p.bw, (uint32_t)p.bh, 1u}};
+  return dispatch(amaps, ov, w, Cout, (long long)9 * Cin + Csc0 + Csc1, p, m_tiles, 0, tile_n, (cudaStream_t)stream);
 }

@@ -51,12 +51,13 @@ static std::mutex g_tmap_mu;
 static std::unordered_map<std::string, CUtensorMap> g_tmap_cache;
 
 int get_tmap_f16(CUtensorMap* out, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
-                 const uint32_t* box, bool swizzle128) {
+                 const uint32_t* box, int swizzle_bytes) {
+  if (swizzle_bytes != 128 && swizzle_bytes != 64) return set_error(IH_ERR_ARG, "unsupported swizzle %d", swizzle_bytes);
   TmapKey key;
   memset(&key, 0, sizeof(key));
   key.base = base;
   key.rank = rank;
-  key.swz = swizzle128 ? 1 : 0;
+  key.swz = swizzle_bytes;
   for (int i = 0; i < rank; ++i) {
     key.dims[i] = dims[i];
     key.box[i] = box[i];
@@ -90,7 +91,7 @@ int get_tmap_f16(CUtensorMap* out, const void* base, int rank, const uint64_t* d
   }
   CUtensorMap m;
   CUresult r = enc(&m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, rank, const_cast<void*>(base), gdim, gstr, bx, estr,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle128 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_NONE,
+                   CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle_bytes == 128 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B,
                    CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) return set_error(IH_ERR_TMAP, "cuTensorMapEncodeTiled failed with CUresult %d (rank %d)", (int)r, rank);
   {

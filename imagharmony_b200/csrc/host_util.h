@@ -20,11 +20,12 @@ int set_error(int code, const char* fmt, ...);
 
 enum { IH_ERR_ARG = -1, IH_ERR_SHAPE = -2, IH_ERR_ALIGN = -3, IH_ERR_TMAP = -4, IH_ERR_CUDA = -100 };
 
-// Encode (or fetch from the process-wide cache) a tiled fp16 tensor map with 128-byte swizzle.
+// Encode (or fetch from the process-wide cache) a tiled fp16 tensor map with a 128-byte (default) or 64-byte swizzle
+// (box rows of 64 bytes: the GEMM epilogue's 32-column output slab).
 // dims[0] is the contiguous dimension; strides_bytes[i] is the byte stride of dims[i+1].
 // Returns 0 on success.
 int get_tmap_f16(CUtensorMap* out, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
-                 const uint32_t* box, bool swizzle128 = true);
+                 const uint32_t* box, int swizzle_bytes = 128);
 
 int num_sms();
 

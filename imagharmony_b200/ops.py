@@ -54,8 +54,8 @@ def linear(x: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor] = None
            stats_out: Optional[torch.Tensor] = None, quick_gelu: bool = False, alpha: float = 1.0) -> torch.Tensor:
     """out = epi(x @ w.T + bias + rowbias[row // rows_per_group]) + residual ; x [M,K], w [N,K] (nn.Linear layout).
 
-    LayerNorm folding: `stats_out` (float32 [ceil(N/64), M, 2]) receives per-row / per-64-column (sum, sumsq) of the
-    stored values; `ln=(stats, eps)` makes this GEMM consume RAW rows `x` with the gamma-scaled, row-centred weight and
+    LayerNorm folding: `stats_out` (float32 [ceil(N/64), M, 2]) receives per-row (sum, sumsq) of the stored values as
+    partial sums whose total over slots is the row's; `ln=(stats, eps)` makes this GEMM consume RAW rows `x` with the gamma-scaled, row-centred weight and
     the constant vector of fold_layernorm (passed as `w`, `bias`) and apply rstd * acc + bias in the epilogue."""
     lib = _lib.load()
     _req(x, "x"); _req(w, "w")

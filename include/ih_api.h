@@ -35,14 +35,17 @@ void ih_launch_count_reset(void);
 /* out[M,N] = epi(A[M,K] @ W[N,K]^T + bias[N] + rowbias[row / rows_per_group, N]) + residual[M,N]
  * Replaces nn.Linear: attention_processor.py:292,299-300,320 (AttnProcessor2_0 to_q/to_k/to_v/to_out),
  * :396,410-411,432-433,453 (IPAttnProcessor2_0 incl. to_k_ip/to_v_ip), and the diffusers proj_in/proj_out/FF/1x1
- * conv layers reached through custom_pipelines.py:338-345.  tile_n: 0 = auto, else 64/128/256. */
+ * conv layers reached through custom_pipelines.py:338-345.  tile_n: 0 = auto, else 64/128/160/192/256 (384 and
+ * 512 mean 192 and 256). */
 int ih_gemm_f16(const void* a, long long lda, const void* w, const void* bias, const void* rowbias,
                 int rows_per_group, long long ld_rowbias, const void* residual, long long ldr, void* out,
                 long long ldo, int M, int N, int K, int epilogue, int tile_n, void* stream);
 
 /* ih_gemm_f16 with LayerNorm folded in (BasicTransformerBlock norm1/2/3 -> attn / FF projections).
- *   stats_out != NULL : additionally write, per output row and 64-column slab, (sum, sum of squares) of the fp16 values
- *                       stored: float [ceil(N/64), M, 2] (one writer per slot; deterministic).
+ *   stats_out != NULL : additionally write, per output row, (sum, sum of squares) of the fp16 values stored as
+ *                       float [ceil(N/64), M, 2]: partial sums whose total over slots is the row's (one writer per
+ *                       slot, every slot written; deterministic).  160-column tiles (tile_n = 160, or the automatic
+ *                       choice) need N % 320 == 0 here; the automatic choice respects that.
  *   ln_stats  != NULL : `a` holds the RAW (un-normalised) rows; `w` is the weight pre-multiplied by the LayerNorm gamma
  *                       with every row centred (w[n,k] = W[n,k] gamma[k] - mean_k(W[n,:] gamma)), so that
  *                       a w^T = (a - mean(a)) (W gamma)^T; `bias` = W beta + b.  The epilogue applies

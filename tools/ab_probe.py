@@ -13,8 +13,9 @@ from tools.microbench import timeit, r  # noqa: E402
 
 def tile_costs():
     M = 2048
-    for bn in (128, 192, 256):
-        N = 9 * bn                      # 9 x 16 = 144 tiles: one wave
+    cols = torch.cuda.get_device_properties(0).multi_processor_count // 16
+    for bn in (128, 160, 192, 256):
+        N = cols * bn                   # cols x 16 tiles <= #SMs: one round with (nearly) every SM busy
         ts = []
         for K in (1280, 5120):
             x, w = r(M, K), r(N, K, scale=K ** -0.5)
