@@ -473,6 +473,121 @@ __global__ void __launch_bounds__(1024) euler_inpaint_kernel(const __half* __res
   }
 }
 
+// ---------------------------------------------------------------------------------------------------------------
+// DPM-Solver++ 2M step ([3P] diffusers==0.30.0 DPMSolverMultistepScheduler, dpmsolver++ / midpoint / epsilon).  The
+// guided prediction is formed as in euler_cfg_kernel / euler_ex_kernel; every per-step scalar comes from the host
+// table coeffs[i, IH_DPM_COEFFS] (torch fp32 0-dim arithmetic, the diffusers expressions), so the kernel has no exp /
+// log and reproduces the fp16 / fp32 tensor arithmetic of convert_model_output + step:
+//   x0  = fp16(fp16(x - fp16(sigma_s * eps)) * inv_alpha_s)       (ATen divides by a CPU scalar as a * (1 / b))
+//   out = fp32(ratio * x) - fp16(c * x0)                            first order
+//       - fp16(c_half * fp16(inv_r0 * fp16(x0 - prev_x0)))          second order (midpoint), prev_x0 = last step's x0
+//   latents = model_in = prev... = fp16(out); prev_x0 <- x0
+// Products and differences use explicit _rn intrinsics so that nvcc cannot contract them into FMAs that torch does not
+// form.  A step is first order iff i == *loop_begin or coeffs[i].first != 0; both are read-only here.
+// ---------------------------------------------------------------------------------------------------------------
+struct DpmCoeffs {
+  float sigma_s, inv_alpha_s, ratio, c, c_half, inv_r0;
+  bool second;
+};
+
+__device__ __forceinline__ float cfg_guided(const __half* __restrict__ noise, long long idx, long long total, int cfg,
+                                            float guidance, float& c_out) {
+  if (!cfg) {
+    c_out = __half2float(noise[idx]);
+    return c_out;
+  }
+  const float u = __half2float(noise[idx]);
+  const float c = __half2float(noise[total + idx]);
+  c_out = c;
+  const float d1 = __half2float(__float2half_rn(c - u));
+  const float d2 = __half2float(__float2half_rn(guidance * d1));
+  return __half2float(__float2half_rn(u + d2));
+}
+
+__device__ __forceinline__ float h16(float v) { return __half2float(__float2half_rn(v)); }
+
+__device__ __forceinline__ void dpm_elem(long long idx, float eps, const DpmCoeffs& k, long long total, int cfg,
+                                         __half* __restrict__ latents, __half* __restrict__ model_in,
+                                         __half* __restrict__ prev_x0) {
+  const float x = __half2float(latents[idx]);
+  const float x0 = h16(__fmul_rn(h16(__fsub_rn(x, h16(__fmul_rn(k.sigma_s, eps)))), k.inv_alpha_s));
+  float out = __fsub_rn(__fmul_rn(k.ratio, x), h16(__fmul_rn(k.c, x0)));
+  if (k.second) {
+    const float d1 = h16(__fmul_rn(k.inv_r0, h16(__fsub_rn(x0, __half2float(prev_x0[idx])))));
+    out = __fsub_rn(out, h16(__fmul_rn(k.c_half, d1)));
+  }
+  const __half xh = __float2half_rn(out);
+  latents[idx] = xh;
+  prev_x0[idx] = __float2half_rn(x0);
+  model_in[idx] = xh;                      // scale_model_input is the identity for this scheduler
+  if (cfg) model_in[total + idx] = xh;
+}
+
+// Without guidance_rescale: grid-stride over all elements.  With it: one block per image, the std ratio reduced in the
+// order of euler_ex_kernel.
+__global__ void __launch_bounds__(1024) dpm_solver_kernel(const __half* __restrict__ noise, __half* __restrict__ latents,
+                                                          __half* __restrict__ model_in, __half* __restrict__ prev_x0,
+                                                          const float* __restrict__ coeffs, const int* __restrict__ step,
+                                                          const int* __restrict__ loop_begin, float guidance,
+                                                          float rescale, long long per_image, int n_images, int cfg) {
+  pdl_launch_dependents();
+  pdl_wait();
+  const int i = *step;
+  const float* row = coeffs + (long long)i * IH_DPM_COEFFS;
+  const DpmCoeffs k{row[0], row[1], row[2], row[3], row[4], row[5], !(i == *loop_begin || row[6] != 0.f)};
+  const long long total = per_image * n_images;
+  const bool resc = cfg && rescale > 0.f;
+  if (!resc) {
+    for (long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x; idx < total;
+         idx += (long long)gridDim.x * blockDim.x) {
+      float c;
+      dpm_elem(idx, cfg_guided(noise, idx, total, cfg, guidance, c), k, total, cfg, latents, model_in, prev_x0);
+    }
+    return;
+  }
+  const long long base = (long long)blockIdx.x * per_image;
+  double s_t = 0.0, q_t = 0.0, s_g = 0.0, q_g = 0.0;
+  for (long long e = threadIdx.x; e < per_image; e += blockDim.x) {
+    float c;
+    const float g = cfg_guided(noise, base + e, total, cfg, guidance, c);
+    s_t += c;
+    q_t += (double)c * c;
+    s_g += g;
+    q_g += (double)g * g;
+  }
+  __shared__ double red[4][32];
+  __shared__ float s_factor;
+  double v[4] = {s_t, q_t, s_g, q_g};
+#pragma unroll
+  for (int q = 0; q < 4; ++q) {
+    for (int o = 16; o > 0; o >>= 1) v[q] += __shfl_xor_sync(0xffffffffu, v[q], o);
+    if ((threadIdx.x & 31) == 0) red[q][threadIdx.x >> 5] = v[q];
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double t[4] = {0, 0, 0, 0};
+    const int nw = (blockDim.x + 31) >> 5;
+    for (int q = 0; q < 4; ++q)
+      for (int w = 0; w < nw; ++w) t[q] += red[q][w];
+    const double n = (double)per_image;
+    const double var_t = fmax((t[1] - t[0] * t[0] / n) / (n - 1.0), 0.0);
+    const double var_g = fmax((t[3] - t[2] * t[2] / n) / (n - 1.0), 0.0);
+    const float std_t = h16((float)sqrt(var_t));
+    const float std_g = h16((float)sqrt(var_g));
+    s_factor = h16(std_t / std_g);
+  }
+  __syncthreads();
+  const float factor = s_factor;
+  for (long long e = threadIdx.x; e < per_image; e += blockDim.x) {
+    float c;
+    const float eps = cfg_guided(noise, base + e, total, cfg, guidance, c);
+    const float r = h16(eps * factor);
+    const float a = h16(rescale * r);
+    const float b = h16((1.f - rescale) * eps);
+    dpm_elem(base + e, h16(a + b), k, total, cfg, latents, model_in, prev_x0);
+  }
+}
+
 __global__ void step_inc_kernel(int* step) {
   pdl_launch_dependents();
   pdl_wait();
@@ -997,6 +1112,27 @@ extern "C" int ih_euler_inpaint_step(const void* noise_pred, void* latents, void
                         (size_t)(0), stream, (const __half*)noise_pred, (__half*)latents, (__half*)model_in,
                         (const float*)sigmas, (const int*)step, guidance, guidance_rescale, n_per_image, n_images, cfg,
                         (const __half*)image_latents, (const __half*)noise, (const __half*)mask, (const int*)blend_end));
+  IH_CUDA(launch_kernel(step_inc_kernel, dim3(1), dim3(1), (size_t)(0), stream, (int*)step));
+  return 0;
+}
+
+extern "C" int ih_dpm_solver_step(const void* noise_pred, void* latents, void* model_in, void* prev_x0,
+                                  const void* coeffs, void* step, const void* loop_begin, float guidance,
+                                  float guidance_rescale, long long n_per_image, int n_images, int use_cfg,
+                                  void* stream_) {
+  cudaStream_t stream = (cudaStream_t)stream_;
+  IH_CHECK(noise_pred && latents && model_in && prev_x0 && coeffs && step && loop_begin, IH_ERR_ARG,
+           "ih_dpm_solver_step: null pointer");
+  IH_CHECK(n_per_image > 1 && n_images > 0, IH_ERR_SHAPE, "ih_dpm_solver_step: bad shape");
+  IH_CHECK(guidance_rescale >= 0.f && guidance_rescale <= 1.f, IH_ERR_ARG,
+           "ih_dpm_solver_step: guidance_rescale outside [0, 1]");
+  const int cfg = use_cfg ? 1 : 0;
+  const bool per_image = cfg && guidance_rescale > 0.f;
+  const long long total = n_per_image * n_images;
+  IH_CUDA(launch_kernel(dpm_solver_kernel, dim3(per_image ? n_images : grid_for(total, 256)), dim3(per_image ? 1024 : 256),
+                        (size_t)(0), stream, (const __half*)noise_pred, (__half*)latents, (__half*)model_in,
+                        (__half*)prev_x0, (const float*)coeffs, (const int*)step, (const int*)loop_begin, guidance,
+                        guidance_rescale, n_per_image, n_images, cfg));
   IH_CUDA(launch_kernel(step_inc_kernel, dim3(1), dim3(1), (size_t)(0), stream, (int*)step));
   return 0;
 }

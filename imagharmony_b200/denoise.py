@@ -10,8 +10,14 @@ not the graph): classifier-free guidance on or off (`guidance_scale <= 1`, :223,
 (:352-354), `denoising_end` (:307-316, via `num_loop_steps`), `callback` / `callback_steps` (:359-363),
 `control_guidance_start/end` IP-scale gating (:326-329), negative micro-conditioning time ids (:286-300).
 
+Schedulers: EulerDiscreteScheduler (the reference's) and DPMSolverMultistepScheduler (DPM-Solver++ 2M, SURVEY A.5), chosen
+by the engine's scheduler object in one place of `run`.  The DPM step reads its per-step scalars from a coefficient table
+and the previous step's data prediction from a static `prev_x0` buffer, both device-resident, so it too is one graph per
+shape.
+
 Graph lifetime: a captured graph holds raw pointers.  Everything it reads lives in buffers that are owned per shape
-and never freed while the graph exists -- the engine's static inputs (`_static`, `_inpaint_static`), the processors'
+and never freed while the graph exists -- the engine's static inputs (`_static`, `_inpaint_static`, `_dpm_static`),
+the schedule tables (`_tables`, `_coeffs`), the processors'
 K/V buffers and the UNet's add-embedding buffer (per-shape dicts inside those objects), and the library's grow-only
 scratch buffers whose re-allocation bumps `ops.workspace_generation()`.  A graph is replayed only if it was captured
 under the current UNet `graph_epoch` (weights / processors unchanged) and the current workspace generation; otherwise
@@ -19,19 +25,20 @@ it is re-captured.
 """
 from __future__ import annotations
 
-from typing import Callable, Dict, Optional, Tuple
+from typing import Callable, Dict, Optional, Tuple, Union
 
+import numpy as np
 import torch
 
 from . import ops
 from ._lib import IHError
-from .scheduler import EulerDiscreteScheduler
+from .scheduler import DPMSolverMultistepScheduler, EulerDiscreteScheduler
 from .unet import UNet2DConditionModel
 
 
 class DenoiseEngine:
     def __init__(self, unet: UNet2DConditionModel, use_cuda_graph: bool = True,
-                 scheduler: Optional[EulerDiscreteScheduler] = None):
+                 scheduler: Optional[Union[EulerDiscreteScheduler, DPMSolverMultistepScheduler]] = None):
         self.unet = unet
         self.device = unet.conv_in.weight.device
         self.scheduler = scheduler or EulerDiscreteScheduler()      # the pipeline's own scheduler object when given
@@ -39,20 +46,31 @@ class DenoiseEngine:
         self._graphs: Dict[Tuple, Tuple[torch.cuda.CUDAGraph, int]] = {}   # key -> (graph, workspace generation)
         self._static: Dict[Tuple, dict] = {}
         self._inpaint_static: Dict[Tuple, dict] = {}
-        self._tables: Dict[int, Tuple[torch.Tensor, torch.Tensor, float]] = {}
+        self._dpm_static: Dict[Tuple, dict] = {}
+        self._tables: Dict[Tuple[str, int], Tuple[torch.Tensor, torch.Tensor, float]] = {}
+        self._coeffs: Dict[Tuple[str, int], torch.Tensor] = {}         # DPM-Solver++ coefficient tables
         self._epoch = getattr(unet, "graph_epoch", 0)
         self.last_launches_per_step = 0
         self.graphs_captured = 0
 
     # ------------------------------------------------------------------------------------------------------------
     def tables(self, num_steps: int):
-        t = self._tables.get(num_steps)
+        """(timesteps fp32, sigmas fp32, init_noise_sigma) of the engine's scheduler on the device, per (kind, T);
+        with DPM-Solver++ the coefficient table is kept next to them (`coeffs`)."""
+        key = (self.scheduler.kind, num_steps)
+        t = self._tables.get(key)
         if t is None:
             s = self.scheduler.set_timesteps(num_steps)
-            t = (torch.from_numpy(s.timesteps).to(self.device), torch.from_numpy(s.sigmas).to(self.device),
-                 s.init_noise_sigma)
-            self._tables[num_steps] = t
+            t = (torch.from_numpy(s.timesteps.astype(np.float32)).to(self.device),
+                 torch.from_numpy(s.sigmas).to(self.device), s.init_noise_sigma)
+            self._tables[key] = t
+            if isinstance(self.scheduler, DPMSolverMultistepScheduler):
+                self._coeffs[key] = torch.from_numpy(s.coeffs).to(self.device)
         return t
+
+    def coeffs(self, num_steps: int) -> torch.Tensor:
+        self.tables(num_steps)
+        return self._coeffs[(self.scheduler.kind, num_steps)]
 
     def set_scale(self, scale: float) -> None:
         """IPAdapter.set_scale / pipeline.set_scale (ip_adapter.py:179-182, custom_pipelines.py:17-20)."""
@@ -94,9 +112,35 @@ class DenoiseEngine:
             self._inpaint_static[key] = ib
         return ib
 
-    def _step(self, st, timesteps, sigmas, guidance, use_cfg=True, rescale=0.0, ib=None):
+    def _dpm_buffers(self, n: int, h: int, w: int):
+        """DPM-Solver++ state per (n, h, w), never freed (the graph-lifetime rule above): the previous step's data
+        prediction and the schedule index the loop starts at (its step is first order)."""
+        key = (n, h, w)
+        db = self._dpm_static.get(key)
+        if db is None:
+            dev = self.device
+            db = {"prev_x0": torch.empty((n, self.unet.config.in_channels, h, w), dtype=torch.float16, device=dev),
+                  "loop_begin": torch.zeros((1,), dtype=torch.int32, device=dev)}
+            self._dpm_static[key] = db
+        return db
+
+    def _first_input(self, st, sigmas, use_cfg: bool, dpm) -> None:
+        """The UNet input of the loop's first step from st["latents"] (custom_pipelines.py:332-334)."""
+        if dpm is None:
+            ops.scale_model_input(st["latents"], st["model_in"], sigmas, st["step"], duplicate=use_cfg)
+            return
+        n = st["latents"].shape[0]                   # DPM-Solver++: scale_model_input is the identity
+        st["model_in"][:n].copy_(st["latents"])
+        if use_cfg:
+            st["model_in"][n:].copy_(st["latents"])
+
+    def _step(self, st, timesteps, sigmas, guidance, use_cfg=True, rescale=0.0, ib=None, dpm=None):
         noise = self.unet(st["model_in"], timesteps, st["ehs"], st["text_embeds"], st["time_ids"], step=st["step"])
-        if ib is None:
+        if dpm is not None:
+            db, coeffs = dpm
+            ops.dpm_solver_step(noise, st["latents"], st["model_in"], db["prev_x0"], coeffs, st["step"],
+                                db["loop_begin"], guidance, use_cfg=use_cfg, guidance_rescale=rescale)
+        elif ib is None:
             ops.euler_step(noise, st["latents"], st["model_in"], sigmas, st["step"], guidance, use_cfg=use_cfg,
                            guidance_rescale=rescale)
         else:
@@ -134,10 +178,19 @@ class DenoiseEngine:
         image latents re-noised to the next sigma, and by the clean image latents after the last step of the loop
         (ops.euler_inpaint_step).  It composes with begin_step, num_loop_steps and the other loop options, not with
         start_step / stop_after (IHError).  Its step graphs are captured once per shape next to the text-to-image
-        ones; the loop end is a device value, so they serve every num_loop_steps."""
+        ones; the loop end is a device value, so they serve every num_loop_steps.
+
+        With a DPMSolverMultistepScheduler the loop is DPM-Solver++ 2M: the first model input is the latents themselves,
+        and every step updates the latents and the previous data prediction on the device.  It runs whole
+        text-to-image loops, with every option above except begin_step, inpaint, start_step and stop_after (IHError):
+        they would need the VP-form add_noise, or the history of another call."""
         use_cfg = guidance_scale > 1.0                                            # :223
         if use_cfg and (negative_prompt_embeds is None or negative_pooled is None):
             raise IHError("classifier-free guidance needs negative_prompt_embeds / negative_pooled")
+        is_dpm = isinstance(self.scheduler, DPMSolverMultistepScheduler)         # the one scheduler dispatch
+        if is_dpm and (begin_step or inpaint is not None or start_step or stop_after is not None):
+            raise IHError("DPMSolverMultistepScheduler runs whole text-to-image loops: begin_step (image-to-image), "
+                          "inpaint, start_step and stop_after need EulerDiscreteScheduler")
         n, _, h, w = latents.shape
         L = prompt_embeds.shape[1]
         T = num_inference_steps
@@ -161,6 +214,9 @@ class DenoiseEngine:
             st["ehs"].copy_(prompt_embeds, non_blocking=True)
             st["text_embeds"].copy_(pooled, non_blocking=True)
             st["time_ids"].copy_(time_ids, non_blocking=True)
+        dpm = None
+        if is_dpm:
+            dpm = (self._dpm_buffers(n, h, w), self.coeffs(T))
         ib = None
         if inpaint is not None:
             if start_step or stop_after is not None:
@@ -180,8 +236,10 @@ class DenoiseEngine:
                 raise IHError(f"begin_step {begin_step} leaves no step of the {loop_T}-step loop")
             start_step = begin_step
         st["step"].fill_(start_step)
+        if dpm is not None:
+            dpm[0]["loop_begin"].fill_(start_step)
         self.unet.prepare_conditioning(st["ehs"], st["text_embeds"], st["time_ids"])
-        ops.scale_model_input(st["latents"], st["model_in"], sigmas, st["step"], duplicate=use_cfg)   # :332-334
+        self._first_input(st, sigmas, use_cfg, dpm)                                    # :332-334
 
         steps = loop_T if stop_after is None else min(stop_after, loop_T)
 
@@ -192,7 +250,7 @@ class DenoiseEngine:
             return 0.0 if off else float(ip_scale)
 
         def gkey(scale: float):
-            return (n, h, w, L, T, use_cfg, float(guidance_scale), rescale, scale, ib is not None)
+            return (n, h, w, L, T, use_cfg, float(guidance_scale), rescale, scale, self.scheduler.kind, ib is not None)
 
         if self.use_cuda_graph:
             if self._epoch != getattr(self.unet, "graph_epoch", 0):       # weights / processors changed since capture
@@ -207,7 +265,7 @@ class DenoiseEngine:
                     break
                 for sc in missing:
                     self.set_scale(sc)
-                    g = self._capture(st, timesteps, sigmas, guidance_scale, use_cfg, rescale, ib)
+                    g = self._capture(st, timesteps, sigmas, guidance_scale, use_cfg, rescale, ib, dpm)
                     self._graphs[gkey(sc)] = (g, ops.workspace_generation())
                     captured = True
             else:
@@ -216,34 +274,34 @@ class DenoiseEngine:
                 # the warm-up pass of a capture advances the state once: restore the initial state
                 st["latents"].copy_(latents, non_blocking=True)
                 st["step"].fill_(start_step)
-                ops.scale_model_input(st["latents"], st["model_in"], sigmas, st["step"], duplicate=use_cfg)
+                self._first_input(st, sigmas, use_cfg, dpm)
         for i in range(start_step, steps):
             sc = scale_at(i)
             if self.use_cuda_graph:
                 self._graphs[gkey(sc)][0].replay()
             else:
                 self.set_scale(sc)
-                self._step(st, timesteps, sigmas, guidance_scale, use_cfg, rescale, ib)
+                self._step(st, timesteps, sigmas, guidance_scale, use_cfg, rescale, ib, dpm)
             if callback is not None and (i - b0) % callback_steps == 0:           # :359-363 (Euler: order 1, no warm-up)
                 callback(i - b0, timesteps[i], st["latents"])
         self.set_scale(ip_scale)
         return st["latents"].clone()
 
-    def _capture(self, st, timesteps, sigmas, guidance, use_cfg=True, rescale=0.0, ib=None):
+    def _capture(self, st, timesteps, sigmas, guidance, use_cfg=True, rescale=0.0, ib=None, dpm=None):
         # warm-up on a side stream (sets kernel attributes, fills the TMA descriptor cache, sizes the allocator and
         # the library's scratch buffers)
         side = torch.cuda.Stream(device=self.device)
         side.wait_stream(torch.cuda.current_stream())
         with torch.cuda.stream(side):
             st["step"].zero_()
-            self._step(st, timesteps, sigmas, guidance, use_cfg, rescale, ib)
+            self._step(st, timesteps, sigmas, guidance, use_cfg, rescale, ib, dpm)
         torch.cuda.current_stream().wait_stream(side)
         torch.cuda.synchronize()
         st["step"].zero_()
         g = torch.cuda.CUDAGraph()
         before = ops.launch_count()
         with torch.cuda.graph(g):
-            self._step(st, timesteps, sigmas, guidance, use_cfg, rescale, ib)
+            self._step(st, timesteps, sigmas, guidance, use_cfg, rescale, ib, dpm)
         self.last_launches_per_step = ops.launch_count() - before
         self.graphs_captured += 1
         return g

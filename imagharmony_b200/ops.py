@@ -636,6 +636,30 @@ def euler_inpaint_step(noise_pred: torch.Tensor, latents: torch.Tensor, model_in
                                     _stream()), "ih_euler_inpaint_step")
 
 
+def dpm_solver_step(noise_pred: torch.Tensor, latents: torch.Tensor, model_in: torch.Tensor, prev_x0: torch.Tensor,
+                    coeffs: torch.Tensor, step: torch.Tensor, loop_begin: torch.Tensor, guidance: float, *,
+                    use_cfg: bool = True, guidance_rescale: float = 0.0) -> None:
+    """One DPM-Solver++ 2M transition (ih_dpm_solver_step) with the loop options of euler_step: the guided prediction's
+    data estimate x0 goes to `prev_x0` for the next step, the new latents to `latents` and, unscaled, to `model_in`.
+    coeffs: fp32 [T, 8] (DPMSolverMultistepScheduler.coeffs) indexed by the device step counter; loop_begin: device
+    int32, the schedule index whose step is first order because it has no history."""
+    lib = _lib.load()
+    _req(noise_pred, "noise_pred"); _req(latents, "latents"); _req(model_in, "model_in"); _req(prev_x0, "prev_x0")
+    _req(coeffs, "coeffs", torch.float32); _req(step, "step", torch.int32); _req(loop_begin, "loop_begin", torch.int32)
+    n = latents.shape[0]
+    per = latents.numel() // n
+    want = (2 * n if use_cfg else n) * per
+    if noise_pred.numel() != want or model_in.numel() != want:
+        raise IHError(f"dpm_solver_step: noise_pred / model_in must hold {want} elements (use_cfg={use_cfg})")
+    if prev_x0.shape != latents.shape or not (latents.is_contiguous() and prev_x0.is_contiguous()):
+        raise IHError("dpm_solver_step: contiguous latents and prev_x0 of one shape required")
+    if coeffs.dim() != 2 or coeffs.shape[1] != 8 or not coeffs.is_contiguous():
+        raise IHError("dpm_solver_step: coeffs must be a contiguous [T, 8] table")
+    check(lib.ih_dpm_solver_step(noise_pred.data_ptr(), latents.data_ptr(), model_in.data_ptr(), prev_x0.data_ptr(),
+                                 coeffs.data_ptr(), step.data_ptr(), loop_begin.data_ptr(), float(guidance),
+                                 float(guidance_rescale), per, n, int(use_cfg), _stream()), "ih_dpm_solver_step")
+
+
 def scale_model_input(latents: torch.Tensor, model_in: torch.Tensor, sigmas: torch.Tensor, step: torch.Tensor,
                       duplicate: bool = True) -> None:
     lib = _lib.load()

@@ -261,6 +261,21 @@ int ih_euler_inpaint_step(const void* noise_pred, void* latents, void* model_in,
                           const void* image_latents, const void* noise, const void* mask, const void* blend_end,
                           void* stream);
 
+/* DPM-Solver++ 2M transition ([3P] diffusers DPMSolverMultistepScheduler: dpmsolver++, midpoint, epsilon prediction)
+ * with the use_cfg / guidance_rescale options and CFG rounding points of ih_euler_step_ex.  Step i = *step reads row i
+ * of coeffs, fp32 [T, IH_DPM_COEFFS] computed on the host:
+ *   {sigma_s, 1/alpha_s, sigma_t/sigma_s, c = alpha_t*(exp(-h)-1), 0.5*c, 1/r0, first, 0}
+ * (VP sigmas, h = lambda_t - lambda_s, r0 = h_prev / h).  With eps the guided prediction and x the fp16 latents:
+ *   x0 = fp16(fp16(x - fp16(sigma_s*eps)) * (1/alpha_s));
+ *   x  <- fp16(fp32(ratio*x) - fp16(c*x0) [- fp16(0.5c * fp16(1/r0 * fp16(x0 - prev_x0)))])
+ * where the bracket (second order) is dropped iff i == *loop_begin or first != 0.  Writes latents, prev_x0 <- x0 and
+ * model_in <- x (unscaled, duplicated with CFG); step counter i += 1.  prev_x0: [n,C,H,W] fp16; loop_begin: device
+ * int32, the first schedule index of the loop (only read). */
+#define IH_DPM_COEFFS 8
+int ih_dpm_solver_step(const void* noise_pred, void* latents, void* model_in, void* prev_x0, const void* coeffs,
+                       void* step, const void* loop_begin, float guidance, float guidance_rescale, long long n_per_image,
+                       int n_images, int use_cfg, void* stream);
+
 /* model_in = cat([latents, latents]) / sqrt(sigma[*step]^2 + 1)   (custom_pipelines.py:332-334, first step). */
 int ih_scale_model_input(const void* latents, void* model_in, const void* sigmas, const void* step, long long total,
                          void* stream);

@@ -7,6 +7,8 @@ a dependency here, so the pieces the reference touches are provided directly:
 
 Denoise loop semantics follow custom_pipelines.py:188-363 (CFG batch [negative, positive], per-step IP-scale gating
 by control_guidance_start/end, Euler update); the loop itself runs as replayed CUDA graphs (imagharmony_b200/denoise.py).
+Text-to-image also runs DPM-Solver++ 2M: pass `scheduler=DPMSolverMultistepScheduler.from_config(pipe.scheduler.config,
+use_karras_sigmas=True)` or assign it to `pipe.scheduler`, as with diffusers.
 VAE decode / PIL post-processing (:365-386, scope row f1) runs on the native decoder `imagharmony_b200.vae` when the
 pipeline owns one (`from_random`, or `from_pretrained` with a `vae/` folder); a `vae_decode` callable overrides it and
 `output_type="latent"` skips it.
@@ -24,7 +26,7 @@ from imagharmony_b200 import ops
 from imagharmony_b200._lib import IHError
 from imagharmony_b200.config import SDXL_BASE, UNetConfig
 from imagharmony_b200.denoise import DenoiseEngine
-from imagharmony_b200.scheduler import EulerDiscreteScheduler
+from imagharmony_b200.scheduler import DPMSolverMultistepScheduler, EulerDiscreteScheduler
 from imagharmony_b200.unet import UNet2DConditionModel
 
 from .utils import is_torch2_available
@@ -62,8 +64,8 @@ class StableDiffusionXLCustomPipeline:
     force_zeros_for_empty_prompt = True     # [3P] SDXL-base pipeline config
 
     def __init__(self, unet: UNet2DConditionModel, prompt_encoder: Optional[Callable] = None,
-                 vae_decode: Optional[Callable] = None, scheduler: Optional[EulerDiscreteScheduler] = None,
-                 vae=None):
+                 vae_decode: Optional[Callable] = None,
+                 scheduler: Optional[Union[EulerDiscreteScheduler, DPMSolverMultistepScheduler]] = None, vae=None):
         self.unet = unet
         self.vae = vae                      # imagharmony_b200.vae.AutoencoderKLDecoder or None
         self.scheduler = scheduler or EulerDiscreteScheduler()
@@ -337,8 +339,9 @@ class StableDiffusionXLImg2ImgPipeline(StableDiffusionXLCustomPipeline):
                    "clip_skip", "callback_on_step_end")
 
     def __init__(self, unet: UNet2DConditionModel, prompt_encoder: Optional[Callable] = None,
-                 vae_decode: Optional[Callable] = None, scheduler: Optional[EulerDiscreteScheduler] = None,
-                 vae=None, vae_encoder=None):
+                 vae_decode: Optional[Callable] = None,
+                 scheduler: Optional[Union[EulerDiscreteScheduler, DPMSolverMultistepScheduler]] = None, vae=None,
+                 vae_encoder=None):
         super().__init__(unet, prompt_encoder=prompt_encoder, vae_decode=vae_decode, scheduler=scheduler, vae=vae)
         self.vae_encoder = vae_encoder      # imagharmony_b200.vae.AutoencoderKLEncoder or None
 
@@ -417,6 +420,7 @@ class StableDiffusionXLImg2ImgPipeline(StableDiffusionXLCustomPipeline):
         """The text-to-image parameter list without height / width, plus `image` (PIL image(s) or a [B, 3, H, W]
         tensor in [-1, 1]) and `strength`.  Unknown keywords are ignored as in the text-to-image pipeline, except the
         diffusers arguments in UNSUPPORTED, which raise IHError."""
+        self._require_euler()
         refused = [k for k in self.UNSUPPORTED if kwargs.get(k) is not None]
         if refused:
             raise IHError(f"StableDiffusionXLImg2ImgPipeline does not implement {refused}")
@@ -452,6 +456,13 @@ class StableDiffusionXLImg2ImgPipeline(StableDiffusionXLCustomPipeline):
         out = self._denoise_from(lat, t_start, num_inference_steps, denoising_end, embeds, sizes, guidance_scale,
                                  guidance_rescale, control_guidance_start, control_guidance_end, callback, callback_steps)
         return self._output(out, output_type, return_dict)
+
+    def _require_euler(self) -> None:
+        """Image-to-image and inpainting noise the image latents with Euler's add_noise (x + sigma * noise) inside the
+        posterior kernel; DPM-Solver++ noises in VP form (alpha * x + sigma_vp * noise), which it does not compute."""
+        if isinstance(self.scheduler, DPMSolverMultistepScheduler):
+            raise IHError(f"{type(self).__name__} supports EulerDiscreteScheduler only; DPMSolverMultistepScheduler runs "
+                          "text-to-image (StableDiffusionXLCustomPipeline)")
 
     def _denoise_from(self, lat, t_start: int, num_inference_steps: int, denoising_end, embeds, sizes, guidance_scale,
                       guidance_rescale, control_guidance_start, control_guidance_end, callback, callback_steps,
@@ -585,6 +596,7 @@ class StableDiffusionXLInpaintPipeline(StableDiffusionXLImg2ImgPipeline):
         """The image-to-image parameter list plus `mask_image` (PIL image(s) or a tensor in [0, 1]; 1 = regenerate),
         `height`, `width` and `padding_mask_crop`.  Unknown keywords are ignored, except the diffusers arguments in
         UNSUPPORTED and a `padding_mask_crop`, which raise IHError."""
+        self._require_euler()
         refused = [k for k in self.UNSUPPORTED if kwargs.get(k) is not None]
         if padding_mask_crop is not None:
             refused.append("padding_mask_crop")
