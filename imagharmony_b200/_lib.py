@@ -123,6 +123,9 @@ SIGNATURES = {
                                       c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "ih_dpm_solver_step": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_float,
                                    c_float, c_longlong, c_int, c_int, c_void_p]),
+    "ih_euler_ancestral_step": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_float, c_float,
+                                        c_longlong, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "ih_euler_ancestral_scale_input": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_longlong, c_int, c_void_p]),
     "ih_scale_model_input": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_longlong, c_void_p]),
     "ih_scale_model_input_ex": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_longlong, c_int, c_void_p]),
 }

@@ -588,6 +588,131 @@ __global__ void __launch_bounds__(1024) dpm_solver_kernel(const __half* __restri
   }
 }
 
+// ---------------------------------------------------------------------------------------------------------------
+// Euler Ancestral step ([3P] diffusers==0.30.0 EulerAncestralDiscreteScheduler, epsilon).  The guided prediction is
+// formed as in euler_cfg_kernel / euler_ex_kernel; the per-step scalars come from the host table
+// coeffs[i, IH_EULER_A_COEFFS] (torch fp32 0-dim arithmetic) and the step's Gaussian noise from row i of a buffer the
+// host fills from the caller's torch generator before the graph replays:
+//   x0   = x - fp16(sigma * eps)             (sample = x.float(); sigma * fp16 tensor is an fp16 tensor)
+//   prev = fp32(fp32((x - x0) * inv_sigma) * dt) + x      (ATen divides by a CPU scalar as a * (1 / b))
+//   prev = fp16(prev + fp16(noise * sigma_up))
+// then, when image latents are given, the inpainting blend of euler_inpaint_elem, and the next model input
+// fp16(x * inv_den_next).  Explicit _rn intrinsics keep nvcc from forming FMAs that torch does not form.
+// ---------------------------------------------------------------------------------------------------------------
+struct EulerACoeffs {
+  float sigma, inv_sigma, dt, sigma_up, inv_den_next;
+};
+
+// ia.image_latents == nullptr: no blend (text-to-image, image-to-image).
+__device__ __forceinline__ void euler_a_elem(long long idx, float eps, const EulerACoeffs& k,
+                                             const __half* __restrict__ step_noise, const InpaintArgs& ia,
+                                             long long per_image, long long total, int cfg,
+                                             __half* __restrict__ latents, __half* __restrict__ model_in) {
+  const float x = __half2float(latents[idx]);
+  const float x0 = __fsub_rn(x, h16(__fmul_rn(k.sigma, eps)));
+  const float d = __fmul_rn(__fsub_rn(x, x0), k.inv_sigma);
+  const float prev = __fadd_rn(x, __fmul_rn(d, k.dt));
+  float xa = h16(__fadd_rn(prev, h16(__fmul_rn(__half2float(step_noise[idx]), k.sigma_up))));
+  if (ia.image_latents) {
+    const long long b = idx / per_image;
+    const float m = __half2float(ia.mask[b * ia.hw + (idx - b * per_image) % ia.hw]);
+    float proper = __half2float(ia.image_latents[idx]);
+    if (ia.renoise) proper = h16(__fadd_rn(proper, h16(__fmul_rn(__half2float(ia.noise[idx]), ia.sig_next16))));
+    const float keep = h16(__fmul_rn(h16(__fsub_rn(1.f, m)), proper));
+    xa = h16(__fadd_rn(keep, h16(__fmul_rn(m, xa))));
+  }
+  const __half xh = __float2half_rn(xa);
+  latents[idx] = xh;
+  const __half mi = __float2half_rn(__fmul_rn(xa, k.inv_den_next));
+  model_in[idx] = mi;
+  if (cfg) model_in[total + idx] = mi;
+}
+
+// fp16(std_text / std_guided) of image blockIdx.x (guidance_rescale), reduced in the order of euler_ex_kernel.
+__device__ float cfg_rescale_factor(const __half* __restrict__ noise, long long base, long long per_image,
+                                    long long total, float guidance) {
+  double s_t = 0.0, q_t = 0.0, s_g = 0.0, q_g = 0.0;
+  for (long long e = threadIdx.x; e < per_image; e += blockDim.x) {
+    float c;
+    const float g = cfg_guided(noise, base + e, total, 1, guidance, c);
+    s_t += c;
+    q_t += (double)c * c;
+    s_g += g;
+    q_g += (double)g * g;
+  }
+  __shared__ double red[4][32];
+  __shared__ float s_factor;
+  double v[4] = {s_t, q_t, s_g, q_g};
+#pragma unroll
+  for (int q = 0; q < 4; ++q) {
+    for (int o = 16; o > 0; o >>= 1) v[q] += __shfl_xor_sync(0xffffffffu, v[q], o);
+    if ((threadIdx.x & 31) == 0) red[q][threadIdx.x >> 5] = v[q];
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double t[4] = {0, 0, 0, 0};
+    const int nw = (blockDim.x + 31) >> 5;
+    for (int q = 0; q < 4; ++q)
+      for (int w = 0; w < nw; ++w) t[q] += red[q][w];
+    const double n = (double)per_image;
+    const double var_t = fmax((t[1] - t[0] * t[0] / n) / (n - 1.0), 0.0);
+    const double var_g = fmax((t[3] - t[2] * t[2] / n) / (n - 1.0), 0.0);
+    s_factor = h16(h16((float)sqrt(var_t)) / h16((float)sqrt(var_g)));
+  }
+  __syncthreads();
+  return s_factor;
+}
+
+// Without guidance_rescale: grid-stride over all elements.  With it: one block per image.
+__global__ void __launch_bounds__(1024) euler_ancestral_kernel(
+    const __half* __restrict__ noise, __half* __restrict__ latents, __half* __restrict__ model_in,
+    const float* __restrict__ coeffs, const __half* __restrict__ step_noise, const int* __restrict__ step,
+    float guidance, float rescale, long long per_image, int n_images, int cfg, const __half* __restrict__ image_latents,
+    const __half* __restrict__ blend_noise, const __half* __restrict__ mask, const int* __restrict__ blend_end) {
+  pdl_launch_dependents();
+  pdl_wait();
+  const int i = *step;
+  const float* row = coeffs + (long long)i * IH_EULER_A_COEFFS;
+  const EulerACoeffs k{row[0], row[1], row[2], row[3], row[4]};
+  const long long total = per_image * n_images;
+  const __half* nz = step_noise + (long long)i * total;
+  const InpaintArgs ia{image_latents, blend_noise, mask, per_image / 4, image_latents && i + 1 < *blend_end, row[5]};
+  if (!(cfg && rescale > 0.f)) {
+    for (long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x; idx < total;
+         idx += (long long)gridDim.x * blockDim.x) {
+      float c;
+      euler_a_elem(idx, cfg_guided(noise, idx, total, cfg, guidance, c), k, nz, ia, per_image, total, cfg, latents,
+                   model_in);
+    }
+    return;
+  }
+  const long long base = (long long)blockIdx.x * per_image;
+  const float factor = cfg_rescale_factor(noise, base, per_image, total, guidance);
+  for (long long e = threadIdx.x; e < per_image; e += blockDim.x) {
+    float c;
+    const float eps = cfg_guided(noise, base + e, total, cfg, guidance, c);
+    const float r = h16(eps * factor);
+    const float a = h16(rescale * r);
+    const float b = h16((1.f - rescale) * eps);
+    euler_a_elem(base + e, h16(a + b), k, nz, ia, per_image, total, cfg, latents, model_in);
+  }
+}
+
+// The loop's first model input in the convention of euler_ancestral_kernel: fp16(x * coeffs[*step, IN_SCALE]).
+__global__ void euler_a_scale_input_kernel(const __half* __restrict__ latents, __half* __restrict__ model_in,
+                                           const float* __restrict__ coeffs, const int* __restrict__ step,
+                                           long long total, int duplicate) {
+  pdl_launch_dependents();
+  pdl_wait();
+  const float s = coeffs[(long long)*step * IH_EULER_A_COEFFS + 6];
+  for (long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x; idx < total;
+       idx += (long long)gridDim.x * blockDim.x) {
+    const __half mi = __float2half_rn(__fmul_rn(__half2float(latents[idx]), s));
+    model_in[idx] = mi;
+    if (duplicate) model_in[total + idx] = mi;
+  }
+}
+
 __global__ void step_inc_kernel(int* step) {
   pdl_launch_dependents();
   pdl_wait();
@@ -1134,6 +1259,42 @@ extern "C" int ih_dpm_solver_step(const void* noise_pred, void* latents, void* m
                         (__half*)prev_x0, (const float*)coeffs, (const int*)step, (const int*)loop_begin, guidance,
                         guidance_rescale, n_per_image, n_images, cfg));
   IH_CUDA(launch_kernel(step_inc_kernel, dim3(1), dim3(1), (size_t)(0), stream, (int*)step));
+  return 0;
+}
+
+extern "C" int ih_euler_ancestral_step(const void* noise_pred, void* latents, void* model_in, const void* coeffs,
+                                       const void* step_noise, void* step, float guidance, float guidance_rescale,
+                                       long long n_per_image, int n_images, int use_cfg, const void* image_latents,
+                                       const void* blend_noise, const void* mask, const void* blend_end,
+                                       void* stream_) {
+  cudaStream_t stream = (cudaStream_t)stream_;
+  IH_CHECK(noise_pred && latents && model_in && coeffs && step_noise && step, IH_ERR_ARG,
+           "ih_euler_ancestral_step: null pointer");
+  const bool blend = image_latents != nullptr;
+  IH_CHECK(blend == (blend_noise != nullptr) && blend == (mask != nullptr) && blend == (blend_end != nullptr),
+           IH_ERR_ARG, "ih_euler_ancestral_step: image_latents, blend_noise, mask and blend_end go together");
+  IH_CHECK(n_per_image > 1 && n_images > 0 && (!blend || n_per_image % 4 == 0), IH_ERR_SHAPE,
+           "ih_euler_ancestral_step: bad shape");
+  IH_CHECK(guidance_rescale >= 0.f && guidance_rescale <= 1.f, IH_ERR_ARG,
+           "ih_euler_ancestral_step: guidance_rescale outside [0, 1]");
+  const int cfg = use_cfg ? 1 : 0;
+  const bool per_image = cfg && guidance_rescale > 0.f;
+  const long long total = n_per_image * n_images;
+  IH_CUDA(launch_kernel(euler_ancestral_kernel, dim3(per_image ? n_images : grid_for(total, 256)),
+                        dim3(per_image ? 1024 : 256), (size_t)(0), stream, (const __half*)noise_pred, (__half*)latents,
+                        (__half*)model_in, (const float*)coeffs, (const __half*)step_noise, (const int*)step, guidance,
+                        guidance_rescale, n_per_image, n_images, cfg, (const __half*)image_latents,
+                        (const __half*)blend_noise, (const __half*)mask, (const int*)blend_end));
+  IH_CUDA(launch_kernel(step_inc_kernel, dim3(1), dim3(1), (size_t)(0), stream, (int*)step));
+  return 0;
+}
+
+extern "C" int ih_euler_ancestral_scale_input(const void* latents, void* model_in, const void* coeffs, const void* step,
+                                              long long total, int duplicate, void* stream) {
+  IH_CHECK(latents && model_in && coeffs && step, IH_ERR_ARG, "ih_euler_ancestral_scale_input: null pointer");
+  IH_CUDA(launch_kernel(euler_a_scale_input_kernel, dim3(grid_for(total, 256)), dim3(256), (size_t)(0),
+                        (cudaStream_t)stream, (const __half*)latents, (__half*)model_in, (const float*)coeffs,
+                        (const int*)step, total, duplicate ? 1 : 0));
   return 0;
 }
 

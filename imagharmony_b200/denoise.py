@@ -10,14 +10,17 @@ not the graph): classifier-free guidance on or off (`guidance_scale <= 1`, :223,
 (:352-354), `denoising_end` (:307-316, via `num_loop_steps`), `callback` / `callback_steps` (:359-363),
 `control_guidance_start/end` IP-scale gating (:326-329), negative micro-conditioning time ids (:286-300).
 
-Schedulers: EulerDiscreteScheduler (the reference's) and DPMSolverMultistepScheduler (DPM-Solver++ 2M, SURVEY A.5), chosen
-by the engine's scheduler object in one place of `run`.  The DPM step reads its per-step scalars from a coefficient table
-and the previous step's data prediction from a static `prev_x0` buffer, both device-resident, so it too is one graph per
-shape.
+Schedulers: EulerDiscreteScheduler (the reference's), EulerAncestralDiscreteScheduler (SURVEY A.6) and
+DPMSolverMultistepScheduler (DPM-Solver++ 2M, SURVEY A.5), chosen by the engine's scheduler object in one place of `run`.
+The DPM step reads its per-step scalars from a coefficient table and the previous step's data prediction from a static
+`prev_x0` buffer, both device-resident, so it too is one graph per shape.  The Euler Ancestral step reads its scalars
+from a coefficient table and its Gaussian noise from row `step` of a static [T, n, 4, h, w] buffer that `run` fills from
+the caller's generator(s) before the replays, outside any capture: the draws are torch's, in diffusers' order, so a seed
+gives diffusers' noise (a Philox stream inside the kernel would not reproduce torch's generator).
 
 Graph lifetime: a captured graph holds raw pointers.  Everything it reads lives in buffers that are owned per shape
-and never freed while the graph exists -- the engine's static inputs (`_static`, `_inpaint_static`, `_dpm_static`),
-the schedule tables (`_tables`, `_coeffs`), the processors'
+and never freed while the graph exists -- the engine's static inputs (`_static`, `_inpaint_static`, `_dpm_static`,
+`_ancestral_noise`), the schedule tables (`_tables`, `_coeffs`), the processors'
 K/V buffers and the UNet's add-embedding buffer (per-shape dicts inside those objects), and the library's grow-only
 scratch buffers whose re-allocation bumps `ops.workspace_generation()`.  A graph is replayed only if it was captured
 under the current UNet `graph_epoch` (weights / processors unchanged) and the current workspace generation; otherwise
@@ -25,20 +28,21 @@ it is re-captured.
 """
 from __future__ import annotations
 
-from typing import Callable, Dict, Optional, Tuple, Union
+from typing import Callable, Dict, List, Optional, Tuple, Union
 
 import numpy as np
 import torch
 
 from . import ops
 from ._lib import IHError
-from .scheduler import DPMSolverMultistepScheduler, EulerDiscreteScheduler
+from .scheduler import DPMSolverMultistepScheduler, EulerAncestralDiscreteScheduler, EulerDiscreteScheduler
 from .unet import UNet2DConditionModel
 
 
 class DenoiseEngine:
     def __init__(self, unet: UNet2DConditionModel, use_cuda_graph: bool = True,
-                 scheduler: Optional[Union[EulerDiscreteScheduler, DPMSolverMultistepScheduler]] = None):
+                 scheduler: Optional[Union[EulerDiscreteScheduler, EulerAncestralDiscreteScheduler,
+                                           DPMSolverMultistepScheduler]] = None):
         self.unet = unet
         self.device = unet.conv_in.weight.device
         self.scheduler = scheduler or EulerDiscreteScheduler()      # the pipeline's own scheduler object when given
@@ -48,7 +52,8 @@ class DenoiseEngine:
         self._inpaint_static: Dict[Tuple, dict] = {}
         self._dpm_static: Dict[Tuple, dict] = {}
         self._tables: Dict[Tuple[str, int], Tuple[torch.Tensor, torch.Tensor, float]] = {}
-        self._coeffs: Dict[Tuple[str, int], torch.Tensor] = {}         # DPM-Solver++ coefficient tables
+        self._coeffs: Dict[Tuple[str, int], torch.Tensor] = {}         # DPM-Solver++ / Euler Ancestral coefficients
+        self._ancestral_noise: Dict[Tuple[int, int, int, int], torch.Tensor] = {}   # Euler Ancestral step noise
         self._epoch = getattr(unet, "graph_epoch", 0)
         self.last_launches_per_step = 0
         self.graphs_captured = 0
@@ -56,7 +61,7 @@ class DenoiseEngine:
     # ------------------------------------------------------------------------------------------------------------
     def tables(self, num_steps: int):
         """(timesteps fp32, sigmas fp32, init_noise_sigma) of the engine's scheduler on the device, per (kind, T);
-        with DPM-Solver++ the coefficient table is kept next to them (`coeffs`)."""
+        with DPM-Solver++ and Euler Ancestral the coefficient table is kept next to them (`coeffs`)."""
         key = (self.scheduler.kind, num_steps)
         t = self._tables.get(key)
         if t is None:
@@ -64,7 +69,7 @@ class DenoiseEngine:
             t = (torch.from_numpy(s.timesteps.astype(np.float32)).to(self.device),
                  torch.from_numpy(s.sigmas).to(self.device), s.init_noise_sigma)
             self._tables[key] = t
-            if isinstance(self.scheduler, DPMSolverMultistepScheduler):
+            if isinstance(self.scheduler, (DPMSolverMultistepScheduler, EulerAncestralDiscreteScheduler)):
                 self._coeffs[key] = torch.from_numpy(s.coeffs).to(self.device)
         return t
 
@@ -124,8 +129,36 @@ class DenoiseEngine:
             self._dpm_static[key] = db
         return db
 
-    def _first_input(self, st, sigmas, use_cfg: bool, dpm) -> None:
+    def _ancestral_buffer(self, n: int, h: int, w: int, T: int) -> torch.Tensor:
+        """Euler Ancestral step noise [T, n, C, h, w] per (n, h, w, T), never freed (the graph-lifetime rule above).
+        Zero-filled, so that a capture's warm-up step reads finite values."""
+        key = (n, h, w, T)
+        buf = self._ancestral_noise.get(key)
+        if buf is None:
+            buf = torch.zeros((T, n, self.unet.config.in_channels, h, w), dtype=torch.float16, device=self.device)
+            self._ancestral_noise[key] = buf
+        return buf
+
+    def _draw_ancestral_noise(self, buf: torch.Tensor, generator, begin: int, end: int) -> None:
+        """Rows [begin, end) of the step noise, one draw per step in step order, as [3P] diffusers' randn_tensor draws
+        it inside EulerAncestralDiscreteScheduler.step: fp16, shaped like the guided prediction, on the generator's
+        device (a CPU generator draws on the CPU), one [1, C, h, w] draw per generator of a list, and from the device's
+        default generator when `generator` is None."""
+        shape = tuple(buf.shape[1:])
+        for i in range(begin, end):
+            if isinstance(generator, list):
+                row = torch.cat([torch.randn((1,) + shape[1:], generator=g, device=g.device, dtype=torch.float16)
+                                 .to(self.device) for g in generator])
+            else:
+                dev = generator.device if generator is not None else self.device
+                row = torch.randn(shape, generator=generator, device=dev, dtype=torch.float16)
+            buf[i].copy_(row)
+
+    def _first_input(self, st, sigmas, use_cfg: bool, dpm, anc=None) -> None:
         """The UNet input of the loop's first step from st["latents"] (custom_pipelines.py:332-334)."""
+        if anc is not None:      # the convention of the ancestral kernel's later inputs: x * fp32(1 / sqrt(s^2 + 1))
+            ops.euler_ancestral_scale_input(st["latents"], st["model_in"], anc[0], st["step"], duplicate=use_cfg)
+            return
         if dpm is None:
             ops.scale_model_input(st["latents"], st["model_in"], sigmas, st["step"], duplicate=use_cfg)
             return
@@ -134,12 +167,16 @@ class DenoiseEngine:
         if use_cfg:
             st["model_in"][n:].copy_(st["latents"])
 
-    def _step(self, st, timesteps, sigmas, guidance, use_cfg=True, rescale=0.0, ib=None, dpm=None):
+    def _step(self, st, timesteps, sigmas, guidance, use_cfg=True, rescale=0.0, ib=None, dpm=None, anc=None):
         noise = self.unet(st["model_in"], timesteps, st["ehs"], st["text_embeds"], st["time_ids"], step=st["step"])
         if dpm is not None:
             db, coeffs = dpm
             ops.dpm_solver_step(noise, st["latents"], st["model_in"], db["prev_x0"], coeffs, st["step"],
                                 db["loop_begin"], guidance, use_cfg=use_cfg, guidance_rescale=rescale)
+        elif anc is not None:
+            blend = None if ib is None else (ib["image_latents"], ib["noise"], ib["mask"], ib["blend_end"])
+            ops.euler_ancestral_step(noise, st["latents"], st["model_in"], anc[0], anc[1], st["step"], guidance,
+                                     use_cfg=use_cfg, guidance_rescale=rescale, inpaint=blend)
         elif ib is None:
             ops.euler_step(noise, st["latents"], st["model_in"], sigmas, st["step"], guidance, use_cfg=use_cfg,
                            guidance_rescale=rescale)
@@ -157,7 +194,8 @@ class DenoiseEngine:
             start_step: int = 0, guidance_rescale: float = 0.0, num_loop_steps: Optional[int] = None,
             callback: Optional[Callable] = None, callback_steps: int = 1,
             negative_time_ids: Optional[torch.Tensor] = None, begin_step: int = 0,
-            inpaint: Optional[Tuple[torch.Tensor, torch.Tensor, torch.Tensor]] = None) -> torch.Tensor:
+            inpaint: Optional[Tuple[torch.Tensor, torch.Tensor, torch.Tensor]] = None,
+            generator: Optional[Union[torch.Generator, List[torch.Generator]]] = None) -> torch.Tensor:
         """latents [n,4,h,w] (already scaled by init_noise_sigma; host or device); embeds host or device tensors.
         Returns the latents after the last executed step as a new device tensor.
 
@@ -183,15 +221,24 @@ class DenoiseEngine:
         With a DPMSolverMultistepScheduler the loop is DPM-Solver++ 2M: the first model input is the latents themselves,
         and every step updates the latents and the previous data prediction on the device.  It runs whole
         text-to-image loops, with every option above except begin_step, inpaint, start_step and stop_after (IHError):
-        they would need the VP-form add_noise, or the history of another call."""
+        they would need the VP-form add_noise, or the history of another call.
+
+        With an EulerAncestralDiscreteScheduler every option above works.  `generator` (a torch.Generator, a list of
+        one per image, or None for the device's default generator) supplies the Gaussian noise of every step; before
+        the steps run, the noise of exactly the steps this call executes is drawn from it, one draw per step in step
+        order.  So `stop_after=k` followed by `start_step=k` with the same, continuing generator object reproduces the
+        uninterrupted run.  The other schedulers draw nothing and ignore `generator`."""
         use_cfg = guidance_scale > 1.0                                            # :223
         if use_cfg and (negative_prompt_embeds is None or negative_pooled is None):
             raise IHError("classifier-free guidance needs negative_prompt_embeds / negative_pooled")
         is_dpm = isinstance(self.scheduler, DPMSolverMultistepScheduler)         # the one scheduler dispatch
+        is_ancestral = isinstance(self.scheduler, EulerAncestralDiscreteScheduler)
         if is_dpm and (begin_step or inpaint is not None or start_step or stop_after is not None):
             raise IHError("DPMSolverMultistepScheduler runs whole text-to-image loops: begin_step (image-to-image), "
                           "inpaint, start_step and stop_after need EulerDiscreteScheduler")
         n, _, h, w = latents.shape
+        if is_ancestral and isinstance(generator, list) and len(generator) != n:
+            raise IHError(f"got {len(generator)} generators for a batch of {n}")
         L = prompt_embeds.shape[1]
         T = num_inference_steps
         loop_T = T if num_loop_steps is None else int(num_loop_steps)
@@ -214,9 +261,11 @@ class DenoiseEngine:
             st["ehs"].copy_(prompt_embeds, non_blocking=True)
             st["text_embeds"].copy_(pooled, non_blocking=True)
             st["time_ids"].copy_(time_ids, non_blocking=True)
-        dpm = None
+        dpm = anc = None
         if is_dpm:
             dpm = (self._dpm_buffers(n, h, w), self.coeffs(T))
+        elif is_ancestral:
+            anc = (self.coeffs(T), self._ancestral_buffer(n, h, w, T))
         ib = None
         if inpaint is not None:
             if start_step or stop_after is not None:
@@ -239,7 +288,7 @@ class DenoiseEngine:
         if dpm is not None:
             dpm[0]["loop_begin"].fill_(start_step)
         self.unet.prepare_conditioning(st["ehs"], st["text_embeds"], st["time_ids"])
-        self._first_input(st, sigmas, use_cfg, dpm)                                    # :332-334
+        self._first_input(st, sigmas, use_cfg, dpm, anc)                               # :332-334
 
         steps = loop_T if stop_after is None else min(stop_after, loop_T)
 
@@ -265,7 +314,7 @@ class DenoiseEngine:
                     break
                 for sc in missing:
                     self.set_scale(sc)
-                    g = self._capture(st, timesteps, sigmas, guidance_scale, use_cfg, rescale, ib, dpm)
+                    g = self._capture(st, timesteps, sigmas, guidance_scale, use_cfg, rescale, ib, dpm, anc)
                     self._graphs[gkey(sc)] = (g, ops.workspace_generation())
                     captured = True
             else:
@@ -274,34 +323,36 @@ class DenoiseEngine:
                 # the warm-up pass of a capture advances the state once: restore the initial state
                 st["latents"].copy_(latents, non_blocking=True)
                 st["step"].fill_(start_step)
-                self._first_input(st, sigmas, use_cfg, dpm)
+                self._first_input(st, sigmas, use_cfg, dpm, anc)
+        if anc is not None:
+            self._draw_ancestral_noise(anc[1], generator, start_step, steps)
         for i in range(start_step, steps):
             sc = scale_at(i)
             if self.use_cuda_graph:
                 self._graphs[gkey(sc)][0].replay()
             else:
                 self.set_scale(sc)
-                self._step(st, timesteps, sigmas, guidance_scale, use_cfg, rescale, ib, dpm)
+                self._step(st, timesteps, sigmas, guidance_scale, use_cfg, rescale, ib, dpm, anc)
             if callback is not None and (i - b0) % callback_steps == 0:           # :359-363 (Euler: order 1, no warm-up)
                 callback(i - b0, timesteps[i], st["latents"])
         self.set_scale(ip_scale)
         return st["latents"].clone()
 
-    def _capture(self, st, timesteps, sigmas, guidance, use_cfg=True, rescale=0.0, ib=None, dpm=None):
+    def _capture(self, st, timesteps, sigmas, guidance, use_cfg=True, rescale=0.0, ib=None, dpm=None, anc=None):
         # warm-up on a side stream (sets kernel attributes, fills the TMA descriptor cache, sizes the allocator and
         # the library's scratch buffers)
         side = torch.cuda.Stream(device=self.device)
         side.wait_stream(torch.cuda.current_stream())
         with torch.cuda.stream(side):
             st["step"].zero_()
-            self._step(st, timesteps, sigmas, guidance, use_cfg, rescale, ib, dpm)
+            self._step(st, timesteps, sigmas, guidance, use_cfg, rescale, ib, dpm, anc)
         torch.cuda.current_stream().wait_stream(side)
         torch.cuda.synchronize()
         st["step"].zero_()
         g = torch.cuda.CUDAGraph()
         before = ops.launch_count()
         with torch.cuda.graph(g):
-            self._step(st, timesteps, sigmas, guidance, use_cfg, rescale, ib, dpm)
+            self._step(st, timesteps, sigmas, guidance, use_cfg, rescale, ib, dpm, anc)
         self.last_launches_per_step = ops.launch_count() - before
         self.graphs_captured += 1
         return g

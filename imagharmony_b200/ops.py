@@ -6,7 +6,7 @@ PyTorch/CPU fallback: a CPU tensor or a missing library raises.
 from __future__ import annotations
 
 import os
-from typing import Optional
+from typing import Optional, Tuple
 
 import torch
 
@@ -658,6 +658,61 @@ def dpm_solver_step(noise_pred: torch.Tensor, latents: torch.Tensor, model_in: t
     check(lib.ih_dpm_solver_step(noise_pred.data_ptr(), latents.data_ptr(), model_in.data_ptr(), prev_x0.data_ptr(),
                                  coeffs.data_ptr(), step.data_ptr(), loop_begin.data_ptr(), float(guidance),
                                  float(guidance_rescale), per, n, int(use_cfg), _stream()), "ih_dpm_solver_step")
+
+
+def euler_ancestral_step(noise_pred: torch.Tensor, latents: torch.Tensor, model_in: torch.Tensor, coeffs: torch.Tensor,
+                         step_noise: torch.Tensor, step: torch.Tensor, guidance: float, *, use_cfg: bool = True,
+                         guidance_rescale: float = 0.0,
+                         inpaint: Optional[Tuple[torch.Tensor, torch.Tensor, torch.Tensor, torch.Tensor]] = None) -> None:
+    """One Euler Ancestral transition (ih_euler_ancestral_step) with the loop options of euler_step.  coeffs: fp32
+    [T, 8] (EulerAncestralDiscreteScheduler.coeffs) and step_noise: fp16 [T, n, C, h, w] (the Gaussian noise of every
+    step, drawn by the caller), both indexed by the device step counter.  `inpaint` = (image_latents, noise, mask,
+    blend_end) adds the blend of euler_inpaint_step."""
+    lib = _lib.load()
+    _req(noise_pred, "noise_pred"); _req(latents, "latents"); _req(model_in, "model_in"); _req(step_noise, "step_noise")
+    _req(coeffs, "coeffs", torch.float32); _req(step, "step", torch.int32)
+    n, c, h, w = latents.shape
+    per = latents.numel() // n
+    want = (2 * n if use_cfg else n) * per
+    if noise_pred.numel() != want or model_in.numel() != want:
+        raise IHError(f"euler_ancestral_step: noise_pred / model_in must hold {want} elements (use_cfg={use_cfg})")
+    if coeffs.dim() != 2 or coeffs.shape[1] != 8 or not coeffs.is_contiguous():
+        raise IHError("euler_ancestral_step: coeffs must be a contiguous [T, 8] table")
+    if (step_noise.dim() != 5 or tuple(step_noise.shape[1:]) != (n, c, h, w) or step_noise.shape[0] != coeffs.shape[0]
+            or not (step_noise.is_contiguous() and latents.is_contiguous())):
+        raise IHError(f"euler_ancestral_step: contiguous latents and step_noise [{coeffs.shape[0]}, {n}, {c}, {h}, {w}] "
+                      "required")
+    blend = (None, None, None, None)
+    if inpaint is not None:
+        image_latents, noise, mask, blend_end = inpaint
+        _req(image_latents, "image_latents"); _req(noise, "noise"); _req(mask, "mask")
+        _req(blend_end, "blend_end", torch.int32)
+        if (c != 4 or tuple(image_latents.shape) != (n, 4, h, w) or tuple(noise.shape) != (n, 4, h, w)
+                or tuple(mask.shape) != (n, 1, h, w)
+                or not all(t.is_contiguous() for t in (image_latents, noise, mask))):
+            raise IHError(f"euler_ancestral_step: contiguous image_latents / noise [{n}, 4, {h}, {w}] and mask "
+                          f"[{n}, 1, {h}, {w}] required")
+        blend = (image_latents.data_ptr(), noise.data_ptr(), mask.data_ptr(), blend_end.data_ptr())
+    check(lib.ih_euler_ancestral_step(noise_pred.data_ptr(), latents.data_ptr(), model_in.data_ptr(),
+                                      coeffs.data_ptr(), step_noise.data_ptr(), step.data_ptr(), float(guidance),
+                                      float(guidance_rescale), per, n, int(use_cfg), *blend, _stream()),
+          "ih_euler_ancestral_step")
+
+
+def euler_ancestral_scale_input(latents: torch.Tensor, model_in: torch.Tensor, coeffs: torch.Tensor,
+                                step: torch.Tensor, duplicate: bool = True) -> None:
+    """The first model input of an Euler Ancestral loop: latents * coeffs[step, 6] (the fp32 reciprocal of
+    sqrt(sigma^2 + 1)), rounded to fp16 as ATen rounds diffusers' scale_model_input."""
+    lib = _lib.load()
+    _req(latents, "latents"); _req(model_in, "model_in"); _req(coeffs, "coeffs", torch.float32)
+    _req(step, "step", torch.int32)
+    if model_in.numel() != (2 if duplicate else 1) * latents.numel():
+        raise IHError("euler_ancestral_scale_input: model_in must hold the CFG pair (duplicate=True) or one copy")
+    if coeffs.dim() != 2 or coeffs.shape[1] != 8 or not coeffs.is_contiguous():
+        raise IHError("euler_ancestral_scale_input: coeffs must be a contiguous [T, 8] table")
+    check(lib.ih_euler_ancestral_scale_input(latents.data_ptr(), model_in.data_ptr(), coeffs.data_ptr(),
+                                             step.data_ptr(), latents.numel(), int(duplicate), _stream()),
+          "ih_euler_ancestral_scale_input")
 
 
 def scale_model_input(latents: torch.Tensor, model_in: torch.Tensor, sigmas: torch.Tensor, step: torch.Tensor,

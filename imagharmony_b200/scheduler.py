@@ -1,5 +1,6 @@
 """EulerDiscreteScheduler tables for the SDXL-base scheduler_config ([3P] diffusers==0.30.0; the reference calls
-set_timesteps / init_noise_sigma / scale_model_input / step at custom_pipelines.py:250,268,334,357), and the tables of
+set_timesteps / init_noise_sigma / scale_model_input / step at custom_pipelines.py:250,268,334,357), the tables of
+EulerAncestralDiscreteScheduler (Euler's, plus a per-step coefficient table; SURVEY A.6) and of
 DPMSolverMultistepScheduler (DPM-Solver++ 2M, optionally with Karras sigmas; SURVEY A.5).
 
 Only the host-side schedule lives here; the per-step arithmetic (scale_model_input, CFG combine, Euler update) is the
@@ -91,6 +92,91 @@ class EulerDiscreteScheduler:
         return self.schedule.init_noise_sigma
 
 
+class _FromConfig:
+    """diffusers' `<Scheduler>.from_config(config, **overrides)` for a scheduler that implements one configuration:
+    the keys of another scheduler's config that this one does not know are ignored, as in diffusers; an override keyword
+    it does not know, or a FIXED field at another value, raises IHError.  PARAMS go to the constructor; NO_EFFECT
+    fields are accepted and unused."""
+
+    FIXED: Mapping[str, Any] = {}
+    NO_EFFECT: tuple = ()
+    PARAMS: tuple = ()
+
+    @classmethod
+    def from_config(cls, config: Mapping[str, Any], **overrides):
+        name = cls.__name__
+        unknown = [k for k in overrides if k not in cls.PARAMS and k not in cls.FIXED and k not in cls.NO_EFFECT]
+        if unknown:
+            raise IHError(f"{name} does not know {unknown}")
+        merged = {**dict(config), **overrides}
+        bad = {k: merged[k] for k, v in cls.FIXED.items() if k in merged and merged[k] != v}
+        if bad:
+            raise IHError(f"{name} implements {({k: cls.FIXED[k] for k in bad})} only, got {bad}")
+        return cls(**{k: merged[k] for k in cls.PARAMS if k in merged})
+
+
+@dataclass
+class EulerAncestralSchedule(EulerSchedule):
+    coeffs: np.ndarray = None    # float32 [T, EULER_A_COEFFS], the per-step scalars of ih_euler_ancestral_step
+
+
+EULER_A_COEFFS = 8   # IH_EULER_A_COEFFS: sigma, 1/sigma, dt, sigma_up, 1/den(next), fp16(next sigma), 1/den(sigma), (pad)
+
+
+class EulerAncestralDiscreteScheduler(_FromConfig, EulerDiscreteScheduler):
+    """Euler Ancestral ([3P] diffusers==0.30.0 EulerAncestralDiscreteScheduler with the SDXL-base config: epsilon
+    prediction, 'leading' spacing, steps_offset 1).  Restated from the published sources (SURVEY A.6, C.28-C.31);
+    parity is unpinned.
+
+    Timesteps, sigmas, init_noise_sigma, scale_model_input and add_noise are Euler's (inherited); only the step differs:
+    it moves to sigma_down and adds fresh Gaussian noise times sigma_up, drawn from the pipeline's generator at every
+    step.  `set_timesteps` evaluates the per-step scalars with torch fp32 0-dim arithmetic, written as diffusers writes
+    it, into `coeffs` (see ih_euler_ancestral_step in include/ih_api.h for the columns)."""
+
+    order = 1
+    kind = "euler_a"
+
+    # fields whose other values change the result and have no native implementation (a config asking for Karras sigmas,
+    # e.g. a DPM-Solver++ Karras config, is refused rather than silently run with Euler's spacing)
+    FIXED = {"beta_schedule": "scaled_linear", "prediction_type": "epsilon", "timestep_spacing": "leading",
+             "trained_betas": None, "rescale_betas_zero_snr": False, "use_karras_sigmas": False}
+    PARAMS = ("num_train_timesteps", "beta_start", "beta_end", "steps_offset")
+
+    def __init__(self, num_train_timesteps: int = 1000, beta_start: float = 0.00085, beta_end: float = 0.012,
+                 steps_offset: int = 1):
+        super().__init__(num_train_timesteps, beta_start, beta_end, steps_offset)
+        self._config = MappingProxyType({
+            "_class_name": "EulerAncestralDiscreteScheduler", "num_train_timesteps": num_train_timesteps,
+            "beta_start": beta_start, "beta_end": beta_end, "steps_offset": steps_offset, **self.FIXED})
+
+    def set_timesteps(self, num_inference_steps: int, device=None) -> EulerAncestralSchedule:
+        s = super().set_timesteps(num_inference_steps, device)
+        self.schedule = EulerAncestralSchedule(s.timesteps, s.sigmas, s.init_noise_sigma, self._coefficients(s.sigmas))
+        return self.schedule
+
+    @staticmethod
+    def _coefficients(sigmas: np.ndarray) -> np.ndarray:
+        """Row i: the scalars step() and scale_model_input use at schedule index i, each a torch fp32 0-dim tensor
+        evaluated as diffusers writes it (the sigmas live on the CPU).  The reciprocals are what ATen multiplies by when
+        it divides a CUDA tensor by a 0-dim CPU tensor."""
+        sig = torch.from_numpy(sigmas)
+        T = len(sigmas) - 1
+        out = np.zeros((T, EULER_A_COEFFS), dtype=np.float32)
+        for i in range(T):
+            sigma_from, sigma_to = sig[i], sig[i + 1]
+            sigma_up = (sigma_to**2 * (sigma_from**2 - sigma_to**2) / sigma_from**2) ** 0.5
+            sigma_down = (sigma_to**2 - sigma_up**2) ** 0.5
+            dt = sigma_down - sigma_from
+            row = (sigma_from, 1.0 / sigma_from, dt, sigma_up, 1.0 / ((sigma_to**2 + 1) ** 0.5),
+                   sigma_to.half().float(), 1.0 / ((sigma_from**2 + 1) ** 0.5))
+            out[i, :7] = [float(v) for v in row]
+        return out
+
+    @property
+    def coeffs(self):
+        return self.schedule.coeffs
+
+
 @dataclass
 class DPMSchedule:
     timesteps: np.ndarray        # int64 [T]
@@ -109,7 +195,7 @@ def _sigma_to_alpha_sigma_t(sigma: torch.Tensor):
     return alpha_t, sigma_t
 
 
-class DPMSolverMultistepScheduler:
+class DPMSolverMultistepScheduler(_FromConfig):
     """DPM-Solver++ 2M ([3P] diffusers==0.30.0 DPMSolverMultistepScheduler with the SDXL-base config: dpmsolver++,
     solver_order 2, midpoint, epsilon prediction, 'leading' spacing, steps_offset 1, final sigma 0), with or without
     Karras sigmas.  Restated from the published sources (SURVEY A.5, C.22-C.27); parity is unpinned.
@@ -146,20 +232,6 @@ class DPMSolverMultistepScheduler:
             "beta_start": beta_start, "beta_end": beta_end, "steps_offset": steps_offset,
             "use_karras_sigmas": self.use_karras_sigmas, "lower_order_final": True, "euler_at_final": False,
             **self.FIXED})
-
-    @classmethod
-    def from_config(cls, config: Mapping[str, Any], **overrides) -> "DPMSolverMultistepScheduler":
-        """diffusers' `DPMSolverMultistepScheduler.from_config(config, **overrides)`: the keys of another scheduler's
-        config that this one does not know are ignored, as in diffusers; an override keyword it does not know, or a
-        FIXED field at another value, raises IHError."""
-        unknown = [k for k in overrides if k not in cls.PARAMS and k not in cls.FIXED and k not in cls.NO_EFFECT]
-        if unknown:
-            raise IHError(f"DPMSolverMultistepScheduler does not know {unknown}")
-        merged = {**dict(config), **overrides}
-        bad = {k: merged[k] for k, v in cls.FIXED.items() if k in merged and merged[k] != v}
-        if bad:
-            raise IHError(f"DPMSolverMultistepScheduler implements {({k: cls.FIXED[k] for k in bad})} only, got {bad}")
-        return cls(**{k: merged[k] for k in cls.PARAMS if k in merged})
 
     @property
     def config(self) -> Mapping[str, Any]:

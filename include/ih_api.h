@@ -276,6 +276,26 @@ int ih_dpm_solver_step(const void* noise_pred, void* latents, void* model_in, vo
                        void* step, const void* loop_begin, float guidance, float guidance_rescale, long long n_per_image,
                        int n_images, int use_cfg, void* stream);
 
+/* Euler Ancestral transition ([3P] diffusers EulerAncestralDiscreteScheduler, epsilon prediction) with the use_cfg /
+ * guidance_rescale options and CFG rounding points of ih_euler_step_ex.  Step i = *step reads row i of coeffs, fp32
+ * [T, IH_EULER_A_COEFFS] computed on the host:
+ *   {sigma_i, 1/sigma_i, dt = sigma_down - sigma_i, sigma_up, 1/sqrt(sigma_{i+1}^2 + 1), fp16(sigma_{i+1}),
+ *    1/sqrt(sigma_i^2 + 1), 0}
+ * and row i of step_noise, fp16 [T, n, 4, H, W] drawn by the caller.  With eps the guided prediction, x the latents:
+ *   x0 = x - fp16(sigma*eps);  x <- fp16(fp32(fp32((x - x0) * (1/sigma)) * dt) + x + fp16(noise * sigma_up))
+ * (fp32 sums left to right).  With image_latents, blend_noise, mask and blend_end (all or none) the inpainting blend of
+ * ih_euler_inpaint_step follows, re-noising with fp16(sigma_{i+1}).  Writes latents and
+ * model_in <- fp16(x * (1/sqrt(sigma_{i+1}^2 + 1))) (duplicated with CFG); step counter i += 1. */
+#define IH_EULER_A_COEFFS 8
+int ih_euler_ancestral_step(const void* noise_pred, void* latents, void* model_in, const void* coeffs,
+                            const void* step_noise, void* step, float guidance, float guidance_rescale,
+                            long long n_per_image, int n_images, int use_cfg, const void* image_latents,
+                            const void* blend_noise, const void* mask, const void* blend_end, void* stream);
+/* The first model input of an Euler Ancestral loop in the same convention: model_in = fp16(latents * coeffs[*step, 6])
+ * (duplicated when duplicate != 0), i.e. diffusers' scale_model_input as ATen evaluates it. */
+int ih_euler_ancestral_scale_input(const void* latents, void* model_in, const void* coeffs, const void* step,
+                                   long long total, int duplicate, void* stream);
+
 /* model_in = cat([latents, latents]) / sqrt(sigma[*step]^2 + 1)   (custom_pipelines.py:332-334, first step). */
 int ih_scale_model_input(const void* latents, void* model_in, const void* sigmas, const void* step, long long total,
                          void* stream);

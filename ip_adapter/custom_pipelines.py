@@ -8,7 +8,9 @@ a dependency here, so the pieces the reference touches are provided directly:
 Denoise loop semantics follow custom_pipelines.py:188-363 (CFG batch [negative, positive], per-step IP-scale gating
 by control_guidance_start/end, Euler update); the loop itself runs as replayed CUDA graphs (imagharmony_b200/denoise.py).
 Text-to-image also runs DPM-Solver++ 2M: pass `scheduler=DPMSolverMultistepScheduler.from_config(pipe.scheduler.config,
-use_karras_sigmas=True)` or assign it to `pipe.scheduler`, as with diffusers.
+use_karras_sigmas=True)` or assign it to `pipe.scheduler`, as with diffusers.  Text-to-image, image-to-image and
+inpainting run Euler Ancestral (`EulerAncestralDiscreteScheduler.from_config(pipe.scheduler.config)`), whose per-step
+noise comes from the call's `generator` in diffusers' order.
 VAE decode / PIL post-processing (:365-386, scope row f1) runs on the native decoder `imagharmony_b200.vae` when the
 pipeline owns one (`from_random`, or `from_pretrained` with a `vae/` folder); a `vae_decode` callable overrides it and
 `output_type="latent"` skips it.
@@ -26,7 +28,8 @@ from imagharmony_b200 import ops
 from imagharmony_b200._lib import IHError
 from imagharmony_b200.config import SDXL_BASE, UNetConfig
 from imagharmony_b200.denoise import DenoiseEngine
-from imagharmony_b200.scheduler import DPMSolverMultistepScheduler, EulerDiscreteScheduler
+from imagharmony_b200.scheduler import (DPMSolverMultistepScheduler, EulerAncestralDiscreteScheduler,
+                                        EulerDiscreteScheduler)
 from imagharmony_b200.unet import UNet2DConditionModel
 
 from .utils import is_torch2_available
@@ -258,7 +261,7 @@ class StableDiffusionXLCustomPipeline:
                                   control_guidance_start=control_guidance_start,
                                   control_guidance_end=control_guidance_end, guidance_rescale=guidance_rescale,
                                   num_loop_steps=loop_steps, callback=callback, callback_steps=callback_steps,
-                                  negative_time_ids=negative_add_time_ids)
+                                  negative_time_ids=negative_add_time_ids, generator=generator)
         else:
             out = lat.to(self.device)
         self.set_scale(conditioning_scale)
@@ -454,7 +457,8 @@ class StableDiffusionXLImg2ImgPipeline(StableDiffusionXLCustomPipeline):
         sizes = (original_size, crops_coords_top_left, target_size, negative_original_size,
                  negative_crops_coords_top_left, negative_target_size)
         out = self._denoise_from(lat, t_start, num_inference_steps, denoising_end, embeds, sizes, guidance_scale,
-                                 guidance_rescale, control_guidance_start, control_guidance_end, callback, callback_steps)
+                                 guidance_rescale, control_guidance_start, control_guidance_end, callback, callback_steps,
+                                 generator=generator)
         return self._output(out, output_type, return_dict)
 
     def _require_euler(self) -> None:
@@ -466,7 +470,7 @@ class StableDiffusionXLImg2ImgPipeline(StableDiffusionXLCustomPipeline):
 
     def _denoise_from(self, lat, t_start: int, num_inference_steps: int, denoising_end, embeds, sizes, guidance_scale,
                       guidance_rescale, control_guidance_start, control_guidance_end, callback, callback_steps,
-                      inpaint=None) -> torch.Tensor:
+                      inpaint=None, generator=None) -> torch.Tensor:
         """The loop over timesteps[t_start:], truncated by denoising_end, from the noised start latents `lat`; the
         micro-conditioning time ids are formed from `sizes` (requires_aesthetics_score = False). -> final latents."""
         batch = embeds[0].shape[0]
@@ -495,7 +499,8 @@ class StableDiffusionXLImg2ImgPipeline(StableDiffusionXLCustomPipeline):
                                   control_guidance_start=control_guidance_start,
                                   control_guidance_end=control_guidance_end, guidance_rescale=guidance_rescale,
                                   num_loop_steps=loop_end, callback=callback, callback_steps=callback_steps,
-                                  negative_time_ids=negative_add_time_ids, begin_step=t_start, inpaint=inpaint)
+                                  negative_time_ids=negative_add_time_ids, begin_step=t_start, inpaint=inpaint,
+                                  generator=generator)
         else:
             out = lat
         self.set_scale(conditioning_scale)
@@ -633,7 +638,10 @@ class StableDiffusionXLInpaintPipeline(StableDiffusionXLImg2ImgPipeline):
                              "this pipeline.")
         lat, image_latents, noise = self.prepare_inpaint_latents(pixels, batch, generator, t_start, strength == 1.0)
         # the masked image's latents only feed a 9-channel UNet: with 4 channels diffusers encodes them unused.  That
-        # encode is skipped; its posterior draw comes after the noise, so no result of this call changes
+        # encode is skipped; its posterior draw comes after the noise, so it changes only what is drawn later: the step
+        # noise of Euler Ancestral, for which the draw is made and dropped (SURVEY C.31)
+        if isinstance(self.scheduler, EulerAncestralDiscreteScheduler):
+            self._skip_masked_image_draw(max(pixels.shape[0], mask.shape[0]), height, width, generator)
         mask_lat = torch.nn.functional.interpolate(mask, size=(height // self.vae_scale_factor,
                                                                width // self.vae_scale_factor)).half()
         if batch % mask_lat.shape[0]:
@@ -643,5 +651,19 @@ class StableDiffusionXLInpaintPipeline(StableDiffusionXLImg2ImgPipeline):
                  negative_original_size, negative_crops_coords_top_left, negative_target_size)
         out = self._denoise_from(lat, t_start, num_inference_steps, denoising_end, embeds, sizes, guidance_scale,
                                  guidance_rescale, control_guidance_start, control_guidance_end, callback, callback_steps,
-                                 inpaint=(image_latents, noise, mask_lat))
+                                 inpaint=(image_latents, noise, mask_lat), generator=generator)
         return self._output(out, output_type, return_dict)
+
+    def _skip_masked_image_draw(self, n_masked: int, height: int, width: int, generator) -> None:
+        """The posterior draw of [3P] diffusers' `_encode_vae_image(masked_image, generator)` in prepare_mask_latents:
+        eps of the n_masked masked images (image * (mask < 0.5) broadcast over both batches), image i with generator[i]
+        for a list, in the dtype and on the device the image latents' eps is drawn with."""
+        L = self.vae_encoder.config.latent_channels
+        shape = (L, height // self.vae_scale_factor, width // self.vae_scale_factor)
+        dtype = torch.float32 if getattr(self.vae_encoder.config, "force_upcast", True) else torch.float16
+        if isinstance(generator, list):
+            for g in generator[:n_masked]:
+                torch.randn((1,) + shape, generator=g, device=g.device, dtype=dtype)
+        else:
+            torch.randn((n_masked,) + shape, generator=generator,
+                        device=generator.device if generator is not None else "cpu", dtype=dtype)
