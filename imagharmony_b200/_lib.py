@@ -92,6 +92,7 @@ SIGNATURES = {
     "ih_softmax_rows_f16": (c_int, [c_void_p, c_longlong, c_longlong, c_int, c_void_p]),
     "ih_softmax_rows_masked_f16": (c_int, [c_void_p, c_longlong, c_longlong, c_int, c_int, c_void_p]),
     "ih_attention_set_split_policy": (None, [c_int]),
+    "ih_attention_set_kernel": (None, [c_int]),
     "ih_attention_set_trace": (None, [c_void_p]),
     "ih_groupnorm_f16": (c_int, [c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_int,
                                  c_int, c_int, c_float, c_int, c_void_p]),

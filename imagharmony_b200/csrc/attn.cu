@@ -10,7 +10,9 @@
 // image-prompt columns [Nk - n_ip, Nk) give P = [P_t / l_t | ip_scale * P_ip / l_ip], and the single PV MMA yields
 //   softmax(q k_t^T) v_t + ip_scale * softmax(q k_ip^T) v_ip  -- attention_processor.py:423-450 (n_ip = 0: plain SDPA).
 // Longer key axes use the online softmax; the last partial wave of query tiles can be cut into KV parts whose
-// un-normalised partial results (fp32 O rows, running max, running sum) are merged by attn_combine_kernel.
+// un-normalised partial results (fp32 O rows, running max, running sum) are merged by attn_combine_kernel.  By default
+// they run on attn_ws_f16_kernel (persistent, warp-specialised, one CTA per SM: see there); attn_f16_kernel serves
+// Nk <= 128 and, through ih_attention_set_kernel(1), the long shapes too, with bit-identical whole rows.
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdlib.h>
@@ -36,13 +38,64 @@ struct AttnParams {
   float ip_scale;
   __half* out;
   long long ldo;
-  // work decomposition: a unit is 128 query rows of one (batch, head).  CTAs [0, n_whole) process a whole unit; CTA
+  // work decomposition: a unit is `rows` query rows of one (batch, head).  CTAs [0, n_whole) process a whole unit; CTA
   // n_whole + i processes KV part (i % split) of unit n_whole + i / split and writes an un-normalised partial result
   // (fp32 O rows, running max, running sum) to the workspace, merged by attn_combine_kernel.
+  int rows;      // query rows per unit: 128 (attn_f16_kernel) or ATW_ROWS (attn_ws_f16_kernel)
   int H, qtiles, n_whole, split;
-  float* ws_o;   // [slots][128][64]
-  float* ws_ml;  // [slots][128][2]
+  float* ws_o;   // [slots][rows][64]
+  float* ws_ml;  // [slots][rows][2]
+  int n_items;   // n_whole + (units - n_whole) * split
 };
+
+// Work item -> KV blocks [jb, je) of query tile q0 of (b, head); slot >= 0: a KV part written to workspace slot `slot`.
+struct AttnItem {
+  int q0, head, b, jb, je, slot;
+};
+__device__ __forceinline__ AttnItem attn_item(const AttnParams& p, int item) {
+  AttnItem w;
+  int unit = item;
+  w.jb = 0;
+  w.je = p.num_kv_blocks;
+  w.slot = -1;
+  if (unit >= p.n_whole) {
+    w.slot = unit - p.n_whole;
+    const int su = w.slot / p.split;
+    const int part = w.slot - su * p.split;
+    unit = p.n_whole + su;
+    w.jb = part * p.num_kv_blocks / p.split;          // balanced contiguous partition of the KV blocks
+    w.je = (part + 1) * p.num_kv_blocks / p.split;
+  }
+  w.q0 = (unit % p.qtiles) * p.rows;
+  w.head = (unit / p.qtiles) % p.H;
+  w.b = unit / (p.qtiles * p.H);
+  return w;
+}
+
+// Rows r0 and r0 + 8 of the item (the two rows of the thread's accumulator fragment): normalised fp16 output, or
+// for a KV part the un-normalised fp32 O rows and (running max, running sum) in the workspace.
+__device__ __forceinline__ void attn_store_rows(const AttnParams& p, const AttnItem& w, int r0, int cq,
+                                                const float (&o)[32], const float (&m_run)[2],
+                                                const float (&l_run)[2], bool single) {
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int r = r0 + 8 * h;                      // row inside the unit
+    const int qrow = w.q0 + r;
+    const float l = quad_sum(l_run[h]);
+    if (w.slot >= 0) {
+      float2* dst = reinterpret_cast<float2*>(p.ws_o + ((long long)w.slot * p.rows + r) * 64);
+#pragma unroll
+      for (int i = 0; i < 8; ++i) dst[(8 * i + cq) >> 1] = make_float2(o[4 * i + 2 * h], o[4 * i + 2 * h + 1]);
+      if (cq == 0) reinterpret_cast<float2*>(p.ws_ml)[(long long)w.slot * p.rows + r] = make_float2(m_run[h], l);
+    } else if (qrow < p.Nq) {
+      const float inv = single ? 1.f : 1.f / l;
+      __half* dst = p.out + ((long long)w.b * p.Nq + qrow) * p.ldo + w.head * 64;
+#pragma unroll
+      for (int i = 0; i < 8; ++i)
+        *reinterpret_cast<uint32_t*>(dst + 8 * i + cq) = pack_half2(o[4 * i + 2 * h] * inv, o[4 * i + 2 * h + 1] * inv);
+    }
+  }
+}
 
 __global__ void __launch_bounds__(ATT_THREADS, 2) attn_f16_kernel(const __grid_constant__ CUtensorMap tmQ,
                                                                    const __grid_constant__ CUtensorMap tmK,
@@ -60,19 +113,9 @@ __global__ void __launch_bounds__(ATT_THREADS, 2) attn_f16_kernel(const __grid_c
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  int unit = blockIdx.x, jb = 0, je = p.num_kv_blocks, slot = -1;
-  if (unit >= p.n_whole) {
-    slot = unit - p.n_whole;
-    const int su = slot / p.split;
-    const int part = slot - su * p.split;
-    unit = p.n_whole + su;
-    jb = part * p.num_kv_blocks / p.split;          // balanced contiguous partition of the KV blocks
-    je = (part + 1) * p.num_kv_blocks / p.split;
-  }
-  const int q0 = (unit % p.qtiles) * 128;
-  const int head = (unit / p.qtiles) % p.H;
-  const int b = unit / (p.qtiles * p.H);
-  const int nb = je - jb;
+  const AttnItem w = attn_item(p, blockIdx.x);
+  const int q0 = w.q0, head = w.head, b = w.b, jb = w.jb;
+  const int nb = w.je - w.jb;
 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmQ);
@@ -128,34 +171,9 @@ __global__ void __launch_bounds__(ATT_THREADS, 2) attn_f16_kernel(const __grid_c
     if (single) {
       softmax_two_segment<16>(sc, cq, valid, p.Nk - p.n_ip, p.n_ip, sl2, p.ip_scale);
     } else {
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        float mx = -INFINITY;
-#pragma unroll
-        for (int i = 0; i < 16; ++i) {
-          const int col = 8 * i + cq;
-          if (col >= valid) sc[4 * i + 2 * h] = -INFINITY;
-          if (col + 1 >= valid) sc[4 * i + 2 * h + 1] = -INFINITY;
-          mx = fmaxf(mx, fmaxf(sc[4 * i + 2 * h], sc[4 * i + 2 * h + 1]));
-        }
-        mx = quad_max(mx);
-        const float m_new = fmaxf(m_run[h], mx * sl2);
-        const float alpha = ex2_approx(m_run[h] - m_new);
-        m_run[h] = m_new;
-        float ls = 0.f;
-#pragma unroll
-        for (int i = 0; i < 16; ++i) {
-          sc[4 * i + 2 * h] = ex2_approx(fmaf(sc[4 * i + 2 * h], sl2, -m_new));
-          sc[4 * i + 2 * h + 1] = ex2_approx(fmaf(sc[4 * i + 2 * h + 1], sl2, -m_new));
-          ls += sc[4 * i + 2 * h] + sc[4 * i + 2 * h + 1];
-        }
-        l_run[h] = l_run[h] * alpha + ls;
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          o[4 * i + 2 * h] *= alpha;
-          o[4 * i + 2 * h + 1] *= alpha;
-        }
-      }
+      float alpha[2];
+      online_softmax_block<true>(sc, m_run, l_run, alpha, cq, valid, sl2);
+      online_softmax_rescale(o, alpha);
     }
     uint32_t pf[32];
     pack_p_frags<8>(sc, pf);
@@ -179,49 +197,270 @@ __global__ void __launch_bounds__(ATT_THREADS, 2) attn_f16_kernel(const __grid_c
     }
   }
 
+  attn_store_rows(p, w, wg * 64 + rw, cq, o, m_run, l_run, single);
+}
+
+// Persistent, warp-specialised kernel for the multi-block path (Nk > 128, n_ip == 0).  One CTA per SM walks the work
+// items blockIdx.x, blockIdx.x + gridDim.x, ...  Warpgroup 0 is the producer: one warp issues every TMA load (Q into a
+// 2-deep ring, K and V into an ATW_KS-deep ring with separate "full" barriers) and is the only thread that waits on
+// "empty" barriers, so it runs ahead into the next item while the current one finishes.  Warpgroups 1..ATW_CONSUMERS
+// own 64 query rows each of a unit of ATW_ROWS rows; they never wait on each other's data, only take turns issuing
+// MMAs (ping-pong, below).  Inside a warpgroup the QK^T of block j is issued before the PV of block j-1, and the
+// softmax of block j runs while that PV is still on the tensor cores; O is rescaled once it lands.
+// The per-row arithmetic (MMA shapes and k order, online_softmax_block, pack_p_frags) is that of attn_f16_kernel.
+// Three MMA warpgroups (192-row units) rather than two: at head dim 64 the softmax (MUFU ex2, fp16 packing) of a
+// block takes about as long as its MMAs, so with three warpgroups taking turns two of them have softmax work to
+// overlap each one's MMAs, and the units per (batch, head) drop by a third.  On an H100 (400 W) this was 1.33x the
+// old kernel at (2,10,4096^2) and 1.43x at (2,20,1024^2); two warpgroups gave 1.0-1.15x.
+#ifndef ATW_CONSUMERS
+#define ATW_CONSUMERS 3                                         // MMA warpgroups (64 query rows each)
+#endif
+constexpr int ATW_ROWS = 64 * ATW_CONSUMERS;                    // query rows per unit
+constexpr int ATW_THREADS = 128 * (1 + ATW_CONSUMERS);
+constexpr int ATW_KS = 4;                                       // K / V stages
+constexpr int ATW_Q_TILE = ATW_ROWS * 64 * 2;
+constexpr int ATW_SMEM_TILES = 2 * ATW_Q_TILE + ATT_TILE * 2 * ATW_KS;   // Q[2] | K[KS] | V[KS]
+// register split (multiples of 8, 64K registers per SM): the producer keeps what TMA issue needs
+constexpr int ATW_PRODUCER_REGS = ATW_CONSUMERS == 2 ? 40 : 32;
+constexpr int ATW_CONSUMER_REGS = ATW_CONSUMERS == 2 ? 232 : 160;
+static_assert(128 * ATW_PRODUCER_REGS + 128 * ATW_CONSUMERS * ATW_CONSUMER_REGS <= 65536, "register budget");
+constexpr int ATW_SMEM_BYTES = ATW_SMEM_TILES + 256 + 1024;     // + barriers + alignment slack
+
+#ifndef ATW_PINGPONG
+#define ATW_PINGPONG 1   // order the MMA warpgroups' tensor-core work (see the consumer loop)
+#endif
+
+// keep the compiler from reusing registers that an asynchronous MMA still reads
+template <int N>
+__device__ __forceinline__ void fence_regs_u32(uint32_t (&d)[N]) {
 #pragma unroll
-  for (int h = 0; h < 2; ++h) {
-    const int r = wg * 64 + rw + 8 * h;          // row inside the 128-row unit
-    const int qrow = q0 + r;
-    const float l = quad_sum(l_run[h]);
-    if (slot >= 0) {
-      float2* dst = reinterpret_cast<float2*>(p.ws_o + ((long long)slot * 128 + r) * 64);
+  for (int i = 0; i < N; ++i) asm volatile("" : "+r"(d[i])::"memory");
+}
+
+__global__ void __launch_bounds__(ATW_THREADS, 1) attn_ws_f16_kernel(const __grid_constant__ CUtensorMap tmQ,
+                                                                     const __grid_constant__ CUtensorMap tmK,
+                                                                     const __grid_constant__ CUtensorMap tmV,
+                                                                     const AttnParams p) {
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint8_t* sQ = smem;                             // [2]
+  uint8_t* sK = smem + 2 * ATW_Q_TILE;            // [KS]
+  uint8_t* sV = sK + ATW_KS * ATT_TILE;           // [KS]
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + ATW_SMEM_TILES);
+  uint64_t* q_full = bars;                        // [2]
+  uint64_t* q_empty = bars + 2;                   // [2]
+  uint64_t* k_full = bars + 4;                    // [KS]
+  uint64_t* v_full = k_full + ATW_KS;             // [KS]
+  uint64_t* kv_empty = v_full + ATW_KS;           // [KS]
+  constexpr uint32_t CONSUMER_WARPS = ATW_CONSUMERS * 4;
+
+  const int warp = threadIdx.x >> 5;
+  const int lane = threadIdx.x & 31;
+  if (threadIdx.x == 0) {
+    tma_prefetch_desc(&tmQ);
+    tma_prefetch_desc(&tmK);
+    tma_prefetch_desc(&tmV);
+    for (int s = 0; s < 2; ++s) {
+      mbar_init(&q_full[s], 1);
+      mbar_init(&q_empty[s], CONSUMER_WARPS);    // lane 0 of every MMA warp
+    }
+    for (int s = 0; s < ATW_KS; ++s) {
+      mbar_init(&k_full[s], 1);
+      mbar_init(&v_full[s], 1);
+      mbar_init(&kv_empty[s], CONSUMER_WARPS);
+    }
+    fence_barrier_init();
+  }
+  __syncthreads();
+  pdl_launch_dependents();
+  pdl_wait();
+
+  if (warp < 4) {
+    // ------------------------------ producer warpgroup ------------------------------
+    setmaxnreg_dec<ATW_PRODUCER_REGS>();
+    if (warp == 0) {
+      int s = 0, qs = 0;
+      uint32_t ph = 0, qph = 0;
+      for (int item = blockIdx.x; item < p.n_items; item += gridDim.x) {
+        const AttnItem w = attn_item(p, item);
+        mbar_wait(&q_empty[qs], qph ^ 1);
+        if (elect_one()) {
+          mbar_arrive_expect_tx(&q_full[qs], ATW_Q_TILE);
+          tma_load_3d(sQ + qs * ATW_Q_TILE, &tmQ, &q_full[qs], w.head * 64, w.q0, w.b);
+        }
+        __syncwarp();
+        if (++qs == 2) {
+          qs = 0;
+          qph ^= 1;
+        }
+        for (int j = w.jb; j < w.je; ++j) {
+          mbar_wait(&kv_empty[s], ph ^ 1);
+          if (elect_one()) {
+            mbar_arrive_expect_tx(&k_full[s], ATT_TILE);
+            tma_load_3d(sK + s * ATT_TILE, &tmK, &k_full[s], w.head * 64, j * 128, w.b);
+            mbar_arrive_expect_tx(&v_full[s], ATT_TILE);
+            tma_load_3d(sV + s * ATT_TILE, &tmV, &v_full[s], w.head * 64, j * 128, w.b);
+          }
+          __syncwarp();
+          if (++s == ATW_KS) {
+            s = 0;
+            ph ^= 1;
+          }
+        }
+      }
+    }
+    return;
+  }
+
+  // ------------------------------ MMA + softmax warpgroups ------------------------------
+  setmaxnreg_inc<ATW_CONSUMER_REGS>();
+  const int wg = (threadIdx.x >> 7) - 1;            // rows [64 wg, 64 wg + 64) of the unit
+  const int rw = ((warp & 3) << 4) + (lane >> 2);   // my rows inside the warpgroup's 64: rw, rw + 8
+  const int cq = (lane & 3) << 1;
+  const float sl2 = p.scale_log2;
+  // Ping-pong: a warpgroup issues its MMAs of a block (QK^T of block j and PV of block j - 1) only after the previous
+  // one in round-robin order has issued its own, through named barriers (1 + wg: "my turn").  The tensor cores then
+  // take the warpgroups in turn, and each one's softmax runs under the others' MMAs.  Warpgroup 0 goes first; the
+  // last warpgroup skips its very last hand-over so that every barrier phase is complete when the CTA exits.
+  auto mma_turn = [&]() {
+    if (ATW_PINGPONG) named_bar_sync(1 + wg, 2 * 128);
+  };
+  auto mma_pass = [&](bool last) {
+    if (ATW_PINGPONG && !(last && wg == ATW_CONSUMERS - 1)) named_bar_arrive(1 + (wg + 1) % ATW_CONSUMERS, 2 * 128);
+  };
+  if (ATW_PINGPONG && wg == ATW_CONSUMERS - 1) named_bar_arrive(1, 2 * 128);
+  int s = 0, qs = 0;
+  uint32_t ph = 0, qph = 0;
+  for (int item = blockIdx.x; item < p.n_items; item += gridDim.x) {
+    const AttnItem w = attn_item(p, item);
+    const int nb = w.je - w.jb;
+    const bool last_item = item + (int)gridDim.x >= p.n_items;
+    const uint64_t q_desc = wgmma_desc_sw128(smem_u32(sQ + qs * ATW_Q_TILE) + wg * (64 * 128));
+    float o[32];
 #pragma unroll
-      for (int i = 0; i < 8; ++i) dst[(8 * i + cq) >> 1] = make_float2(o[4 * i + 2 * h], o[4 * i + 2 * h + 1]);
-      if (cq == 0) reinterpret_cast<float2*>(p.ws_ml)[(long long)slot * 128 + r] = make_float2(m_run[h], l);
-    } else if (qrow < p.Nq) {
-      const float inv = single ? 1.f : 1.f / l;
-      __half* dst = p.out + ((long long)b * p.Nq + qrow) * p.ldo + head * 64;
+    for (int i = 0; i < 32; ++i) o[i] = 0.f;
+    float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f}, alpha[2];
+    float sc[64];
+    uint32_t pf[32];
+    mbar_wait(&q_full[qs], qph);
+
+    // block jb: S = Q K^T and its softmax (O is still zero: no rescale)
+    mbar_wait(&k_full[s], ph);
+    {
+      const uint64_t k_desc = wgmma_desc_sw128(smem_u32(sK + s * ATT_TILE));
+      mma_turn();
+      wgmma_fence();
 #pragma unroll
-      for (int i = 0; i < 8; ++i)
-        *reinterpret_cast<uint32_t*>(dst + 8 * i + cq) = pack_half2(o[4 * i + 2 * h] * inv, o[4 * i + 2 * h + 1] * inv);
+      for (int k = 0; k < 4; ++k) wgmma_ss<128>(sc, q_desc + 2 * k, k_desc + 2 * k, k != 0);
+      wgmma_commit();
+      mma_pass(false);
+      wgmma_wait<0>();
+      fence_regs(sc);
+    }
+    if (nb == 1) {
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&q_empty[qs]);
+    }
+    {
+      const int valid = p.Nk - w.jb * 128;
+      if (valid < 128) online_softmax_block<true>(sc, m_run, l_run, alpha, cq, valid, sl2);
+      else online_softmax_block<false>(sc, m_run, l_run, alpha, cq, valid, sl2);
+    }
+    pack_p_frags<8>(sc, pf);
+    int sp = s;                                      // stage of the block whose P V is pending
+    uint32_t php = ph;
+    if (++s == ATW_KS) {
+      s = 0;
+      ph ^= 1;
+    }
+
+    for (int j = 1; j < nb; ++j) {
+      mbar_wait(&k_full[s], ph);
+      mbar_wait(&v_full[sp], php);
+      const uint64_t k_desc = wgmma_desc_sw128(smem_u32(sK + s * ATT_TILE));
+      const uint32_t v_addr = smem_u32(sV + sp * ATT_TILE);
+      mma_turn();
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < 4; ++k) wgmma_ss<128>(sc, q_desc + 2 * k, k_desc + 2 * k, k != 0);
+      wgmma_commit();
+#pragma unroll
+      for (int kk = 0; kk < 8; ++kk)   // V: MN-major, 16 keys = 16 rows of 128 B = 2048 B per step
+        wgmma_rs<64, 1>(o, *reinterpret_cast<const uint32_t(*)[4]>(pf + 4 * kk), wgmma_desc_sw128(v_addr + kk * 2048), 1);
+      wgmma_commit();
+      mma_pass(false);
+      wgmma_wait<1>();                               // S of block j is in; P V of block j - 1 may still run
+      fence_regs(sc);
+      if (j == nb - 1) {
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&q_empty[qs]);
+      }
+      const int valid = p.Nk - (w.jb + j) * 128;
+      if (valid < 128) online_softmax_block<true>(sc, m_run, l_run, alpha, cq, valid, sl2);
+      else online_softmax_block<false>(sc, m_run, l_run, alpha, cq, valid, sl2);
+      wgmma_wait<0>();
+      fence_regs(o);
+      fence_regs_u32(pf);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&kv_empty[sp]);
+      online_softmax_rescale(o, alpha);
+      pack_p_frags<8>(sc, pf);
+      sp = s;
+      php = ph;
+      if (++s == ATW_KS) {
+        s = 0;
+        ph ^= 1;
+      }
+    }
+
+    mbar_wait(&v_full[sp], php);
+    {
+      const uint32_t v_addr = smem_u32(sV + sp * ATT_TILE);
+      mma_turn();
+      wgmma_fence();
+#pragma unroll
+      for (int kk = 0; kk < 8; ++kk)
+        wgmma_rs<64, 1>(o, *reinterpret_cast<const uint32_t(*)[4]>(pf + 4 * kk), wgmma_desc_sw128(v_addr + kk * 2048), 1);
+      wgmma_commit();
+      mma_pass(last_item);
+      wgmma_wait<0>();
+      fence_regs(o);
+      fence_regs_u32(pf);
+    }
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&kv_empty[sp]);
+    attn_store_rows(p, w, wg * 64 + rw, cq, o, m_run, l_run, false);
+    if (++qs == 2) {
+      qs = 0;
+      qph ^= 1;
     }
   }
 }
 
 // Merge the `split` KV parts of the units that attn_f16_kernel processed piecewise:
 //   M = max_i m_i,  out = sum_i O_i 2^(m_i - M) / sum_i l_i 2^(m_i - M)   (fixed order: deterministic).
-// grid = (#split units * 2), block = 256: 64 rows per block, 4 threads (16 columns each) per row.
+// grid = (#split units * rows / 64), block = 256: 64 rows per block, 4 threads (16 columns each) per row.
 __global__ void __launch_bounds__(256) attn_combine_kernel(const AttnParams p) {
   pdl_launch_dependents();
   pdl_wait();
-  const int su = blockIdx.x >> 1;
-  const int row = (blockIdx.x & 1) * 64 + (threadIdx.x >> 2);
+  const int per_unit = p.rows / 64;
+  const int su = blockIdx.x / per_unit;
+  const int row = (blockIdx.x - su * per_unit) * 64 + (threadIdx.x >> 2);
   const int c0 = (threadIdx.x & 3) * 16;
   const int unit = p.n_whole + su;
-  const int qrow = (unit % p.qtiles) * 128 + row;
+  const int qrow = (unit % p.qtiles) * p.rows + row;
   if (qrow >= p.Nq) return;
   const int head = (unit / p.qtiles) % p.H;
   const int b = unit / (p.qtiles * p.H);
   const float2* ml = reinterpret_cast<const float2*>(p.ws_ml);
   float mmax = -INFINITY;
-  for (int i = 0; i < p.split; ++i) mmax = fmaxf(mmax, ml[((long long)su * p.split + i) * 128 + row].x);
+  for (int i = 0; i < p.split; ++i) mmax = fmaxf(mmax, ml[((long long)su * p.split + i) * p.rows + row].x);
   float acc[16];
 #pragma unroll
   for (int e = 0; e < 16; ++e) acc[e] = 0.f;
   float l = 0.f;
   for (int i = 0; i < p.split; ++i) {
-    const long long wrow = ((long long)su * p.split + i) * 128 + row;
+    const long long wrow = ((long long)su * p.split + i) * p.rows + row;
     const float2 v = ml[wrow];
     const float w = ex2_approx(v.x - mmax);
     l = fmaf(v.y, w, l);
@@ -253,19 +492,27 @@ __global__ void __launch_bounds__(256) attn_combine_kernel(const AttnParams p) {
 // Cost model in KV-block iterations (an estimate, not a measurement): a part pays ATT_SPLIT_OVERHEAD iterations for
 // its partial write and the merge kernel.  Returns split (1 = none) and the number of units processed whole.
 constexpr float ATT_SPLIT_OVERHEAD = 3.0f;
-static int g_split_policy = 0;   // 0: cost model, 1: split whenever a split plan exists (tests)
+static int g_split_policy = 0;   // 0: cost model, 1: split every partial last wave of a multi-block shape (tests)
+static int g_kernel = 0;         // multi-block path: 0 = attn_ws_f16_kernel, 1 = attn_f16_kernel (tests, A/B tools)
 
-static int attn_slots() {
-  static const int slots = [] {
-    int per_sm = 0;
-    if (cudaFuncSetAttribute(attn_f16_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, ATT_SMEM_BYTES) != cudaSuccess ||
-        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, attn_f16_kernel, ATT_THREADS, ATT_SMEM_BYTES) != cudaSuccess ||
-        per_sm < 1)
-      per_sm = 1;
-    return num_sms() * per_sm;
-  }();
-  return slots;
+template <typename K>
+static int attn_resident_ctas(K kernel, int threads, int smem) {
+  int per_sm = 0;
+  if (cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) != cudaSuccess ||
+      cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, threads, smem) != cudaSuccess || per_sm < 1)
+    per_sm = 1;
+  return num_sms() * per_sm;
 }
+
+// resident CTA slots of the kernel that serves the multi-block path (also sets the shared-memory attributes once)
+static int attn_slots() {
+  static const int slots_old = attn_resident_ctas(attn_f16_kernel, ATT_THREADS, ATT_SMEM_BYTES);
+  static const int slots_ws = attn_resident_ctas(attn_ws_f16_kernel, ATW_THREADS, ATW_SMEM_BYTES);
+  return g_kernel == 1 ? slots_old : slots_ws;
+}
+
+// query rows per unit of the kernel that serves a shape (Nk > 128 is the multi-block path)
+static int attn_rows(int Nk) { return (Nk > 128 && g_kernel == 0) ? ATW_ROWS : 128; }
 
 static void attn_plan(int units, int nb, int* n_whole, int* split) {
   const int G = attn_slots();
@@ -275,7 +522,10 @@ static void attn_plan(int units, int nb, int* n_whole, int* split) {
   if (rem == 0 || nb < 2) return;
   int s = G / rem;
   if (s > nb) s = nb;
-  if (s < 2) return;
+  if (s < 2) {
+    if (g_split_policy == 0) return;
+    s = 2;   // policy 1: cut the partial wave even where its parts overflow into one more
+  }
   const float t_whole = (float)nb, t_split = (float)((nb + s - 1) / s) + ATT_SPLIT_OVERHEAD;
   if (t_split >= t_whole && g_split_policy == 0) return;
   *n_whole = units - rem;
@@ -287,16 +537,18 @@ static void attn_plan(int units, int nb, int* n_whole, int* split) {
 using namespace ih;
 
 extern "C" void ih_attention_set_split_policy(int policy) { g_split_policy = policy; }
+extern "C" void ih_attention_set_kernel(int kernel) { g_kernel = kernel == 1 ? 1 : 0; }
 // kept for ABI compatibility: the wgmma kernels record no per-block trace
 extern "C" void ih_attention_set_trace(void* device_buffer) { (void)device_buffer; }
 
 extern "C" long long ih_attention_workspace_bytes(int B, int H, int Nq, int Nk, int n_ip) {
   if (B <= 0 || H <= 0 || Nq <= 0 || Nk <= 128 || n_ip != 0) return 0;
   int n_whole, split;
-  const int units = B * H * ((Nq + 127) / 128);
+  const int rows = attn_rows(Nk);
+  const int units = B * H * ((Nq + rows - 1) / rows);
   attn_plan(units, (Nk + 127) / 128, &n_whole, &split);
   if (units == n_whole) return 0;
-  return (long long)(units - n_whole) * split * 128 * (64 + 2) * (long long)sizeof(float);
+  return (long long)(units - n_whole) * split * rows * (64 + 2) * (long long)sizeof(float);
 }
 
 extern "C" int ih_attention_f16(const void* q, long long ldq, const void* k, long long ldk, const void* v,
@@ -315,12 +567,14 @@ extern "C" int ih_attention_ws_f16(const void* q, long long ldq, const void* k, 
   IH_CHECK(n_ip >= 0 && n_ip < Nk, IH_ERR_ARG, "ih_attention_f16: n_ip out of range");
   IH_CHECK(n_ip == 0 || Nk <= 128, IH_ERR_SHAPE, "ih_attention_f16: decoupled IP path needs Nk <= 128");
 
+  const int rows = n_ip == 0 ? attn_rows(Nk) : 128;
   CUtensorMap tq, tk, tv;
   const uint32_t box[3] = {64u, 128u, 1u};
   {
     const uint64_t dims[3] = {(uint64_t)H * 64, (uint64_t)Nq, (uint64_t)B};
     const uint64_t str[2] = {(uint64_t)ldq * 2, (uint64_t)Nq * ldq * 2};
-    int rc = get_tmap_f16(&tq, q, 3, dims, str, box);
+    const uint32_t qbox[3] = {64u, (uint32_t)rows, 1u};
+    int rc = get_tmap_f16(&tq, q, 3, dims, str, qbox);
     if (rc) return rc;
   }
   {
@@ -345,25 +599,33 @@ extern "C" int ih_attention_ws_f16(const void* q, long long ldq, const void* k, 
   p.out = (__half*)out;
   p.ldo = ldo;
   p.H = H;
-  p.qtiles = (Nq + 127) / 128;
+  p.rows = rows;
+  p.qtiles = (Nq + rows - 1) / rows;
   const int units = B * H * p.qtiles;
   attn_slots();   // sets the shared-memory attribute once
   p.n_whole = units;
   p.split = 1;
   if (n_ip == 0) attn_plan(units, p.num_kv_blocks, &p.n_whole, &p.split);
   const long long slots = (long long)(units - p.n_whole) * p.split;
-  const long long need = slots * 128 * 66 * (long long)sizeof(float);
+  const long long need = slots * rows * 66 * (long long)sizeof(float);
   if (slots > 0 && (!workspace || workspace_bytes < need)) {
     p.n_whole = units;   // no (or too small a) workspace: every unit runs whole
     p.split = 1;
   }
   const int n_split_ctas = (units - p.n_whole) * p.split;
+  p.n_items = p.n_whole + n_split_ctas;
   p.ws_o = reinterpret_cast<float*>(workspace);
-  p.ws_ml = p.ws_o ? p.ws_o + (long long)n_split_ctas * 128 * 64 : nullptr;
-  IH_CUDA(launch_kernel(attn_f16_kernel, dim3(p.n_whole + n_split_ctas), dim3(ATT_THREADS), (size_t)ATT_SMEM_BYTES,
-                        (cudaStream_t)stream, tq, tk, tv, p));
+  p.ws_ml = p.ws_o ? p.ws_o + (long long)n_split_ctas * rows * 64 : nullptr;
+  if (rows != 128) {
+    const int grid = p.n_items < num_sms() ? p.n_items : num_sms();
+    IH_CUDA(launch_kernel(attn_ws_f16_kernel, dim3(grid), dim3(ATW_THREADS), (size_t)ATW_SMEM_BYTES,
+                          (cudaStream_t)stream, tq, tk, tv, p));
+  } else {
+    IH_CUDA(launch_kernel(attn_f16_kernel, dim3(p.n_items), dim3(ATT_THREADS), (size_t)ATT_SMEM_BYTES,
+                          (cudaStream_t)stream, tq, tk, tv, p));
+  }
   if (n_split_ctas > 0)
-    IH_CUDA(launch_kernel(attn_combine_kernel, dim3((units - p.n_whole) * 2), dim3(256), (size_t)0, (cudaStream_t)stream,
+    IH_CUDA(launch_kernel(attn_combine_kernel, dim3((units - p.n_whole) * (rows / 64)), dim3(256), (size_t)0, (cudaStream_t)stream,
                           p));
   return 0;
 }

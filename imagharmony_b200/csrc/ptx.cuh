@@ -296,4 +296,7 @@ __device__ __forceinline__ void tma_store_wait_read() { asm volatile("cp.async.b
 __device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
+__device__ __forceinline__ void named_bar_arrive(uint32_t id, uint32_t nthreads) {
+  asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
+}
 }  // namespace ih

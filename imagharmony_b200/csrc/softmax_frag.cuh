@@ -63,6 +63,50 @@ __device__ __forceinline__ void softmax_two_segment(float (&sc)[4 * NI], int cq,
   }
 }
 
+// Online-softmax update for one 128-key block of the two rows (h = 0, 1) a thread holds: masks the columns >= valid
+// (MASK: only the clipped last block has any), raises the running max, replaces the scores in place by
+// 2^(s sl2 - m_new) and folds their sum into the running sum.  alpha[h] is the factor the O rows must be rescaled by
+// (online_softmax_rescale); the caller applies it once no MMA into O is in flight.  Every attention kernel that walks
+// key blocks uses this one sequence of operations, so a row's result does not depend on which kernel computed it.
+template <bool MASK>
+__device__ __forceinline__ void online_softmax_block(float (&sc)[64], float (&m_run)[2], float (&l_run)[2],
+                                                     float (&alpha)[2], int cq, int valid, float sl2) {
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    float mx = -INFINITY;
+#pragma unroll
+    for (int i = 0; i < 16; ++i) {
+      const int col = 8 * i + cq;
+      if (MASK && col >= valid) sc[4 * i + 2 * h] = -INFINITY;
+      if (MASK && col + 1 >= valid) sc[4 * i + 2 * h + 1] = -INFINITY;
+      mx = fmaxf(mx, fmaxf(sc[4 * i + 2 * h], sc[4 * i + 2 * h + 1]));
+    }
+    mx = quad_max(mx);
+    const float m_new = fmaxf(m_run[h], mx * sl2);
+    alpha[h] = ex2_approx(m_run[h] - m_new);
+    m_run[h] = m_new;
+    float ls = 0.f;
+#pragma unroll
+    for (int i = 0; i < 16; ++i) {
+      sc[4 * i + 2 * h] = ex2_approx(fmaf(sc[4 * i + 2 * h], sl2, -m_new));
+      sc[4 * i + 2 * h + 1] = ex2_approx(fmaf(sc[4 * i + 2 * h + 1], sl2, -m_new));
+      ls += sc[4 * i + 2 * h] + sc[4 * i + 2 * h + 1];
+    }
+    l_run[h] = l_run[h] * alpha[h] + ls;
+  }
+}
+
+// O rows (accumulator fragment of 64 head columns) *= alpha of their row
+__device__ __forceinline__ void online_softmax_rescale(float (&o)[32], const float (&alpha)[2]) {
+#pragma unroll
+  for (int h = 0; h < 2; ++h)
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      o[4 * i + 2 * h] *= alpha[h];
+      o[4 * i + 2 * h + 1] *= alpha[h];
+    }
+}
+
 // fp32 probabilities (accumulator fragment of KS16 x 16 keys) -> fp16 A-operand fragments of KS16 k16 steps
 template <int KS16>
 __device__ __forceinline__ void pack_p_frags(const float (&sc)[8 * KS16], uint32_t (&pf)[4 * KS16]) {

@@ -126,8 +126,13 @@ int ih_xattn_q_fused_f16(const void* h, long long ldh, const void* wq, const voi
                          void* out, long long ldo, int B, int H, int Nq, int Nk, int n_ip, float ip_scale, int K,
                          void* stream);
 
-/* Test aid: 0 (default) = split only when the cost model predicts a gain, 1 = split whenever a plan exists. */
+/* Test aid: 0 (default) = split only when the cost model predicts a gain, 1 = split every partial last wave (at
+ * least 2 parts, even where they overflow into one more wave). */
 void ih_attention_set_split_policy(int policy);
+/* Test / A-B aid: the kernel of the multi-block path (Nk > 128).  0 (default) = the persistent warp-specialised
+ * kernel, 1 = the two-CTA-per-SM kernel that also serves Nk <= 128.  Rows processed whole are bit-identical between
+ * the two; the KV-split plan (and so the rows of split units) follows the selected kernel's residency. */
+void ih_attention_set_kernel(int kernel);
 /* Kept for ABI compatibility: a no-op, the attention kernels record no trace. */
 void ih_attention_set_trace(void* device_buffer);
 int ih_attention_ws_f16(const void* q, long long ldq, const void* k, long long ldk, const void* v, long long ldv,
