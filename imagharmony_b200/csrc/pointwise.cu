@@ -1420,6 +1420,7 @@ extern "C" int ih_im2col3x3_nchw_f16(const void* x_nchw, void* out, int B, int C
   return 0;
 }
 
+
 extern "C" int ih_nhwc_to_nchw_f16(const void* x, long long ldc, void* out, int B, long long HW, int C, void* stream) {
   IH_CHECK(x && out && C >= 1, IH_ERR_ARG, "ih_nhwc_to_nchw_f16: bad arguments");
   const long long total = (long long)B * C * HW;
@@ -1443,5 +1444,58 @@ extern "C" int ih_vae_posterior_noise_f16(const void* moments, long long ldc, co
   IH_CUDA(launch_kernel(vae_posterior_noise_kernel, dim3(grid_for(total, 256)), dim3(256), (size_t)0, (cudaStream_t)stream,
                         (const __half*)moments, ldc, eps, eps_f32, (const __half*)noise, (__half*)out, B, B_moments, B_eps,
                         HW, C, scaling_factor, sigma));
+  return 0;
+}
+
+namespace ih {
+
+// conv_in of the 9-channel inpainting UNet: the same patch matrix for the channel concatenation [x0 | x1] of two NCHW
+// tensors (x0 [B, C0, H, W] the per-step latents, x1 [B, C1, H, W] the static mask | masked-image latents), read from
+// the two sources directly so the 9-channel input is never materialised.  Column k = ci*9 + ky*3 + kx, ci < C0 from x0.
+__global__ void im2col3x3_nchw_cat_kernel(const __half* __restrict__ x0, int C0, const __half* __restrict__ x1, int C1,
+                                          __half* __restrict__ out, int B, int H, int W, int Kpad) {
+  pdl_launch_dependents();
+  pdl_wait();
+  const long long npix = (long long)B * H * W;
+  const int kv = Kpad >> 3;  // 16-byte vectors per row
+  const long long total = npix * kv;
+  const int kvalid = (C0 + C1) * 9;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+    const int v = (int)(i % kv);
+    const long long pix = i / kv;
+    const int xw = (int)(pix % W);
+    const int yh = (int)((pix / W) % H);
+    const int b = (int)(pix / ((long long)W * H));
+    __align__(16) __half vals[8];
+#pragma unroll
+    for (int e = 0; e < 8; ++e) {
+      const int k = v * 8 + e;
+      __half hv = __float2half_rn(0.f);
+      if (k < kvalid) {
+        const int ci = k / 9, t = k - ci * 9;
+        const int yy = yh + t / 3 - 1, xx = xw + t % 3 - 1;
+        if (yy >= 0 && yy < H && xx >= 0 && xx < W) {
+          hv = ci < C0 ? x0[(((long long)b * C0 + ci) * H + yy) * W + xx]
+                       : x1[(((long long)b * C1 + (ci - C0)) * H + yy) * W + xx];
+        }
+      }
+      vals[e] = hv;
+    }
+    *reinterpret_cast<uint4*>(out + pix * Kpad + v * 8) = *reinterpret_cast<const uint4*>(vals);
+  }
+}
+
+}  // namespace ih
+
+extern "C" int ih_im2col3x3_nchw_cat_f16(const void* x0, int C0, const void* x1, int C1, void* out, int B, int H, int W,
+                                         int Kpad, void* stream) {
+  IH_CHECK(x0 && x1 && out, IH_ERR_ARG, "ih_im2col3x3_nchw_cat_f16: null pointer");
+  IH_CHECK(B >= 1 && H >= 1 && W >= 1 && C0 >= 1 && C1 >= 1, IH_ERR_SHAPE,
+           "ih_im2col3x3_nchw_cat_f16: empty shape (B=%d, H=%d, W=%d, C0=%d, C1=%d)", B, H, W, C0, C1);
+  IH_CHECK(Kpad % 8 == 0 && Kpad >= (C0 + C1) * 9, IH_ERR_ARG,
+           "ih_im2col3x3_nchw_cat_f16: Kpad=%d must be a multiple of 8 and >= (C0 + C1) * 9 = %d", Kpad, (C0 + C1) * 9);
+  const long long total = (long long)B * H * W * (Kpad / 8);
+  IH_CUDA(launch_kernel(im2col3x3_nchw_cat_kernel, dim3(grid_for(total, 256)), dim3(256), (size_t)0,
+                        (cudaStream_t)stream, (const __half*)x0, C0, (const __half*)x1, C1, (__half*)out, B, H, W, Kpad));
   return 0;
 }

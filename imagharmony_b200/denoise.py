@@ -20,7 +20,7 @@ gives diffusers' noise (a Philox stream inside the kernel would not reproduce to
 
 Graph lifetime: a captured graph holds raw pointers.  Everything it reads lives in buffers that are owned per shape
 and never freed while the graph exists -- the engine's static inputs (`_static`, `_inpaint_static`, `_dpm_static`,
-`_ancestral_noise`), the schedule tables (`_tables`, `_coeffs`), the processors'
+`_cond_static`, `_ancestral_noise`), the schedule tables (`_tables`, `_coeffs`), the processors'
 K/V buffers and the UNet's add-embedding buffer (per-shape dicts inside those objects), and the library's grow-only
 scratch buffers whose re-allocation bumps `ops.workspace_generation()`.  A graph is replayed only if it was captured
 under the current UNet `graph_epoch` (weights / processors unchanged) and the current workspace generation; otherwise
@@ -51,6 +51,7 @@ class DenoiseEngine:
         self._static: Dict[Tuple, dict] = {}
         self._inpaint_static: Dict[Tuple, dict] = {}
         self._dpm_static: Dict[Tuple, dict] = {}
+        self._cond_static: Dict[Tuple, torch.Tensor] = {}               # 9-channel UNet: mask | masked-image latents
         self._tables: Dict[Tuple[str, int], Tuple[torch.Tensor, torch.Tensor, float]] = {}
         self._coeffs: Dict[Tuple[str, int], torch.Tensor] = {}         # DPM-Solver++ / Euler Ancestral coefficients
         self._ancestral_noise: Dict[Tuple[int, int, int, int], torch.Tensor] = {}   # Euler Ancestral step noise
@@ -94,8 +95,8 @@ class DenoiseEngine:
             dev = self.device
             b = 2 * n if use_cfg else n
             st = {
-                "latents": torch.empty((n, cfg.in_channels, h, w), dtype=torch.float16, device=dev),
-                "model_in": torch.empty((b, cfg.in_channels, h, w), dtype=torch.float16, device=dev),
+                "latents": torch.empty((n, cfg.out_channels, h, w), dtype=torch.float16, device=dev),
+                "model_in": torch.empty((b, cfg.out_channels, h, w), dtype=torch.float16, device=dev),
                 "ehs": torch.empty((b, L, cfg.cross_attention_dim), dtype=torch.float16, device=dev),
                 "text_embeds": torch.empty((b, cfg.pooled_embed_dim), dtype=torch.float16, device=dev),
                 "time_ids": torch.empty((b, 6), dtype=torch.float32, device=dev),
@@ -124,7 +125,7 @@ class DenoiseEngine:
         db = self._dpm_static.get(key)
         if db is None:
             dev = self.device
-            db = {"prev_x0": torch.empty((n, self.unet.config.in_channels, h, w), dtype=torch.float16, device=dev),
+            db = {"prev_x0": torch.empty((n, self.unet.config.out_channels, h, w), dtype=torch.float16, device=dev),
                   "loop_begin": torch.zeros((1,), dtype=torch.int32, device=dev)}
             self._dpm_static[key] = db
         return db
@@ -135,8 +136,20 @@ class DenoiseEngine:
         key = (n, h, w, T)
         buf = self._ancestral_noise.get(key)
         if buf is None:
-            buf = torch.zeros((T, n, self.unet.config.in_channels, h, w), dtype=torch.float16, device=self.device)
+            buf = torch.zeros((T, n, self.unet.config.out_channels, h, w), dtype=torch.float16, device=self.device)
             self._ancestral_noise[key] = buf
+        return buf
+
+    def _cond_buffer(self, n: int, h: int, w: int, use_cfg: bool) -> torch.Tensor:
+        """The 9-channel UNet's extra input [b, C_in - C_lat, h, w] (mask | masked-image latents, both CFG halves) per
+        (n, h, w, use_cfg), never freed (the graph-lifetime rule above)."""
+        key = (n, h, w, use_cfg)
+        buf = self._cond_static.get(key)
+        if buf is None:
+            cfg = self.unet.config
+            buf = torch.empty((2 * n if use_cfg else n, cfg.in_channels - cfg.out_channels, h, w), dtype=torch.float16,
+                              device=self.device)
+            self._cond_static[key] = buf
         return buf
 
     def _draw_ancestral_noise(self, buf: torch.Tensor, generator, begin: int, end: int) -> None:
@@ -167,8 +180,9 @@ class DenoiseEngine:
         if use_cfg:
             st["model_in"][n:].copy_(st["latents"])
 
-    def _step(self, st, timesteps, sigmas, guidance, use_cfg=True, rescale=0.0, ib=None, dpm=None, anc=None):
-        noise = self.unet(st["model_in"], timesteps, st["ehs"], st["text_embeds"], st["time_ids"], step=st["step"])
+    def _step(self, st, timesteps, sigmas, guidance, use_cfg=True, rescale=0.0, ib=None, dpm=None, anc=None, cond=None):
+        noise = self.unet(st["model_in"], timesteps, st["ehs"], st["text_embeds"], st["time_ids"], step=st["step"],
+                          cond=cond)
         if dpm is not None:
             db, coeffs = dpm
             ops.dpm_solver_step(noise, st["latents"], st["model_in"], db["prev_x0"], coeffs, st["step"],
@@ -195,7 +209,8 @@ class DenoiseEngine:
             callback: Optional[Callable] = None, callback_steps: int = 1,
             negative_time_ids: Optional[torch.Tensor] = None, begin_step: int = 0,
             inpaint: Optional[Tuple[torch.Tensor, torch.Tensor, torch.Tensor]] = None,
-            generator: Optional[Union[torch.Generator, List[torch.Generator]]] = None) -> torch.Tensor:
+            generator: Optional[Union[torch.Generator, List[torch.Generator]]] = None,
+            unet_cond: Optional[Tuple[torch.Tensor, torch.Tensor]] = None) -> torch.Tensor:
         """latents [n,4,h,w] (already scaled by init_noise_sigma; host or device); embeds host or device tensors.
         Returns the latents after the last executed step as a new device tensor.
 
@@ -223,6 +238,14 @@ class DenoiseEngine:
         text-to-image loops, with every option above except begin_step, inpaint, start_step and stop_after (IHError):
         they would need the VP-form add_noise, or the history of another call.
 
+        `unet_cond` = (mask [n,1,h,w], masked_image_latents [n,4,h,w]) is inpainting with the 9-channel inpainting UNet
+        ([3P] StableDiffusionXLInpaintPipeline with unet.config.in_channels == 9): every step's UNet input is the scaled
+        latents followed by the mask and the masked-image latents (their CFG halves equal), and there is no blend.  It
+        is required exactly when the UNet has 9 input channels.  It composes with begin_step, num_loop_steps and the
+        other loop options, not with inpaint, start_step or stop_after (IHError).  The two tensors are copied once per
+        call into a static buffer that the UNet's conv_in reads next to the step's latents (ops.im2col3x3_nchw_cat), so
+        the step kernels are those of text-to-image.
+
         With an EulerAncestralDiscreteScheduler every option above works.  `generator` (a torch.Generator, a list of
         one per image, or None for the device's default generator) supplies the Gaussian noise of every step; before
         the steps run, the noise of exactly the steps this call executes is drawn from it, one draw per step in step
@@ -233,9 +256,16 @@ class DenoiseEngine:
             raise IHError("classifier-free guidance needs negative_prompt_embeds / negative_pooled")
         is_dpm = isinstance(self.scheduler, DPMSolverMultistepScheduler)         # the one scheduler dispatch
         is_ancestral = isinstance(self.scheduler, EulerAncestralDiscreteScheduler)
-        if is_dpm and (begin_step or inpaint is not None or start_step or stop_after is not None):
+        if is_dpm and (begin_step or inpaint is not None or unet_cond is not None or start_step
+                       or stop_after is not None):
             raise IHError("DPMSolverMultistepScheduler runs whole text-to-image loops: begin_step (image-to-image), "
-                          "inpaint, start_step and stop_after need EulerDiscreteScheduler")
+                          "inpaint, unet_cond, start_step and stop_after need EulerDiscreteScheduler")
+        ucfg = self.unet.config
+        if (unet_cond is not None) != (ucfg.in_channels != ucfg.out_channels):
+            raise IHError(f"unet_cond (mask, masked_image_latents) is required exactly for the 9-channel inpainting "
+                          f"UNet; this UNet has {ucfg.in_channels} input channels")
+        if unet_cond is not None and (inpaint is not None or start_step or stop_after is not None):
+            raise IHError("unet_cond cannot be combined with inpaint / start_step / stop_after")
         n, _, h, w = latents.shape
         if is_ancestral and isinstance(generator, list) and len(generator) != n:
             raise IHError(f"got {len(generator)} generators for a batch of {n}")
@@ -276,6 +306,17 @@ class DenoiseEngine:
                     raise IHError(f"inpaint {name}: expected shape {tuple(ib[name].shape)}, got {tuple(t.shape)}")
                 ib[name].copy_(t, non_blocking=True)
             ib["blend_end"].fill_(loop_T)
+        cond = None
+        if unet_cond is not None:
+            cond = self._cond_buffer(n, h, w, use_cfg)
+            mask, masked = unet_cond
+            want = ((n, 1, h, w), (n, cond.shape[1] - 1, h, w))
+            if (tuple(mask.shape), tuple(masked.shape)) != want:
+                raise IHError(f"unet_cond: expected mask {want[0]} and masked_image_latents {want[1]}, got "
+                              f"{tuple(mask.shape)} and {tuple(masked.shape)}")
+            for half in ((0, n), (n, 2 * n)) if use_cfg else ((0, n),):     # [3P] cat([mask] * 2) under CFG
+                cond[half[0]:half[1], :1].copy_(mask, non_blocking=True)
+                cond[half[0]:half[1], 1:].copy_(masked, non_blocking=True)
         if not 0 <= start_step <= loop_T:
             raise IHError(f"start_step {start_step} outside the {loop_T}-step loop")
         if begin_step:
@@ -299,7 +340,8 @@ class DenoiseEngine:
             return 0.0 if off else float(ip_scale)
 
         def gkey(scale: float):
-            return (n, h, w, L, T, use_cfg, float(guidance_scale), rescale, scale, self.scheduler.kind, ib is not None)
+            return (n, h, w, L, T, use_cfg, float(guidance_scale), rescale, scale, self.scheduler.kind, cond is not None,
+                    ib is not None)
 
         if self.use_cuda_graph:
             if self._epoch != getattr(self.unet, "graph_epoch", 0):       # weights / processors changed since capture
@@ -314,7 +356,7 @@ class DenoiseEngine:
                     break
                 for sc in missing:
                     self.set_scale(sc)
-                    g = self._capture(st, timesteps, sigmas, guidance_scale, use_cfg, rescale, ib, dpm, anc)
+                    g = self._capture(st, timesteps, sigmas, guidance_scale, use_cfg, rescale, ib, dpm, anc, cond)
                     self._graphs[gkey(sc)] = (g, ops.workspace_generation())
                     captured = True
             else:
@@ -332,27 +374,28 @@ class DenoiseEngine:
                 self._graphs[gkey(sc)][0].replay()
             else:
                 self.set_scale(sc)
-                self._step(st, timesteps, sigmas, guidance_scale, use_cfg, rescale, ib, dpm, anc)
+                self._step(st, timesteps, sigmas, guidance_scale, use_cfg, rescale, ib, dpm, anc, cond)
             if callback is not None and (i - b0) % callback_steps == 0:           # :359-363 (Euler: order 1, no warm-up)
                 callback(i - b0, timesteps[i], st["latents"])
         self.set_scale(ip_scale)
         return st["latents"].clone()
 
-    def _capture(self, st, timesteps, sigmas, guidance, use_cfg=True, rescale=0.0, ib=None, dpm=None, anc=None):
+    def _capture(self, st, timesteps, sigmas, guidance, use_cfg=True, rescale=0.0, ib=None, dpm=None, anc=None,
+                 cond=None):
         # warm-up on a side stream (sets kernel attributes, fills the TMA descriptor cache, sizes the allocator and
         # the library's scratch buffers)
         side = torch.cuda.Stream(device=self.device)
         side.wait_stream(torch.cuda.current_stream())
         with torch.cuda.stream(side):
             st["step"].zero_()
-            self._step(st, timesteps, sigmas, guidance, use_cfg, rescale, ib, dpm, anc)
+            self._step(st, timesteps, sigmas, guidance, use_cfg, rescale, ib, dpm, anc, cond)
         torch.cuda.current_stream().wait_stream(side)
         torch.cuda.synchronize()
         st["step"].zero_()
         g = torch.cuda.CUDAGraph()
         before = ops.launch_count()
         with torch.cuda.graph(g):
-            self._step(st, timesteps, sigmas, guidance, use_cfg, rescale, ib, dpm, anc)
+            self._step(st, timesteps, sigmas, guidance, use_cfg, rescale, ib, dpm, anc, cond)
         self.last_launches_per_step = ops.launch_count() - before
         self.graphs_captured += 1
         return g

@@ -556,6 +556,22 @@ def im2col3x3_nchw(x_nchw: torch.Tensor, kpad: int = 64, out: Optional[torch.Ten
     return out
 
 
+def im2col3x3_nchw_cat(x0: torch.Tensor, x1: torch.Tensor, kpad: int, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """im2col3x3_nchw of torch.cat([x0, x1], 1) without forming the concatenation: x0 [B, C0, H, W], x1 [B, C1, H, W]
+    -> A [B*H*W, kpad] (conv_in of the 9-channel inpainting UNet: latents | mask | masked-image latents)."""
+    lib = _lib.load()
+    _req(x0, "x0")
+    _req(x1, "x1")
+    B, C0, H, W = x0.shape
+    if x1.dim() != 4 or x1.shape[0] != B or tuple(x1.shape[2:]) != (H, W):
+        raise IHError(f"im2col3x3_nchw_cat: x1 {tuple(x1.shape)} does not match x0 {tuple(x0.shape)}")
+    if out is None:
+        out = torch.empty((B * H * W, kpad), dtype=torch.float16, device=x0.device)
+    check(lib.ih_im2col3x3_nchw_cat_f16(x0.data_ptr(), C0, x1.data_ptr(), x1.shape[1], out.data_ptr(), B, H, W, kpad,
+                                        _stream()), "ih_im2col3x3_nchw_cat_f16")
+    return out
+
+
 def softmax_rows_masked_(x: torch.Tensor, valid_cols: int) -> torch.Tensor:
     """softmax_rows_ over the first `valid_cols` columns of each row; the remaining (padding) columns become 0."""
     lib = _lib.load()

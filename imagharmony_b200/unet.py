@@ -324,6 +324,9 @@ class UNet2DConditionModel(nn.Module):
 
     def __init__(self, cfg: UNetConfig):
         super().__init__()
+        if cfg.in_channels not in (4, 9):
+            raise IHError(f"UNet2DConditionModel: in_channels must be 4 (latents) or 9 (inpainting: latents | mask | "
+                          f"masked-image latents), got {cfg.in_channels}")
         self.config = cfg
         boc = cfg.block_out_channels
         tl = cfg.transformer_layers_per_block
@@ -429,10 +432,14 @@ class UNet2DConditionModel(nn.Module):
         self._w_temb = torch.cat(ws, 0).contiguous()
         self._b_temb = torch.cat(bs, 0).contiguous()
         # the 4-channel ends run on the tensor-core GEMM: conv_in weight flattened [320, 36] -> [320, 64] (zero pad);
-        # conv_out weight tap-major with Cout padded 4 -> 16
+        # conv_out weight tap-major with Cout padded 4 -> 16.  The 9-channel inpainting conv_in pads 81 -> 128: two
+        # whole 64-wide K blocks, like every other GEMM caller (none runs a partial K block)
         w_in = self.conv_in.weight.detach()
         co, ci = w_in.shape[0], w_in.shape[1]
-        self._w_in = torch.zeros((co, 64), dtype=w_in.dtype, device=w_in.device)
+        if ci != self.config.in_channels:
+            raise IHError(f"UNet2DConditionModel: config.in_channels = {self.config.in_channels} but conv_in.weight has "
+                          f"{ci} input channels")
+        self._w_in = torch.zeros((co, 64 if ci == 4 else 128), dtype=w_in.dtype, device=w_in.device)
         self._w_in[:, : ci * 9] = w_in.reshape(co, ci * 9)
         w_out = ops.pack_conv3x3_weight(self.conv_out.weight.detach())            # [4, 9*320]
         self._w_out = torch.zeros((16, w_out.shape[1]), dtype=w_out.dtype, device=w_out.device)
@@ -491,12 +498,21 @@ class UNet2DConditionModel(nn.Module):
 
     def forward(self, sample: torch.Tensor, timesteps: torch.Tensor, encoder_hidden_states: torch.Tensor,
                 text_embeds: Optional[torch.Tensor] = None, time_ids: Optional[torch.Tensor] = None,
-                step: Optional[torch.Tensor] = None) -> torch.Tensor:
+                step: Optional[torch.Tensor] = None, cond: Optional[torch.Tensor] = None) -> torch.Tensor:
         """sample NCHW fp16 [B,4,H,W]; timesteps fp32 device tensor ([B] values, or the whole schedule when `step`
-        -- a device int32 index -- is given); returns noise prediction NCHW fp16."""
+        -- a device int32 index -- is given); returns noise prediction NCHW fp16.  The 9-channel inpainting UNet also
+        takes `cond` NCHW fp16 [B,5,H,W] (mask | masked-image latents), which conv_in reads after the 4 latent channels;
+        the 4-channel UNet takes no `cond`."""
         if self._w_temb is None:
             raise IHError("UNet2DConditionModel.finalize() has not been called")
         B = sample.shape[0]
+        n_cond = self.config.in_channels - sample.shape[1]
+        if n_cond == 0 and cond is not None:
+            raise IHError(f"UNet2DConditionModel: `sample` already has all {self.config.in_channels} input channels; "
+                          "`cond` must be None")
+        if n_cond > 0 and (cond is None or tuple(cond.shape) != (B, n_cond) + tuple(sample.shape[2:])):
+            raise IHError(f"UNet2DConditionModel: the {self.config.in_channels}-channel UNet needs `cond` of shape "
+                          f"{(B, n_cond) + tuple(sample.shape[2:])}, got {None if cond is None else tuple(cond.shape)}")
         key = None if text_embeds is None else self._aug_key(text_embeds, time_ids, B)
         if self._aug is None or (key is not None and self._aug[0] != key):
             if text_embeds is None:
@@ -504,7 +520,9 @@ class UNet2DConditionModel(nn.Module):
             self.prepare_conditioning(encoder_hidden_states, text_embeds, time_ids)
         temb_all = self.time_embeddings(timesteps, step, B)
         Bs, _, Hs, Ws = sample.shape
-        x = ops.linear(ops.im2col3x3_nchw(sample, 64), self._w_in, self.conv_in.bias).reshape(Bs, Hs, Ws, -1)
+        kpad = self._w_in.shape[1]
+        a = ops.im2col3x3_nchw(sample, kpad) if cond is None else ops.im2col3x3_nchw_cat(sample, cond, kpad)
+        x = ops.linear(a, self._w_in, self.conv_in.bias).reshape(Bs, Hs, Ws, -1)
         skips = [x]
         ehs = encoder_hidden_states
         for blk in self.down_blocks:

@@ -199,6 +199,11 @@ int ih_conv_out_f16(const void* x, const void* w, const void* bias, void* out_nc
 /* conv_in on the tensor-core GEMM: im2col of the NCHW latent into A [B*H*W, Kpad] (k = ci*9 + ky*3 + kx, zero padded),
  * to be multiplied with the OIHW weight flattened (and zero padded) to [Cout, Kpad] by ih_gemm_f16. */
 int ih_im2col3x3_nchw_f16(const void* x_nchw, void* out, int B, int Cin, int H, int W, int Kpad, void* stream);
+/* The same patch matrix for the channel concatenation of x0 [B,C0,H,W] and x1 [B,C1,H,W] (NCHW fp16) without forming it:
+ * column k = ci*9 + ky*3 + kx reads x0 for ci < C0 and x1 channel ci - C0 otherwise (conv_in of the 9-channel
+ * inpainting UNet: latents | mask | masked-image latents).  Kpad % 8 == 0 and Kpad >= (C0 + C1) * 9. */
+int ih_im2col3x3_nchw_cat_f16(const void* x0, int C0, const void* x1, int C1, void* out, int B, int H, int W, int Kpad,
+                              void* stream);
 /* conv_out on ih_conv2d_f16 with Cout padded to 16: gather NHWC [B, HW, ldc] channels [0, C) into NCHW [B, C, HW]. */
 int ih_nhwc_to_nchw_f16(const void* x, long long ldc, void* out, int B, long long HW, int C, void* stream);
 

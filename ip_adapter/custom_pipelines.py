@@ -98,14 +98,15 @@ class StableDiffusionXLCustomPipeline:
 
     @classmethod
     def from_pretrained(cls, path: str, torch_dtype=torch.float16, add_watermarker: bool = False, device="cuda",
-                        cfg: UNetConfig = SDXL_BASE, vae_cfg=None, **kwargs):
+                        cfg: Optional[UNetConfig] = None, vae_cfg=None, **kwargs):
         """test.py:68-72.  Loads `<path>/unet/diffusion_pytorch_model.safetensors` (diffusers key names are the native
-        UNet's key names, so no key map is needed)."""
+        UNet's key names, so no key map is needed).  Without `cfg` the UNet is SDXL-base with the input channel count
+        of the checkpoint's conv_in (4, or 9 for the inpainting UNet)."""
         unet, enc, vae, _, _ = cls._load_pretrained(path, torch_dtype, device, cfg, vae_cfg)
         return cls(unet, prompt_encoder=enc, vae=vae)
 
     @staticmethod
-    def _load_pretrained(path: str, torch_dtype, device, cfg: UNetConfig, vae_cfg):
+    def _load_pretrained(path: str, torch_dtype, device, cfg: Optional[UNetConfig], vae_cfg):
         """-> (unet, prompt encoder or None, VAE decoder or None, VAE state dict or None, VAE config or None)."""
         from safetensors.torch import load_file
         f = os.path.join(path, "unet", "diffusion_pytorch_model.safetensors")
@@ -113,7 +114,13 @@ class StableDiffusionXLCustomPipeline:
             f = os.path.join(path, "unet", "diffusion_pytorch_model.fp16.safetensors")
         if not os.path.exists(f):
             raise FileNotFoundError(f"no SDXL UNet weights under {path}/unet (safetensors)")
-        unet = UNet2DConditionModel.from_state_dict(cfg, load_file(f), device=device)
+        usd = load_file(f)
+        if cfg is None:
+            cfg = SDXL_BASE
+            if "conv_in.weight" in usd and usd["conv_in.weight"].shape[1] != cfg.in_channels:
+                import dataclasses
+                cfg = dataclasses.replace(cfg, in_channels=int(usd["conv_in.weight"].shape[1]))
+        unet = UNet2DConditionModel.from_state_dict(cfg, usd, device=device)
         vae = vsd = vcfg = None
         for name in ("diffusion_pytorch_model.fp16.safetensors", "diffusion_pytorch_model.safetensors"):
             vf = os.path.join(path, "vae", name)
@@ -222,6 +229,7 @@ class StableDiffusionXLCustomPipeline:
                  control_guidance_start: float = 0.0, control_guidance_end: float = 1.0, **ignored):
         """Parameter list of custom_pipelines.py:23-56.  Unknown keyword arguments are accepted and ignored, because
         IPAdapterXL.generate forwards a stray `number_class_crossattention=` into this call (test.py:38, demo.py:124)."""
+        self._require_latent_unet()
         height = height or self.default_sample_size * self.vae_scale_factor           # :189-190
         width = width or self.default_sample_size * self.vae_scale_factor
         original_size = original_size or (height, width)                              # :192-193
@@ -266,6 +274,12 @@ class StableDiffusionXLCustomPipeline:
             out = lat.to(self.device)
         self.set_scale(conditioning_scale)
         return self._output(out, output_type, return_dict)
+
+    def _require_latent_unet(self) -> None:
+        """Text-to-image and image-to-image have no mask to feed the 9-channel inpainting UNet."""
+        if self.unet.config.in_channels != 4:
+            raise IHError(f"{type(self).__name__} needs a 4-channel UNet (this one has {self.unet.config.in_channels} "
+                          "input channels); the 9-channel inpainting UNet runs in StableDiffusionXLInpaintPipeline")
 
     def _output(self, out: torch.Tensor, output_type: Optional[str], return_dict: bool):
         """Final latents -> images (:365-386) in the requested output type."""
@@ -365,7 +379,7 @@ class StableDiffusionXLImg2ImgPipeline(StableDiffusionXLCustomPipeline):
 
     @classmethod
     def from_pretrained(cls, path: str, torch_dtype=torch.float16, add_watermarker: bool = False, device="cuda",
-                        cfg: UNetConfig = SDXL_BASE, vae_cfg=None, **kwargs):
+                        cfg: Optional[UNetConfig] = None, vae_cfg=None, **kwargs):
         """As StableDiffusionXLCustomPipeline.from_pretrained; the VAE checkpoint also provides the encoder."""
         unet, enc, vae, vsd, vcfg = cls._load_pretrained(path, torch_dtype, device, cfg, vae_cfg)
         vae_encoder = None
@@ -424,6 +438,7 @@ class StableDiffusionXLImg2ImgPipeline(StableDiffusionXLCustomPipeline):
         tensor in [-1, 1]) and `strength`.  Unknown keywords are ignored as in the text-to-image pipeline, except the
         diffusers arguments in UNSUPPORTED, which raise IHError."""
         self._require_euler()
+        self._require_latent_unet()
         refused = [k for k in self.UNSUPPORTED if kwargs.get(k) is not None]
         if refused:
             raise IHError(f"StableDiffusionXLImg2ImgPipeline does not implement {refused}")
@@ -470,7 +485,7 @@ class StableDiffusionXLImg2ImgPipeline(StableDiffusionXLCustomPipeline):
 
     def _denoise_from(self, lat, t_start: int, num_inference_steps: int, denoising_end, embeds, sizes, guidance_scale,
                       guidance_rescale, control_guidance_start, control_guidance_end, callback, callback_steps,
-                      inpaint=None, generator=None) -> torch.Tensor:
+                      inpaint=None, generator=None, unet_cond=None) -> torch.Tensor:
         """The loop over timesteps[t_start:], truncated by denoising_end, from the noised start latents `lat`; the
         micro-conditioning time ids are formed from `sizes` (requires_aesthetics_score = False). -> final latents."""
         batch = embeds[0].shape[0]
@@ -500,7 +515,7 @@ class StableDiffusionXLImg2ImgPipeline(StableDiffusionXLCustomPipeline):
                                   control_guidance_end=control_guidance_end, guidance_rescale=guidance_rescale,
                                   num_loop_steps=loop_end, callback=callback, callback_steps=callback_steps,
                                   negative_time_ids=negative_add_time_ids, begin_step=t_start, inpaint=inpaint,
-                                  generator=generator)
+                                  generator=generator, unet_cond=unet_cond)
         else:
             out = lat
         self.set_scale(conditioning_scale)
@@ -543,7 +558,12 @@ class StableDiffusionXLInpaintPipeline(StableDiffusionXLImg2ImgPipeline):
     guidance_scale = 7.5; height / width default to the UNet's sample size x 8, not to the image's size, and the image
     and the mask are resized to them.  Image and mask batches are tiled to the prompt batch with `repeat` (slot b gets
     image b % n_images and mask b % n_masks); with a list of generators only the first n_images encode (SURVEY C.19).
-    The 9-channel inpainting UNet and `padding_mask_crop` are not implemented and raise IHError."""
+
+    With the 9-channel inpainting UNet (diffusers' stable-diffusion-xl-1.0-inpainting-0.1; `from_pretrained` reads the
+    channel count from the checkpoint) there is no blend: every step the UNet sees the latents, the mask and the latents
+    of the masked image (image * (mask < 0.5)), which conv_in reads from a static buffer next to the step's latents
+    (DenoiseEngine.run(unet_cond=...)).  At strength 1 the image itself is not encoded (SURVEY C.32).
+    `padding_mask_crop` is not implemented and raises IHError, as does a UNet with any other channel count."""
 
     UNSUPPORTED = StableDiffusionXLImg2ImgPipeline.UNSUPPORTED + ("masked_image_latents",)
 
@@ -607,9 +627,11 @@ class StableDiffusionXLInpaintPipeline(StableDiffusionXLImg2ImgPipeline):
             refused.append("padding_mask_crop")
         if refused:
             raise IHError(f"StableDiffusionXLInpaintPipeline does not implement {refused}")
-        if self.unet.config.in_channels != 4:
-            raise IHError(f"StableDiffusionXLInpaintPipeline supports the 4-channel UNet only (this one has "
-                          f"{self.unet.config.in_channels} input channels)")
+        unet9 = self.unet.config.in_channels == 9 and self.unet.conv_in.weight.shape[1] == 9
+        if self.unet.config.in_channels != 4 and not unet9:
+            raise IHError(f"StableDiffusionXLInpaintPipeline supports the 4-channel UNet and the 9-channel inpainting "
+                          f"UNet (this one has config.in_channels = {self.unet.config.in_channels} and a conv_in of "
+                          f"{self.unet.conv_in.weight.shape[1]} input channels)")
         if not 0.0 <= strength <= 1.0:
             raise ValueError(f"The value of strength should in [0.0, 1.0] but is {strength}")          # [3P] check_inputs
         height = height or self.default_sample_size * self.vae_scale_factor
@@ -636,34 +658,84 @@ class StableDiffusionXLInpaintPipeline(StableDiffusionXLImg2ImgPipeline):
             raise ValueError(f"After adjusting the num_inference_steps by strength parameter: {strength}, the number of "
                              f"pipeline steps is {num_inference_steps - t_start} which is < 1 and not appropriate for "
                              "this pipeline.")
+        sizes = (original_size or (height, width), crops_coords_top_left, target_size or (height, width),
+                 negative_original_size, negative_crops_coords_top_left, negative_target_size)
+        if unet9:
+            lat, mask_lat, masked_lat = self.prepare_inpaint9_inputs(pixels, mask, batch, generator, t_start,
+                                                                     strength == 1.0)
+            out = self._denoise_from(lat, t_start, num_inference_steps, denoising_end, embeds, sizes, guidance_scale,
+                                     guidance_rescale, control_guidance_start, control_guidance_end, callback,
+                                     callback_steps, generator=generator, unet_cond=(mask_lat, masked_lat))
+            return self._output(out, output_type, return_dict)
         lat, image_latents, noise = self.prepare_inpaint_latents(pixels, batch, generator, t_start, strength == 1.0)
         # the masked image's latents only feed a 9-channel UNet: with 4 channels diffusers encodes them unused.  That
         # encode is skipped; its posterior draw comes after the noise, so it changes only what is drawn later: the step
         # noise of Euler Ancestral, for which the draw is made and dropped (SURVEY C.31)
         if isinstance(self.scheduler, EulerAncestralDiscreteScheduler):
-            self._skip_masked_image_draw(max(pixels.shape[0], mask.shape[0]), height, width, generator)
+            self._posterior_eps(max(pixels.shape[0], mask.shape[0]), height, width, generator)
         mask_lat = torch.nn.functional.interpolate(mask, size=(height // self.vae_scale_factor,
                                                                width // self.vae_scale_factor)).half()
         if batch % mask_lat.shape[0]:
             raise ValueError(f"cannot duplicate a mask batch of {mask_lat.shape[0]} to a prompt batch of {batch}")
         mask_lat = mask_lat.repeat(batch // mask_lat.shape[0], 1, 1, 1).to(self.device)
-        sizes = (original_size or (height, width), crops_coords_top_left, target_size or (height, width),
-                 negative_original_size, negative_crops_coords_top_left, negative_target_size)
         out = self._denoise_from(lat, t_start, num_inference_steps, denoising_end, embeds, sizes, guidance_scale,
                                  guidance_rescale, control_guidance_start, control_guidance_end, callback, callback_steps,
                                  inpaint=(image_latents, noise, mask_lat), generator=generator)
         return self._output(out, output_type, return_dict)
 
-    def _skip_masked_image_draw(self, n_masked: int, height: int, width: int, generator) -> None:
-        """The posterior draw of [3P] diffusers' `_encode_vae_image(masked_image, generator)` in prepare_mask_latents:
-        eps of the n_masked masked images (image * (mask < 0.5) broadcast over both batches), image i with generator[i]
-        for a list, in the dtype and on the device the image latents' eps is drawn with."""
+    def prepare_inpaint9_inputs(self, image: torch.Tensor, mask: torch.Tensor, batch_size: int, generator, t_start: int,
+                                is_strength_max: bool) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+        """[3P] StableDiffusionXLInpaintPipeline.prepare_latents (return_image_latents=False) and prepare_mask_latents
+        for the 9-channel UNet -> (start latents [batch_size, 4, h, w], mask [batch_size, 1, h, w], masked-image latents
+        [batch_size, 4, h, w]), fp16 on the device, CFG halves not yet formed.  Per generator the draws come in
+        diffusers' order: the image's posterior eps (strength < 1 only: at strength 1 the image is not encoded), the
+        noise, then the masked images' posterior eps (SURVEY C.32).  Both encodes use the posterior kernel; with sigma 0
+        and zero noise it returns the scaled posterior sample exactly."""
+        venc = self.vae_encoder
+        n_img, n_mask = image.shape[0], mask.shape[0]
+        if n_img != n_mask and 1 not in (n_img, n_mask):
+            raise ValueError(f"an image batch of {n_img} and a mask batch of {n_mask} do not broadcast")
+        n_masked = max(n_img, n_mask)
+        for what, k in (("image", n_img), ("mask", n_mask), ("masked image", n_masked)):
+            if batch_size % k:
+                raise ValueError(f"cannot duplicate a {what} batch of {k} to a prompt batch of {batch_size}")
+        if isinstance(generator, list) and len(generator) != batch_size:
+            raise ValueError(f"got {len(generator)} generators for a batch of {batch_size}")
+        height, width = image.shape[2], image.shape[3]
+        L, sf = venc.config.latent_channels, venc.config.scaling_factor
+        shape = (batch_size, L, height // self.vae_scale_factor, width // self.vae_scale_factor)
+
+        def draw_noise():
+            if isinstance(generator, list):
+                return torch.cat([torch.randn((1,) + shape[1:], generator=g, device=g.device, dtype=torch.float16)
+                                  .to(self.device) for g in generator])
+            return torch.randn(shape, generator=generator, device=generator.device if generator is not None else "cpu",
+                               dtype=torch.float16).to(self.device)
+        if is_strength_max:
+            latents = (draw_noise().float() * self.scheduler.init_noise_sigma).half()
+        else:
+            moments = venc.encode_moments_nhwc(image.to(self.device, torch.float16))
+            eps = self._posterior_eps(n_img, height, width, generator)
+            latents = ops.vae_posterior_noise(moments, eps, draw_noise().contiguous(), L, sf,
+                                              self.scheduler.add_noise_sigma(t_start))
+        masked = image * (mask < 0.5)
+        moments = venc.encode_moments_nhwc(masked.to(self.device, torch.float16))
+        eps = self._posterior_eps(n_masked, height, width, generator)
+        zeros = torch.zeros(shape, dtype=torch.float16, device=self.device)
+        masked_latents = ops.vae_posterior_noise(moments, eps, zeros, L, sf, 0.0)
+        mask_lat = torch.nn.functional.interpolate(mask, size=shape[2:]).half()
+        return latents, mask_lat.repeat(batch_size // n_mask, 1, 1, 1).to(self.device), masked_latents
+
+    def _posterior_eps(self, n: int, height: int, width: int, generator) -> torch.Tensor:
+        """The posterior draw of [3P] diffusers' `_encode_vae_image(images, generator)` for n images: image i with
+        generator[i] for a list, fp32 when the VAE is upcast (else fp16), on the generator's device; -> on the device.
+        For the masked images (image * (mask < 0.5) broadcast over both batches) the 4-channel path draws and drops it
+        (SURVEY C.31); the 9-channel path encodes with it, and with the same draw of the image batch (SURVEY C.32)."""
         L = self.vae_encoder.config.latent_channels
         shape = (L, height // self.vae_scale_factor, width // self.vae_scale_factor)
         dtype = torch.float32 if getattr(self.vae_encoder.config, "force_upcast", True) else torch.float16
         if isinstance(generator, list):
-            for g in generator[:n_masked]:
-                torch.randn((1,) + shape, generator=g, device=g.device, dtype=dtype)
-        else:
-            torch.randn((n_masked,) + shape, generator=generator,
-                        device=generator.device if generator is not None else "cpu", dtype=dtype)
+            return torch.cat([torch.randn((1,) + shape, generator=g, device=g.device, dtype=dtype).to(self.device)
+                              for g in generator[:n]]).contiguous()
+        return torch.randn((n,) + shape, generator=generator,
+                           device=generator.device if generator is not None else "cpu", dtype=dtype).to(self.device)
