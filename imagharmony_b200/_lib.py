@@ -22,6 +22,12 @@ class IHError(RuntimeError):
     pass
 
 
+class IhCnResidual(ctypes.Structure):
+    """One entry of ih_controlnet_add_residuals_f16 (include/ih_api.h)."""
+    _fields_ = [("skip", c_void_p), ("residual", c_void_p), ("rows", c_longlong), ("skip_row0", c_longlong),
+                ("channels", c_int)]
+
+
 def source_hash() -> str:
     """sha256 over the CUDA / header sources the library is built from (name + content, sorted)."""
     import hashlib
@@ -131,6 +137,9 @@ SIGNATURES = {
     "ih_euler_ancestral_scale_input": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_longlong, c_int, c_void_p]),
     "ih_scale_model_input": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_longlong, c_void_p]),
     "ih_scale_model_input_ex": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_longlong, c_int, c_void_p]),
+    "ih_conv3x3_small_f16": (c_int, [c_void_p, c_longlong, c_longlong, c_longlong, c_longlong, c_void_p, c_void_p,
+                                     c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p]),
+    "ih_controlnet_add_residuals_f16": (c_int, [ctypes.POINTER(IhCnResidual), c_int, c_void_p, c_void_p]),
 }
 
 _lib = None

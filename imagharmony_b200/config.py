@@ -52,6 +52,31 @@ TINY = UNetConfig(
 
 
 @dataclass(frozen=True)
+class ControlNetConfig(UNetConfig):
+    """[3P] diffusers ControlNetModel config of an SDXL ControlNet (e.g. diffusers/controlnet-canny-sdxl-1.0
+    config.json): the UNet's encoder half (same block fields as UNetConfig) plus the conditioning-image embedding
+    (SURVEY appendix A.7).  `global_pool_conditions` models are not supported (IHError at construction)."""
+    conditioning_channels: int = 3
+    conditioning_embedding_out_channels: Tuple[int, ...] = (16, 32, 96, 256)
+    controlnet_conditioning_channel_order: str = "rgb"
+    global_pool_conditions: bool = False
+
+
+SDXL_CONTROLNET = ControlNetConfig()
+# TINY's encoder with the SDXL embedding's small widths 16/32/96 (the direct small-channel conv path); the last width
+# is 128 so that the embedding's conv_out (-> 64) runs on the implicit-GEMM conv as SDXL's 256 -> 320 does
+TINY_CONTROLNET = ControlNetConfig(
+    block_out_channels=TINY.block_out_channels,
+    transformer_layers_per_block=TINY.transformer_layers_per_block,
+    cross_attention_dim=TINY.cross_attention_dim,
+    addition_time_embed_dim=TINY.addition_time_embed_dim,
+    pooled_embed_dim=TINY.pooled_embed_dim,
+    sample_size=TINY.sample_size,
+    conditioning_embedding_out_channels=(16, 32, 96, 128),
+)
+
+
+@dataclass(frozen=True)
 class HarmonyConfig:
     """HarmonyAttention hyper-parameters (train.py:189-197; shipped values run.sh:17-20, test.py:12-15)."""
     image_hidden_size: int = 1280

@@ -1499,3 +1499,113 @@ extern "C" int ih_im2col3x3_nchw_cat_f16(const void* x0, int C0, const void* x1,
                         (cudaStream_t)stream, (const __half*)x0, C0, (const __half*)x1, C1, (__half*)out, B, H, W, Kpad));
   return 0;
 }
+
+namespace ih {
+
+// ControlNet conditioning embedding ([3P] diffusers ControlNetConditioningEmbedding): 3x3 convs, pad 1, stride 1 or 2,
+// over the 3/16/32/96 channel widths that the implicit-GEMM conv cannot take (it needs whole 64-wide K blocks per tap).
+// One thread per output element (pixel, cout), cout fastest; fp32 accumulation over the 9 * Cin products in tap order,
+// then + bias, optional SiLU, one fp16 rounding.  The input is read through element strides, so the NCHW control image
+// and the NHWC intermediate activations take the same kernel; the weight is tap-major [Cout, 9 * Cin].  It runs once
+// per pipeline call, so the simple form is kept.
+__global__ void conv3x3_small_kernel(const __half* __restrict__ x, long long sb, long long sh, long long sw, long long sc,
+                                     const __half* __restrict__ w, const __half* __restrict__ bias,
+                                     __half* __restrict__ out, int B, int H, int W, int Cin, int Cout, int stride,
+                                     int Ho, int Wo, int silu) {
+  pdl_launch_dependents();
+  pdl_wait();
+  const long long total = (long long)B * Ho * Wo * Cout;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+    const int co = (int)(i % Cout);
+    const long long pix = i / Cout;
+    const int xo = (int)(pix % Wo);
+    const int yo = (int)((pix / Wo) % Ho);
+    const int b = (int)(pix / ((long long)Wo * Ho));
+    const __half* wr = w + (long long)co * 9 * Cin;
+    float acc = 0.f;
+#pragma unroll 1
+    for (int t = 0; t < 9; ++t) {
+      const int yy = yo * stride + t / 3 - 1, xx = xo * stride + t % 3 - 1;
+      if (yy < 0 || yy >= H || xx < 0 || xx >= W) continue;
+      const __half* xp = x + b * sb + yy * sh + xx * sw;
+      const __half* wp = wr + t * Cin;
+      for (int ci = 0; ci < Cin; ++ci) acc = fmaf(__half2float(xp[ci * sc]), __half2float(wp[ci]), acc);
+    }
+    if (bias) acc += __half2float(bias[co]);
+    if (silu) acc = acc / (1.f + __expf(-acc));
+    out[i] = __float2half_rn(acc);
+  }
+}
+
+// ControlNet residual injection: for every entry k, rows [0, rows) of residual k are added to rows
+// [skip_row0, skip_row0 + rows) of skip tensor k in place, skip = fp16(skip + fp16(res * scale[k])) -- diffusers'
+// rounding points (the ControlNet scales its fp16 outputs, the UNet adds them).  The entry table is a kernel argument,
+// so a captured CUDA graph keeps it with the launch; the scales are read from device memory, so one graph serves every
+// conditioning scale.  blockIdx.y selects the entry; 8 halves per thread.
+struct CnTable {
+  IhCnResidual e[IH_CN_MAX_RESIDUALS];
+};
+
+__global__ void controlnet_add_residuals_kernel(const __grid_constant__ CnTable tab, const float* __restrict__ scale) {
+  pdl_launch_dependents();
+  pdl_wait();
+  const IhCnResidual en = tab.e[blockIdx.y];
+  const float s = scale[blockIdx.y];
+  const long long nvec = en.rows * (en.channels / 8);
+  const uint4* r = reinterpret_cast<const uint4*>(en.residual);
+  uint4* d = reinterpret_cast<uint4*>(en.skip) + en.skip_row0 * (en.channels / 8);
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < nvec; i += (long long)gridDim.x * blockDim.x) {
+    uint4 rv = r[i], dv = d[i];
+    __half2* rh = reinterpret_cast<__half2*>(&rv);
+    __half2* dh = reinterpret_cast<__half2*>(&dv);
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const float2 rf = __half22float2(rh[j]), df = __half22float2(dh[j]);
+      const float a = __half2float(__float2half_rn(__fmul_rn(rf.x, s)));
+      const float b = __half2float(__float2half_rn(__fmul_rn(rf.y, s)));
+      dh[j] = __floats2half2_rn(__fadd_rn(df.x, a), __fadd_rn(df.y, b));
+    }
+    d[i] = dv;
+  }
+}
+
+}  // namespace ih
+
+extern "C" int ih_conv3x3_small_f16(const void* x, long long sb, long long sh, long long sw, long long sc, const void* w,
+                                    const void* bias, void* out, int B, int H, int W, int Cin, int Cout, int stride,
+                                    int silu, void* stream) {
+  IH_CHECK(x && w && out, IH_ERR_ARG, "ih_conv3x3_small_f16: null pointer");
+  IH_CHECK(B >= 1 && H >= 1 && W >= 1 && Cin >= 1 && Cout >= 1, IH_ERR_SHAPE,
+           "ih_conv3x3_small_f16: empty shape (B=%d, H=%d, W=%d, Cin=%d, Cout=%d)", B, H, W, Cin, Cout);
+  IH_CHECK(stride == 1 || stride == 2, IH_ERR_ARG, "ih_conv3x3_small_f16: stride must be 1 or 2, got %d", stride);
+  IH_CHECK(silu == 0 || silu == 1, IH_ERR_ARG, "ih_conv3x3_small_f16: silu must be 0 or 1");
+  const int Ho = (H - 1) / stride + 1, Wo = (W - 1) / stride + 1;
+  const long long total = (long long)B * Ho * Wo * Cout;
+  IH_CUDA(launch_kernel(conv3x3_small_kernel, dim3(grid_for(total, 256)), dim3(256), (size_t)0, (cudaStream_t)stream,
+                        (const __half*)x, sb, sh, sw, sc, (const __half*)w, (const __half*)bias, (__half*)out, B, H, W,
+                        Cin, Cout, stride, Ho, Wo, silu));
+  return 0;
+}
+
+extern "C" int ih_controlnet_add_residuals_f16(const IhCnResidual* entries, int n_entries, const void* scale,
+                                               void* stream) {
+  IH_CHECK(entries && scale, IH_ERR_ARG, "ih_controlnet_add_residuals_f16: null pointer");
+  IH_CHECK(n_entries >= 1 && n_entries <= IH_CN_MAX_RESIDUALS, IH_ERR_SHAPE,
+           "ih_controlnet_add_residuals_f16: n_entries=%d outside [1, %d]", n_entries, IH_CN_MAX_RESIDUALS);
+  ih::CnTable tab{};
+  long long most = 0;
+  for (int k = 0; k < n_entries; ++k) {
+    const IhCnResidual& e = entries[k];
+    IH_CHECK(e.skip && e.residual, IH_ERR_ARG, "ih_controlnet_add_residuals_f16: entry %d has a null pointer", k);
+    IH_CHECK(e.rows >= 1 && e.skip_row0 >= 0 && e.channels >= 8 && e.channels % 8 == 0, IH_ERR_SHAPE,
+             "ih_controlnet_add_residuals_f16: entry %d: rows=%lld, skip_row0=%lld, channels=%d (a multiple of 8)", k,
+             e.rows, e.skip_row0, e.channels);
+    IH_CHECK(((unsigned long long)e.skip | (unsigned long long)e.residual) % 16 == 0, IH_ERR_ALIGN,
+             "ih_controlnet_add_residuals_f16: entry %d is not 16-byte aligned", k);
+    tab.e[k] = e;
+    most = e.rows * (e.channels / 8) > most ? e.rows * (e.channels / 8) : most;
+  }
+  IH_CUDA(launch_kernel(ih::controlnet_add_residuals_kernel, dim3(grid_for(most, 256), n_entries), dim3(256), (size_t)0,
+                        (cudaStream_t)stream, tab, (const float*)scale));
+  return 0;
+}

@@ -20,11 +20,16 @@ gives diffusers' noise (a Philox stream inside the kernel would not reproduce to
 
 Graph lifetime: a captured graph holds raw pointers.  Everything it reads lives in buffers that are owned per shape
 and never freed while the graph exists -- the engine's static inputs (`_static`, `_inpaint_static`, `_dpm_static`,
-`_cond_static`, `_ancestral_noise`), the schedule tables (`_tables`, `_coeffs`), the processors'
+`_cond_static`, `_ancestral_noise`, `_cn_static`: the ControlNet's conditioning embedding and scale vector), the schedule tables (`_tables`, `_coeffs`), the processors'
 K/V buffers and the UNet's add-embedding buffer (per-shape dicts inside those objects), and the library's grow-only
 scratch buffers whose re-allocation bumps `ops.workspace_generation()`.  A graph is replayed only if it was captured
 under the current UNet `graph_epoch` (weights / processors unchanged) and the current workspace generation; otherwise
-it is re-captured.
+it is re-captured; graphs with the ControlNet also need the ControlNet's `graph_epoch` they were captured under.
+
+ControlNet (`run(controlnet=...)`): a step runs the ControlNet forward, then the UNet with its residuals injected
+after the mid block, then the unchanged step kernel, all in the one graph.  Steps where the ControlNet is off
+(keep[i] = 0) replay the ControlNet-free graph.  The scale vector is read from device memory, so a new
+controlnet_conditioning_scale does not re-capture.
 """
 from __future__ import annotations
 
@@ -35,6 +40,7 @@ import torch
 
 from . import ops
 from ._lib import IHError
+from .controlnet import controlnet_scales
 from .scheduler import DPMSolverMultistepScheduler, EulerAncestralDiscreteScheduler, EulerDiscreteScheduler
 from .unet import UNet2DConditionModel
 
@@ -55,6 +61,10 @@ class DenoiseEngine:
         self._tables: Dict[Tuple[str, int], Tuple[torch.Tensor, torch.Tensor, float]] = {}
         self._coeffs: Dict[Tuple[str, int], torch.Tensor] = {}         # DPM-Solver++ / Euler Ancestral coefficients
         self._ancestral_noise: Dict[Tuple[int, int, int, int], torch.Tensor] = {}   # Euler Ancestral step noise
+        self._cn_static: Dict[Tuple, dict] = {}        # ControlNet: conditioning embedding + scale vector per shape
+        # (ControlNet, graph_epoch) the ControlNet graphs were captured for.  The model object itself is kept, not its id:
+        # a freed model's id can be reused by a new one that reaches the same epoch
+        self._cn_epoch = None
         self._epoch = getattr(unet, "graph_epoch", 0)
         self.last_launches_per_step = 0
         self.graphs_captured = 0
@@ -152,6 +162,18 @@ class DenoiseEngine:
             self._cond_static[key] = buf
         return buf
 
+    def _cn_buffers(self, b: int, h: int, w: int) -> dict:
+        """ControlNet static inputs per (ControlNet batch, h, w), never freed (the graph-lifetime rule above): the
+        conditioning embedding NHWC [b, h, w, C0] and the fp32 scale vector [10], refilled by every call."""
+        key = (b, h, w)
+        cb = self._cn_static.get(key)
+        if cb is None:
+            C0 = self.unet.config.block_out_channels[0]
+            cb = {"emb": torch.empty((b, h, w, C0), dtype=torch.float16, device=self.device),
+                  "scale": torch.zeros((10,), dtype=torch.float32, device=self.device)}
+            self._cn_static[key] = cb
+        return cb
+
     def _draw_ancestral_noise(self, buf: torch.Tensor, generator, begin: int, end: int) -> None:
         """Rows [begin, end) of the step noise, one draw per step in step order, as [3P] diffusers' randn_tensor draws
         it inside EulerAncestralDiscreteScheduler.step: fp16, shaped like the guided prediction, on the generator's
@@ -180,9 +202,16 @@ class DenoiseEngine:
         if use_cfg:
             st["model_in"][n:].copy_(st["latents"])
 
-    def _step(self, st, timesteps, sigmas, guidance, use_cfg=True, rescale=0.0, ib=None, dpm=None, anc=None, cond=None):
+    def _step(self, st, timesteps, sigmas, guidance, use_cfg=True, rescale=0.0, ib=None, dpm=None, anc=None, cond=None,
+              cn=None):
+        residuals = None
+        if cn is not None:          # (ControlNet, static buffers, first image of the batch it runs on)
+            model, cb, b0 = cn
+            out = model(st["model_in"][b0:], timesteps, st["ehs"][b0:], text_embeds=st["text_embeds"][b0:],
+                        time_ids=st["time_ids"][b0:], step=st["step"], cond_embedding=cb["emb"], scale=cb["scale"])
+            residuals = (out, b0)
         noise = self.unet(st["model_in"], timesteps, st["ehs"], st["text_embeds"], st["time_ids"], step=st["step"],
-                          cond=cond)
+                          cond=cond, controlnet_residuals=residuals)
         if dpm is not None:
             db, coeffs = dpm
             ops.dpm_solver_step(noise, st["latents"], st["model_in"], db["prev_x0"], coeffs, st["step"],
@@ -210,7 +239,7 @@ class DenoiseEngine:
             negative_time_ids: Optional[torch.Tensor] = None, begin_step: int = 0,
             inpaint: Optional[Tuple[torch.Tensor, torch.Tensor, torch.Tensor]] = None,
             generator: Optional[Union[torch.Generator, List[torch.Generator]]] = None,
-            unet_cond: Optional[Tuple[torch.Tensor, torch.Tensor]] = None) -> torch.Tensor:
+            unet_cond: Optional[Tuple[torch.Tensor, torch.Tensor]] = None, controlnet=None) -> torch.Tensor:
         """latents [n,4,h,w] (already scaled by init_noise_sigma; host or device); embeds host or device tensors.
         Returns the latents after the last executed step as a new device tensor.
 
@@ -250,7 +279,14 @@ class DenoiseEngine:
         one per image, or None for the device's default generator) supplies the Gaussian noise of every step; before
         the steps run, the noise of exactly the steps this call executes is drawn from it, one draw per step in step
         order.  So `stop_after=k` followed by `start_step=k` with the same, continuing generator object reproduces the
-        uninterrupted run.  The other schedulers draw nothing and ignore `generator`."""
+        uninterrupted run.  The other schedulers draw nothing and ignore `generator`.
+
+        `controlnet` = a ControlNetCall ([3P] StableDiffusionXLControlNetPipeline): at every step i with keep[i] = 1 the
+        ControlNet runs on the step's model input (the CFG batch, or in guess mode with CFG the conditional half only)
+        and its scaled residuals are added to the UNet's skip connections and mid-block output; at steps with keep[i] =
+        0 the step is the plain one.  The control image's embedding is computed once per call.  It works with every
+        scheduler and the loop options of text-to-image, not with begin_step, inpaint, unet_cond, start_step or
+        stop_after (IHError).  It draws no random numbers."""
         use_cfg = guidance_scale > 1.0                                            # :223
         if use_cfg and (negative_prompt_embeds is None or negative_pooled is None):
             raise IHError("classifier-free guidance needs negative_prompt_embeds / negative_pooled")
@@ -266,6 +302,10 @@ class DenoiseEngine:
                           f"UNet; this UNet has {ucfg.in_channels} input channels")
         if unet_cond is not None and (inpaint is not None or start_step or stop_after is not None):
             raise IHError("unet_cond cannot be combined with inpaint / start_step / stop_after")
+        if controlnet is not None and (begin_step or inpaint is not None or unet_cond is not None or start_step
+                                       or stop_after is not None):
+            raise IHError("controlnet runs text-to-image loops: it cannot be combined with begin_step, inpaint, "
+                          "unet_cond, start_step or stop_after")
         n, _, h, w = latents.shape
         if is_ancestral and isinstance(generator, list) and len(generator) != n:
             raise IHError(f"got {len(generator)} generators for a batch of {n}")
@@ -329,6 +369,30 @@ class DenoiseEngine:
         if dpm is not None:
             dpm[0]["loop_begin"].fill_(start_step)
         self.unet.prepare_conditioning(st["ehs"], st["text_embeds"], st["time_ids"])
+        cn = None
+        keep = [1.0] * T
+        if controlnet is not None:
+            model = controlnet.model
+            if model.config.block_out_channels != ucfg.block_out_channels:
+                raise IHError("the ControlNet's block_out_channels differ from the UNet's")
+            if controlnet.keep is not None:
+                keep = [float(k) for k in controlnet.keep]
+                if len(keep) != T:
+                    raise IHError(f"controlnet keep has {len(keep)} entries for a {T}-step schedule")
+            guess = bool(controlnet.guess_mode)
+            b0 = n if (use_cfg and guess) else 0                    # guess mode + CFG: the conditional half only
+            b_cn = (2 * n if use_cfg else n) - b0
+            image = controlnet.image
+            if tuple(image.shape) != (n, model.config.conditioning_channels, 8 * h, 8 * w):
+                raise IHError(f"controlnet image: expected {(n, model.config.conditioning_channels, 8 * h, 8 * w)}, "
+                              f"got {tuple(image.shape)}")
+            cb = self._cn_buffers(b_cn, h, w)
+            model.embed_condition(image.to(self.device, torch.float16).contiguous(), out=cb["emb"][:n])
+            if b_cn > n:                                            # [3P] cat([image] * 2) under CFG
+                cb["emb"][n:].copy_(cb["emb"][:n])
+            cb["scale"].copy_(controlnet_scales(controlnet.conditioning_scale, guess))
+            model.prepare_conditioning(st["ehs"][b0:], st["text_embeds"][b0:], st["time_ids"][b0:])
+            cn = (model, cb, b0)
         self._first_input(st, sigmas, use_cfg, dpm, anc)                               # :332-334
 
         steps = loop_T if stop_after is None else min(stop_after, loop_T)
@@ -339,25 +403,36 @@ class DenoiseEngine:
             off = ((i - b0) / n_loop < control_guidance_start) or ((i - b0 + 1) / n_loop > control_guidance_end)  # :326-329
             return 0.0 if off else float(ip_scale)
 
-        def gkey(scale: float):
+        def cn_at(i: int):
+            return cn if (cn is not None and keep[i] > 0) else None
+
+        def gkey(scale: float, cn_step):
             return (n, h, w, L, T, use_cfg, float(guidance_scale), rescale, scale, self.scheduler.kind, cond is not None,
-                    ib is not None)
+                    ib is not None, None if cn_step is None else ("controlnet", cn_step[2] > 0))
 
         if self.use_cuda_graph:
             if self._epoch != getattr(self.unet, "graph_epoch", 0):       # weights / processors changed since capture
                 self._graphs.clear()
                 self._epoch = getattr(self.unet, "graph_epoch", 0)
-            needed = sorted({scale_at(i) for i in range(start_step, steps)})
+            if cn is not None and (self._cn_epoch is None or self._cn_epoch[0] is not cn[0]
+                                   or self._cn_epoch[1] != cn[0].graph_epoch):     # another / a reloaded ControlNet
+                self._graphs = {k: v for k, v in self._graphs.items() if k[-1] is None}
+                self._cn_epoch = (cn[0], cn[0].graph_epoch)
+            needed = {}
+            for i in range(start_step, steps):
+                needed.setdefault(gkey(scale_at(i), cn_at(i)), (scale_at(i), cn_at(i)))
             captured = False
             for _ in range(4):      # a warm-up may grow a scratch buffer, which invalidates graphs captured before it
                 gen = ops.workspace_generation()
-                missing = [sc for sc in needed if self._graphs.get(gkey(sc), (None, -1))[1] != gen]
+                missing = [k for k in needed if self._graphs.get(k, (None, -1))[1] != gen]
                 if not missing:
                     break
-                for sc in missing:
+                for k in missing:
+                    sc, cn_step = needed[k]
                     self.set_scale(sc)
-                    g = self._capture(st, timesteps, sigmas, guidance_scale, use_cfg, rescale, ib, dpm, anc, cond)
-                    self._graphs[gkey(sc)] = (g, ops.workspace_generation())
+                    g = self._capture(st, timesteps, sigmas, guidance_scale, use_cfg, rescale, ib, dpm, anc, cond,
+                                      cn_step)
+                    self._graphs[k] = (g, ops.workspace_generation())
                     captured = True
             else:
                 raise IHError("scratch buffers kept growing during graph capture")
@@ -371,31 +446,31 @@ class DenoiseEngine:
         for i in range(start_step, steps):
             sc = scale_at(i)
             if self.use_cuda_graph:
-                self._graphs[gkey(sc)][0].replay()
+                self._graphs[gkey(sc, cn_at(i))][0].replay()
             else:
                 self.set_scale(sc)
-                self._step(st, timesteps, sigmas, guidance_scale, use_cfg, rescale, ib, dpm, anc, cond)
+                self._step(st, timesteps, sigmas, guidance_scale, use_cfg, rescale, ib, dpm, anc, cond, cn_at(i))
             if callback is not None and (i - b0) % callback_steps == 0:           # :359-363 (Euler: order 1, no warm-up)
                 callback(i - b0, timesteps[i], st["latents"])
         self.set_scale(ip_scale)
         return st["latents"].clone()
 
     def _capture(self, st, timesteps, sigmas, guidance, use_cfg=True, rescale=0.0, ib=None, dpm=None, anc=None,
-                 cond=None):
+                 cond=None, cn=None):
         # warm-up on a side stream (sets kernel attributes, fills the TMA descriptor cache, sizes the allocator and
         # the library's scratch buffers)
         side = torch.cuda.Stream(device=self.device)
         side.wait_stream(torch.cuda.current_stream())
         with torch.cuda.stream(side):
             st["step"].zero_()
-            self._step(st, timesteps, sigmas, guidance, use_cfg, rescale, ib, dpm, anc, cond)
+            self._step(st, timesteps, sigmas, guidance, use_cfg, rescale, ib, dpm, anc, cond, cn)
         torch.cuda.current_stream().wait_stream(side)
         torch.cuda.synchronize()
         st["step"].zero_()
         g = torch.cuda.CUDAGraph()
         before = ops.launch_count()
         with torch.cuda.graph(g):
-            self._step(st, timesteps, sigmas, guidance, use_cfg, rescale, ib, dpm, anc, cond)
+            self._step(st, timesteps, sigmas, guidance, use_cfg, rescale, ib, dpm, anc, cond, cn)
         self.last_launches_per_step = ops.launch_count() - before
         self.graphs_captured += 1
         return g

@@ -739,3 +739,55 @@ def scale_model_input(latents: torch.Tensor, model_in: torch.Tensor, sigmas: tor
         raise IHError("scale_model_input: model_in must hold the CFG pair (duplicate=True) or one copy of the latents")
     check(lib.ih_scale_model_input_ex(latents.data_ptr(), model_in.data_ptr(), sigmas.data_ptr(), step.data_ptr(),
                                       latents.numel(), int(duplicate), _stream()), "ih_scale_model_input_ex")
+
+
+def conv3x3_small(x: torch.Tensor, w_packed: torch.Tensor, bias: Optional[torch.Tensor] = None, *, stride: int = 1,
+                  silu: bool = False, nchw: bool = False, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """3x3 conv, pad 1, stride 1 or 2, for small channel counts (ih_conv3x3_small_f16, the ControlNet conditioning
+    embedding): x NHWC [B, H, W, Cin] (or NCHW [B, Cin, H, W] with nchw=True); w_packed [Cout, 9*Cin] tap-major;
+    -> NHWC [B, ceil(H/stride), ceil(W/stride), Cout], bias and SiLU fused."""
+    lib = _lib.load()
+    _req(x, "x"); _req(w_packed, "w")
+    if nchw:
+        B, Cin, H, W = x.shape
+        sb, sc, sh, sw = x.stride()
+    else:
+        B, H, W, Cin = x.shape
+        sb, sh, sw, sc = x.stride()
+    Cout = w_packed.shape[0]
+    if not w_packed.is_contiguous() or w_packed.shape[1] != 9 * Cin:
+        raise IHError(f"conv3x3_small: w_packed must be contiguous [Cout, {9 * Cin}], got {tuple(w_packed.shape)}")
+    if bias is not None:
+        _req(bias, "bias")
+    Ho, Wo = (H - 1) // stride + 1, (W - 1) // stride + 1
+    if out is None:
+        out = torch.empty((B, Ho, Wo, Cout), dtype=torch.float16, device=x.device)
+    elif tuple(out.shape) != (B, Ho, Wo, Cout) or not out.is_contiguous():
+        raise IHError(f"conv3x3_small: out must be contiguous {(B, Ho, Wo, Cout)}")
+    rc = lib.ih_conv3x3_small_f16(x.data_ptr(), sb, sh, sw, sc, w_packed.data_ptr(), _p(bias), out.data_ptr(), B, H, W,
+                                  Cin, Cout, stride, int(silu), _stream())
+    check(rc, "ih_conv3x3_small_f16")
+    return out
+
+
+def controlnet_add_residuals(skips, residuals, scale: torch.Tensor, skip_row0s) -> None:
+    """ih_controlnet_add_residuals_f16: skips[k][rows r0 .. r0 + R) = fp16(skip + fp16(residuals[k] * scale[k])) in
+    place, all k in one launch.  skips[k] / residuals[k] are contiguous fp16 with the channel count last (the residual
+    has R rows); scale is a device float32 vector with one value per entry; skip_row0s[k] is r0."""
+    lib = _lib.load()
+    _req(scale, "scale", torch.float32)
+    n = len(skips)
+    if not (n == len(residuals) == len(skip_row0s)) or scale.numel() < n or not scale.is_contiguous():
+        raise IHError(f"controlnet_add_residuals: {n} skips, {len(residuals)} residuals, {len(skip_row0s)} offsets "
+                      f"and {scale.numel()} scales")
+    table = (_lib.IhCnResidual * n)()
+    for k, (s, r, r0) in enumerate(zip(skips, residuals, skip_row0s)):
+        _req(s, f"skip[{k}]"); _req(r, f"residual[{k}]")
+        C = s.shape[-1]
+        rows = r.numel() // C
+        if (not s.is_contiguous() or not r.is_contiguous() or r.shape[-1] != C or r0 < 0
+                or r0 + rows > s.numel() // C):
+            raise IHError(f"controlnet_add_residuals: entry {k}: skip {tuple(s.shape)} cannot take residual "
+                          f"{tuple(r.shape)} at row {r0}")
+        table[k] = _lib.IhCnResidual(s.data_ptr(), r.data_ptr(), rows, int(r0), C)
+    check(lib.ih_controlnet_add_residuals_f16(table, n, scale.data_ptr(), _stream()), "ih_controlnet_add_residuals_f16")

@@ -319,38 +319,14 @@ class TimestepEmbedding(nn.Module):
         self.linear_2 = nn.Linear(dim, dim)
 
 
-class UNet2DConditionModel(nn.Module):
-    """Native SDXL UNet. Build on the meta device + `load_state_dict(..., assign=True)` or via `from_state_dict`."""
+class SDXLEncoderModel(nn.Module):
+    """What the UNet and the ControlNet share: processor plumbing (`attn_processors` / `set_attn_processor`), the
+    kernel-layout weights of the blocks (`finalize`), the step-invariant conditioning (`prepare_conditioning`: the
+    cross-attention K/V and the text_time embedding) and the per-step time embeddings.  Subclasses own `conv_in`,
+    `time_embedding`, `add_embedding`, the blocks, and `_finalize_ends()` for the weights outside the blocks."""
 
-    def __init__(self, cfg: UNetConfig):
+    def __init__(self):
         super().__init__()
-        if cfg.in_channels not in (4, 9):
-            raise IHError(f"UNet2DConditionModel: in_channels must be 4 (latents) or 9 (inpainting: latents | mask | "
-                          f"masked-image latents), got {cfg.in_channels}")
-        self.config = cfg
-        boc = cfg.block_out_channels
-        tl = cfg.transformer_layers_per_block
-        self.conv_in = nn.Conv2d(cfg.in_channels, boc[0], 3, padding=1)
-        self.time_embedding = TimestepEmbedding(boc[0], cfg.time_embed_dim)
-        self.add_embedding = TimestepEmbedding(cfg.add_embed_in, cfg.time_embed_dim)
-        downs = []
-        ch = boc[0]
-        for i, co in enumerate(boc):
-            downs.append(DownBlock(cfg, ch, co, tl[i], add_down=i < len(boc) - 1))
-            ch = co
-        self.down_blocks = nn.ModuleList(downs)
-        rev = list(reversed(boc))
-        rtl = list(reversed(tl))
-        ups = []
-        prev = rev[0]
-        for i, co in enumerate(rev):
-            skip_ch = rev[min(i + 1, len(rev) - 1)]
-            ups.append(UpBlock(cfg, prev, skip_ch, co, rtl[i], add_up=i < len(rev) - 1))
-            prev = co
-        self.up_blocks = nn.ModuleList(ups)
-        self.mid_block = MidBlock(cfg, boc[-1], tl[-1])
-        self.conv_norm_out = nn.GroupNorm(cfg.norm_num_groups, boc[0], eps=1e-5)
-        self.conv_out = nn.Conv2d(boc[0], cfg.out_channels, 3, padding=1)
         self._w_temb = None
         self._b_temb = None
         self._aug = None          # (key, aug_emb [B, time_embed_dim]) of the last prepare_conditioning()
@@ -360,7 +336,7 @@ class UNet2DConditionModel(nn.Module):
 
     # ------------------------------------------------------------------------------------------------------------
     @classmethod
-    def from_state_dict(cls, cfg: UNetConfig, state_dict: Dict[str, torch.Tensor], device="cuda"):
+    def from_state_dict(cls, cfg, state_dict: Dict[str, torch.Tensor], device="cuda"):
         with torch.device("meta"):
             m = cls(cfg)
         sd = {k: v.to(device=device, dtype=torch.float16) for k, v in state_dict.items()}
@@ -369,28 +345,6 @@ class UNet2DConditionModel(nn.Module):
         m.install_default_processors()
         m.finalize()
         return m
-
-    def install_default_processors(self, scale: float = 1.0):
-        """IPAdapter.set_ip_adapter (ip_adapter.py:99-125) for this UNet; IP weights are zero until loaded."""
-        from ip_adapter.attention_processor import AttnProcessor2_0, IPAttnProcessor2_0
-        cfg = self.config
-        procs = {}
-        dev = self.conv_in.weight.device
-        for name, attn in self._attn_modules():
-            if name.endswith("attn1"):
-                procs[name + ".processor"] = AttnProcessor2_0()
-            else:
-                C = attn.to_q.weight.shape[0]
-                with torch.device("meta"):
-                    p = IPAttnProcessor2_0(C, cfg.cross_attention_dim, scale=scale, num_tokens=cfg.num_ip_tokens,
-                                           skip=cfg.ip_target_substring not in name)
-                p = p.to_empty(device=dev).half()
-                for q in p.parameters():
-                    q.data.zero_()
-                    q.requires_grad_(False)
-                procs[name + ".processor"] = p
-        self.set_attn_processor(procs)
-        return procs
 
     def _attn_modules(self):
         for name, m in self.named_modules():
@@ -431,31 +385,32 @@ class UNet2DConditionModel(nn.Module):
                 m.link_prefetch()
         self._w_temb = torch.cat(ws, 0).contiguous()
         self._b_temb = torch.cat(bs, 0).contiguous()
-        # the 4-channel ends run on the tensor-core GEMM: conv_in weight flattened [320, 36] -> [320, 64] (zero pad);
-        # conv_out weight tap-major with Cout padded 4 -> 16.  The 9-channel inpainting conv_in pads 81 -> 128: two
-        # whole 64-wide K blocks, like every other GEMM caller (none runs a partial K block)
-        w_in = self.conv_in.weight.detach()
-        co, ci = w_in.shape[0], w_in.shape[1]
-        if ci != self.config.in_channels:
-            raise IHError(f"UNet2DConditionModel: config.in_channels = {self.config.in_channels} but conv_in.weight has "
-                          f"{ci} input channels")
-        self._w_in = torch.zeros((co, 64 if ci == 4 else 128), dtype=w_in.dtype, device=w_in.device)
-        self._w_in[:, : ci * 9] = w_in.reshape(co, ci * 9)
-        w_out = ops.pack_conv3x3_weight(self.conv_out.weight.detach())            # [4, 9*320]
-        self._w_out = torch.zeros((16, w_out.shape[1]), dtype=w_out.dtype, device=w_out.device)
-        self._w_out[: w_out.shape[0]] = w_out
-        self._b_out = torch.zeros((16,), dtype=w_out.dtype, device=w_out.device)
-        self._b_out[: w_out.shape[0]] = self.conv_out.bias.detach()
+        self._finalize_ends()
         self._aug = None
         for p in self.attn_processors.values():
             if hasattr(p, "invalidate"):
                 p.invalidate()
         self.graph_epoch += 1
 
+    def _finalize_ends(self):
+        raise NotImplementedError
+
+    def _pack_conv_in(self):
+        """conv_in runs on the tensor-core GEMM over ops.im2col3x3_nchw's patch matrix: the weight flattened to
+        [320, Cin*9] and zero-padded to whole 64-wide K blocks (4 channels: 36 -> 64; 9 channels: 81 -> 128), like
+        every other GEMM caller (none runs a partial K block)."""
+        w_in = self.conv_in.weight.detach()
+        co, ci = w_in.shape[0], w_in.shape[1]
+        if ci != self.config.in_channels:
+            raise IHError(f"{type(self).__name__}: config.in_channels = {self.config.in_channels} but conv_in.weight "
+                          f"has {ci} input channels")
+        self._w_in = torch.zeros((co, 64 if ci == 4 else 128), dtype=w_in.dtype, device=w_in.device)
+        self._w_in[:, : ci * 9] = w_in.reshape(co, ci * 9)
+
     # ------------------------------------------------------------------------------------------------------------
     def prepare_conditioning(self, encoder_hidden_states: torch.Tensor, text_embeds: torch.Tensor,
                              time_ids: torch.Tensor) -> None:
-        """Everything that does not depend on the step: cross-attention K/V of all 70 attn2 layers (text and image
+        """Everything that does not depend on the step: cross-attention K/V of all attn2 layers (text and image
         tokens) and the text_time additional embedding."""
         cfg = self.config
         ehs = encoder_hidden_states
@@ -487,6 +442,15 @@ class UNet2DConditionModel(nn.Module):
                 return -1
         return (text_embeds.data_ptr(), ver(text_embeds), time_ids.data_ptr(), ver(time_ids), B)
 
+    def _ensure_conditioning(self, encoder_hidden_states, text_embeds, time_ids, B: int) -> None:
+        if self._w_temb is None:
+            raise IHError(f"{type(self).__name__}.finalize() has not been called")
+        key = None if text_embeds is None else self._aug_key(text_embeds, time_ids, B)
+        if self._aug is None or (key is not None and self._aug[0] != key):
+            if text_embeds is None:
+                raise IHError("forward() needs text_embeds/time_ids (or a prior prepare_conditioning())")
+            self.prepare_conditioning(encoder_hidden_states, text_embeds, time_ids)
+
     def time_embeddings(self, timesteps: torch.Tensor, step: Optional[torch.Tensor], B: int) -> torch.Tensor:
         """-> temb_all [B, sum(Cout)]: every ResBlock's time_emb_proj(silu(emb)) in one launch."""
         cfg = self.config
@@ -496,13 +460,85 @@ class UNet2DConditionModel(nn.Module):
                                addend=self._aug[1])
         return ops.linear_small(emb, self._w_temb, self._b_temb, act_in=True)
 
+
+class UNet2DConditionModel(SDXLEncoderModel):
+    """Native SDXL UNet. Build on the meta device + `load_state_dict(..., assign=True)` or via `from_state_dict`."""
+
+    def __init__(self, cfg: UNetConfig):
+        super().__init__()
+        if cfg.in_channels not in (4, 9):
+            raise IHError(f"UNet2DConditionModel: in_channels must be 4 (latents) or 9 (inpainting: latents | mask | "
+                          f"masked-image latents), got {cfg.in_channels}")
+        self.config = cfg
+        boc = cfg.block_out_channels
+        tl = cfg.transformer_layers_per_block
+        self.conv_in = nn.Conv2d(cfg.in_channels, boc[0], 3, padding=1)
+        self.time_embedding = TimestepEmbedding(boc[0], cfg.time_embed_dim)
+        self.add_embedding = TimestepEmbedding(cfg.add_embed_in, cfg.time_embed_dim)
+        downs = []
+        ch = boc[0]
+        for i, co in enumerate(boc):
+            downs.append(DownBlock(cfg, ch, co, tl[i], add_down=i < len(boc) - 1))
+            ch = co
+        self.down_blocks = nn.ModuleList(downs)
+        rev = list(reversed(boc))
+        rtl = list(reversed(tl))
+        ups = []
+        prev = rev[0]
+        for i, co in enumerate(rev):
+            skip_ch = rev[min(i + 1, len(rev) - 1)]
+            ups.append(UpBlock(cfg, prev, skip_ch, co, rtl[i], add_up=i < len(rev) - 1))
+            prev = co
+        self.up_blocks = nn.ModuleList(ups)
+        self.mid_block = MidBlock(cfg, boc[-1], tl[-1])
+        self.conv_norm_out = nn.GroupNorm(cfg.norm_num_groups, boc[0], eps=1e-5)
+        self.conv_out = nn.Conv2d(boc[0], cfg.out_channels, 3, padding=1)
+
+    def install_default_processors(self, scale: float = 1.0):
+        """IPAdapter.set_ip_adapter (ip_adapter.py:99-125) for this UNet; IP weights are zero until loaded."""
+        from ip_adapter.attention_processor import AttnProcessor2_0, IPAttnProcessor2_0
+        cfg = self.config
+        procs = {}
+        dev = self.conv_in.weight.device
+        for name, attn in self._attn_modules():
+            if name.endswith("attn1"):
+                procs[name + ".processor"] = AttnProcessor2_0()
+            else:
+                C = attn.to_q.weight.shape[0]
+                with torch.device("meta"):
+                    p = IPAttnProcessor2_0(C, cfg.cross_attention_dim, scale=scale, num_tokens=cfg.num_ip_tokens,
+                                           skip=cfg.ip_target_substring not in name)
+                p = p.to_empty(device=dev).half()
+                for q in p.parameters():
+                    q.data.zero_()
+                    q.requires_grad_(False)
+                procs[name + ".processor"] = p
+        self.set_attn_processor(procs)
+        return procs
+
+    def _finalize_ends(self):
+        # conv_in and conv_out run on the tensor-core GEMM: conv_in as in _pack_conv_in; conv_out weight tap-major with
+        # Cout padded 4 -> 16
+        self._pack_conv_in()
+        w_out = ops.pack_conv3x3_weight(self.conv_out.weight.detach())            # [4, 9*320]
+        self._w_out = torch.zeros((16, w_out.shape[1]), dtype=w_out.dtype, device=w_out.device)
+        self._w_out[: w_out.shape[0]] = w_out
+        self._b_out = torch.zeros((16,), dtype=w_out.dtype, device=w_out.device)
+        self._b_out[: w_out.shape[0]] = self.conv_out.bias.detach()
+
     def forward(self, sample: torch.Tensor, timesteps: torch.Tensor, encoder_hidden_states: torch.Tensor,
                 text_embeds: Optional[torch.Tensor] = None, time_ids: Optional[torch.Tensor] = None,
-                step: Optional[torch.Tensor] = None, cond: Optional[torch.Tensor] = None) -> torch.Tensor:
+                step: Optional[torch.Tensor] = None, cond: Optional[torch.Tensor] = None,
+                controlnet_residuals=None) -> torch.Tensor:
         """sample NCHW fp16 [B,4,H,W]; timesteps fp32 device tensor ([B] values, or the whole schedule when `step`
         -- a device int32 index -- is given); returns noise prediction NCHW fp16.  The 9-channel inpainting UNet also
         takes `cond` NCHW fp16 [B,5,H,W] (mask | masked-image latents), which conv_in reads after the 4 latent channels;
-        the 4-channel UNet takes no `cond`."""
+        the 4-channel UNet takes no `cond`.
+
+        `controlnet_residuals` = (ControlNetOutput, row offset in images): diffusers' down_block_additional_residuals
+        and mid_block_additional_residual.  Residual k, times the output's scale[k], is added to skip k (9 of them) and
+        to the mid-block output, into the rows of the images from the offset on (n in guess mode: the ControlNet ran on
+        the conditional half only, the unconditional half gets nothing)."""
         if self._w_temb is None:
             raise IHError("UNet2DConditionModel.finalize() has not been called")
         B = sample.shape[0]
@@ -513,11 +549,7 @@ class UNet2DConditionModel(nn.Module):
         if n_cond > 0 and (cond is None or tuple(cond.shape) != (B, n_cond) + tuple(sample.shape[2:])):
             raise IHError(f"UNet2DConditionModel: the {self.config.in_channels}-channel UNet needs `cond` of shape "
                           f"{(B, n_cond) + tuple(sample.shape[2:])}, got {None if cond is None else tuple(cond.shape)}")
-        key = None if text_embeds is None else self._aug_key(text_embeds, time_ids, B)
-        if self._aug is None or (key is not None and self._aug[0] != key):
-            if text_embeds is None:
-                raise IHError("forward() needs text_embeds/time_ids (or a prior prepare_conditioning())")
-            self.prepare_conditioning(encoder_hidden_states, text_embeds, time_ids)
+        self._ensure_conditioning(encoder_hidden_states, text_embeds, time_ids, B)
         temb_all = self.time_embeddings(timesteps, step, B)
         Bs, _, Hs, Ws = sample.shape
         kpad = self._w_in.shape[1]
@@ -528,6 +560,15 @@ class UNet2DConditionModel(nn.Module):
         for blk in self.down_blocks:
             x = blk(x, temb_all, ehs, skips)
         x = self.mid_block(x, temb_all, ehs)
+        if controlnet_residuals is not None:
+            # in place, and only here: the mid block has consumed skips[-1] (its input), and no skip is read again
+            # before the up blocks pop them, so nothing sees a skip both before and after the addition
+            cn, images = controlnet_residuals
+            targets = skips + [x]
+            if len(cn.residuals) != len(targets):
+                raise IHError(f"controlnet_residuals: {len(cn.residuals)} residuals for {len(targets)} skip tensors")
+            ops.controlnet_add_residuals(targets, cn.residuals, cn.scale,
+                                         [images * (t.numel() // (t.shape[-1] * B)) for t in targets])
         for blk in self.up_blocks:
             x = blk(x, temb_all, ehs, skips)
         x = ops.groupnorm(x, self.conv_norm_out.weight, self.conv_norm_out.bias, groups=self.config.norm_num_groups,

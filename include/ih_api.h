@@ -313,6 +313,32 @@ int ih_scale_model_input(const void* latents, void* model_in, const void* sigmas
 int ih_scale_model_input_ex(const void* latents, void* model_in, const void* sigmas, const void* step, long long total,
                             int duplicate, void* stream);
 
+/* 3x3 conv, pad 1, stride 1 or 2, for the small channel counts of the ControlNet conditioning embedding ([3P] diffusers
+ * ControlNetConditioningEmbedding: 3/16/32/96 input channels, which the implicit-GEMM conv cannot take).
+ *   out[b, yo, xo, co] = fp16(act(bias[co] + sum_{tap, ci} x[b, yo*stride + ky - 1, xo*stride + kx - 1, ci] w[co, tap, ci]))
+ * with fp32 accumulation, act = SiLU when silu = 1.  x is read through the element strides (sb, sh, sw, sc), so NCHW
+ * and NHWC inputs both work; w is tap-major [Cout, 9 * Cin] (ops.pack_conv3x3_weight); bias may be NULL; out is NHWC
+ * [B, Ho, Wo, Cout] contiguous with Ho = ceil(H / stride), Wo = ceil(W / stride). */
+int ih_conv3x3_small_f16(const void* x, long long sb, long long sh, long long sw, long long sc, const void* w,
+                         const void* bias, void* out, int B, int H, int W, int Cin, int Cout, int stride, int silu,
+                         void* stream);
+
+/* ControlNet residual injection ([3P] diffusers UNet2DConditionModel with down_block_additional_residuals /
+ * mid_block_additional_residual): for each entry k, in place on rows [skip_row0, skip_row0 + rows) of `skip`
+ * ([*, channels] contiguous fp16),  skip = fp16(skip + fp16(residual * scale[k]))  with residual [rows, channels]
+ * contiguous fp16 and scale a device fp32 vector of n_entries values.  One launch for all entries; the entries are
+ * copied into the kernel's arguments (a captured graph keeps them), the scales are read from device memory at run
+ * time.  channels must be a multiple of 8 and both pointers 16-byte aligned. */
+#define IH_CN_MAX_RESIDUALS 16
+typedef struct IhCnResidual {
+  void* skip;
+  const void* residual;
+  long long rows;
+  long long skip_row0;
+  int channels;
+} IhCnResidual;
+int ih_controlnet_add_residuals_f16(const IhCnResidual* entries, int n_entries, const void* scale, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -196,9 +196,49 @@ class IPAttnProcessor2_0(torch.nn.Module):
         return out.reshape(B, N, C)
 
 
-# names the reference exports for torch < 2 / ControlNet are intentionally absent (out of scope, SURVEY.md section 2)
+class CNAttnProcessor2_0(AttnProcessor2_0):
+    """The processor IPAdapter installs on a ControlNet -- reference CNAttnProcessor2_0 (:534-621): self-attention as
+    AttnProcessor2_0, cross-attention over the text tokens only (the last `num_tokens` image-prompt tokens are
+    dropped, :570-571), so the ControlNet never sees the image prompt.  Like the reference it is one object installed
+    on every attention module.  Cross-attention is delegated to one text-only IPAttnProcessor2_0 (skip=True) per
+    module, which caches that module's step-invariant text K/V; its unused image-prompt weights stay on the meta
+    device (no memory), and it is not a registered submodule, so this processor has no parameters."""
+
+    def __init__(self, num_tokens=4):
+        super().__init__()
+        self.num_tokens = num_tokens
+        self._text = {}                # id(attn) -> IPAttnProcessor2_0(skip=True) of that attention module
+
+    def _text_processor(self, attn) -> IPAttnProcessor2_0:
+        p = self._text.get(id(attn))
+        if p is None:
+            C, D = attn.to_q.weight.shape[0], attn.to_k.weight.shape[1]
+            with torch.device("meta"):
+                p = IPAttnProcessor2_0(C, D, num_tokens=self.num_tokens, skip=True)
+            self._text[id(attn)] = p
+        return p
+
+    def invalidate(self):
+        """Drop the cached K/V (weights changed); the owner bumps its graph epoch."""
+        self._text = {}
+
+    def prepare(self, attn, encoder_hidden_states: torch.Tensor, text_only: Optional[torch.Tensor] = None):
+        return self._text_processor(attn).prepare(attn, encoder_hidden_states, text_only=text_only)
+
+    def __call__(self, attn, hidden_states, encoder_hidden_states=None, attention_mask=None, temb=None,
+                 residual: Optional[torch.Tensor] = None, ln_stats: Optional[torch.Tensor] = None,
+                 ln_eps: float = 1e-5, stats_out: Optional[torch.Tensor] = None):
+        if encoder_hidden_states is None:
+            return super().__call__(attn, hidden_states, None, attention_mask, temb, residual=residual,
+                                    ln_stats=ln_stats, ln_eps=ln_eps, stats_out=stats_out)
+        return self._text_processor(attn)(attn, hidden_states, encoder_hidden_states, attention_mask, temb,
+                                          residual=residual, ln_stats=ln_stats, ln_eps=ln_eps, stats_out=stats_out)
+
+
+# names the reference exports for torch < 2 are intentionally absent (out of scope, SURVEY.md section 2)
 AttnProcessor = AttnProcessor2_0
 IPAttnProcessor = IPAttnProcessor2_0
+CNAttnProcessor = CNAttnProcessor2_0
 
 # `from ip_adapter.attention_processor import Cross_Attention` (train.py:32): HarmonyAttention's attention block
 # (attention_processor.py:12-56) lives with the adapter modules

@@ -26,7 +26,7 @@ import torch
 
 from imagharmony_b200 import ops
 from imagharmony_b200._lib import IHError
-from imagharmony_b200.config import SDXL_BASE, UNetConfig
+from imagharmony_b200.config import SDXL_BASE, SDXL_CONTROLNET, ControlNetConfig, UNetConfig
 from imagharmony_b200.denoise import DenoiseEngine
 from imagharmony_b200.scheduler import (DPMSolverMultistepScheduler, EulerAncestralDiscreteScheduler,
                                         EulerDiscreteScheduler)
@@ -246,22 +246,15 @@ class StableDiffusionXLCustomPipeline:
         lat = self.prepare_latents(batch, self.unet.config.in_channels, height, width, torch.float16, self.device,
                                    generator, latents)                               # :255-265
 
-        def time_ids(size, crop, target):                                             # :277-284 _get_add_time_ids [3P]
-            return torch.tensor([list(size) + list(crop) + list(target)], dtype=torch.float32).repeat(batch, 1)
-        add_time_ids = time_ids(original_size, crops_coords_top_left, target_size)
-        negative_add_time_ids = None
-        if negative_original_size is not None and negative_target_size is not None:   # :285-294
-            negative_add_time_ids = time_ids(negative_original_size, negative_crops_coords_top_left, negative_target_size)
+        add_time_ids, negative_add_time_ids = self._add_time_ids(
+            batch, (original_size, crops_coords_top_left, target_size, negative_original_size,
+                    negative_crops_coords_top_left, negative_target_size))
         loop_steps = num_inference_steps
         if denoising_end is not None and isinstance(denoising_end, float) and 0 < denoising_end < 1:   # :307-316
             n_train = self.scheduler.num_train_timesteps
             cutoff = int(round(n_train - denoising_end * n_train))
             loop_steps = int(sum(1 for t in self.scheduler.timesteps if t >= cutoff))
-        conditioning_scale = 1.0
-        for attn_processor in self.unet.attn_processors.values():                     # :319-322
-            if isinstance(attn_processor, IPAttnProcessor):
-                conditioning_scale = attn_processor.scale
-                break
+        conditioning_scale = self._ip_scale()                                         # :319-322
         if loop_steps > 0:
             out = self.engine.run(lat, prompt_embeds, negative_prompt_embeds, pooled_prompt_embeds,
                                   negative_pooled_prompt_embeds, add_time_ids, num_inference_steps,
@@ -274,6 +267,27 @@ class StableDiffusionXLCustomPipeline:
             out = lat.to(self.device)
         self.set_scale(conditioning_scale)
         return self._output(out, output_type, return_dict)
+
+    @staticmethod
+    def _add_time_ids(batch: int, sizes) -> Tuple[torch.Tensor, Optional[torch.Tensor]]:
+        """:277-294 [3P] _get_add_time_ids: (positive, negative or None) micro-conditioning ids [batch, 6] from `sizes` =
+        (original_size, crops_coords_top_left, target_size, negative_original_size, negative_crops_coords_top_left,
+        negative_target_size); requires_aesthetics_score = False."""
+        original_size, crops, target_size, neg_original_size, neg_crops, neg_target_size = sizes
+
+        def time_ids(size, crop, target):
+            return torch.tensor([list(size) + list(crop) + list(target)], dtype=torch.float32).repeat(batch, 1)
+        negative = None
+        if neg_original_size is not None and neg_target_size is not None:
+            negative = time_ids(neg_original_size, neg_crops, neg_target_size)
+        return time_ids(original_size, crops, target_size), negative
+
+    def _ip_scale(self) -> float:
+        """The IP scale of the first image-prompt processor (:319-322), 1.0 without one."""
+        for attn_processor in self.unet.attn_processors.values():
+            if isinstance(attn_processor, IPAttnProcessor):
+                return attn_processor.scale
+        return 1.0
 
     def _require_latent_unet(self) -> None:
         """Text-to-image and image-to-image have no mask to feed the 9-channel inpainting UNet."""
@@ -488,26 +502,13 @@ class StableDiffusionXLImg2ImgPipeline(StableDiffusionXLCustomPipeline):
                       inpaint=None, generator=None, unet_cond=None) -> torch.Tensor:
         """The loop over timesteps[t_start:], truncated by denoising_end, from the noised start latents `lat`; the
         micro-conditioning time ids are formed from `sizes` (requires_aesthetics_score = False). -> final latents."""
-        batch = embeds[0].shape[0]
-        original_size, crops_coords_top_left, target_size, neg_original_size, neg_crops_coords_top_left, \
-            neg_target_size = sizes
-
-        def time_ids(size, crop, target):
-            return torch.tensor([list(size) + list(crop) + list(target)], dtype=torch.float32).repeat(batch, 1)
-        add_time_ids = time_ids(original_size, crops_coords_top_left, target_size)
-        negative_add_time_ids = None
-        if neg_original_size is not None and neg_target_size is not None:
-            negative_add_time_ids = time_ids(neg_original_size, neg_crops_coords_top_left, neg_target_size)
+        add_time_ids, negative_add_time_ids = self._add_time_ids(embeds[0].shape[0], sizes)
         loop_end = num_inference_steps
         if denoising_end is not None and isinstance(denoising_end, float) and 0 < denoising_end < 1:
             n_train = self.scheduler.num_train_timesteps
             cutoff = int(round(n_train - denoising_end * n_train))
             loop_end = t_start + int(sum(1 for t in self.scheduler.timesteps[t_start:] if t >= cutoff))
-        conditioning_scale = 1.0
-        for attn_processor in self.unet.attn_processors.values():
-            if isinstance(attn_processor, IPAttnProcessor):
-                conditioning_scale = attn_processor.scale
-                break
+        conditioning_scale = self._ip_scale()
         if loop_end > t_start:
             out = self.engine.run(lat, *embeds, add_time_ids, num_inference_steps,
                                   guidance_scale=guidance_scale, ip_scale=conditioning_scale,
@@ -739,3 +740,151 @@ class StableDiffusionXLInpaintPipeline(StableDiffusionXLImg2ImgPipeline):
                               for g in generator[:n]]).contiguous()
         return torch.randn((n,) + shape, generator=generator,
                            device=generator.device if generator is not None else "cpu", dtype=dtype).to(self.device)
+
+
+def preprocess_control_image(image, height: Optional[int] = None, width: Optional[int] = None,
+                             vae_scale_factor: int = 8) -> torch.Tensor:
+    """[3P] diffusers VaeImageProcessor(do_convert_rgb=True, do_normalize=False).preprocess, the ControlNet pipeline's
+    control-image processor: PIL image(s) -> RGB, Lanczos resize to width x height, / 255; a [B, 3, H, W] / [3, H, W]
+    tensor in [0, 1] is resized with nearest interpolation.  Without height / width the first image's size floored to
+    multiples of `vae_scale_factor` is used.  -> float32 [B, 3, height, width] in [0, 1]."""
+    import numpy as np
+    from PIL import Image
+    if isinstance(image, Image.Image) or (isinstance(image, (list, tuple)) and image and isinstance(image[0], Image.Image)):
+        images = [image] if isinstance(image, Image.Image) else list(image)
+        w0, h0 = images[0].size
+        h = height if height is not None else h0 - h0 % vae_scale_factor
+        w = width if width is not None else w0 - w0 % vae_scale_factor
+        if h <= 0 or w <= 0:
+            raise ValueError(f"control image of size {images[0].size} is smaller than {vae_scale_factor} pixels")
+        images = [im.convert("RGB") if im.mode != "RGB" else im for im in images]
+        images = [im if im.size == (w, h) else im.resize((w, h), resample=Image.LANCZOS) for im in images]
+        arr = np.stack([np.array(im).astype(np.float32) / 255.0 for im in images])
+        return torch.from_numpy(arr).permute(0, 3, 1, 2).contiguous()
+    if isinstance(image, torch.Tensor):
+        x = image.unsqueeze(0) if image.dim() == 3 else image
+        if x.dim() != 4 or x.shape[1] != 3:
+            raise ValueError(f"control image tensor must be [B, 3, H, W] or [3, H, W], got {tuple(image.shape)}")
+        x = x.float()
+        h = height if height is not None else x.shape[2] - x.shape[2] % vae_scale_factor
+        w = width if width is not None else x.shape[3] - x.shape[3] % vae_scale_factor
+        if h <= 0 or w <= 0:
+            raise ValueError(f"control image of size {tuple(x.shape[2:])} is smaller than {vae_scale_factor} pixels")
+        if (h, w) != tuple(x.shape[2:]):
+            x = torch.nn.functional.interpolate(x, size=(h, w))
+        return x.contiguous()
+    raise ValueError(f"`image` must be a PIL image, a list of them or a tensor, got {type(image).__name__}")
+
+
+class StableDiffusionXLControlNetPipeline(StableDiffusionXLCustomPipeline):
+    """Text-to-image with one SDXL ControlNet, with the call surface of [3P] diffusers
+    `StableDiffusionXLControlNetPipeline`, so that `IPAdapterXL(controlnet_pipe, ...).generate(pil_image=...,
+    image=control, controlnet_conditioning_scale=s)` works as on the reference (ip_adapter.py:128-133 installs
+    CNAttnProcessor on `pipe.controlnet`).  Every step runs the ControlNet and adds its residuals to the UNet's skip
+    connections inside the replayed step graph (DenoiseEngine.run(controlnet=...)).
+
+    Note: here `control_guidance_start` / `control_guidance_end` gate the CONTROLNET (it runs at step i only when
+    i/T >= start and (i+1)/T <= end), as in diffusers' ControlNet pipeline -- not the IP-adapter scale, which the
+    reference's text-to-image pipeline gates with the same names (custom_pipelines.py:326-329).  The IP scale is not
+    gated here.  Multi-ControlNet, `global_pool_conditions` models, ControlNet image-to-image / inpainting,
+    `denoising_end` and the diffusers arguments in UNSUPPORTED raise IHError."""
+
+    UNSUPPORTED = ("denoising_end", "timesteps", "sigmas", "ip_adapter_image", "ip_adapter_image_embeds", "clip_skip",
+                   "callback_on_step_end", "strength", "mask_image")
+
+    def __init__(self, unet: UNet2DConditionModel, controlnet, prompt_encoder: Optional[Callable] = None,
+                 vae_decode: Optional[Callable] = None, scheduler=None, vae=None):
+        if isinstance(controlnet, (list, tuple)):
+            raise IHError("Multi-ControlNet (a list of ControlNets) is not supported: pass one ControlNetModel")
+        super().__init__(unet, prompt_encoder=prompt_encoder, vae_decode=vae_decode, scheduler=scheduler, vae=vae)
+        self.controlnet = controlnet
+
+    @classmethod
+    def from_random(cls, cfg: UNetConfig = SDXL_BASE, controlnet_cfg: ControlNetConfig = SDXL_CONTROLNET, seed: int = 0,
+                    device="cuda", vae_cfg=None):
+        """Random-init UNet and ControlNet weights (every weight random, zero convs included)."""
+        from imagharmony_b200.controlnet import ControlNetModel
+        from imagharmony_b200.weights import random_state_dict, shapes_of
+        base = StableDiffusionXLCustomPipeline.from_random(cfg, seed=seed, device=device, vae_cfg=vae_cfg)
+        with torch.device("meta"):
+            shapes = shapes_of(ControlNetModel(controlnet_cfg))
+        gen_dev = device if str(device).startswith("cuda") else "cpu"
+        cn = ControlNetModel.from_state_dict(controlnet_cfg, random_state_dict(shapes, seed + 23, device=gen_dev),
+                                             device=device)
+        return cls(base.unet, cn, vae=base.vae)
+
+    @classmethod
+    def from_pretrained(cls, path: str, controlnet=None, torch_dtype=torch.float16, add_watermarker: bool = False,
+                        device="cuda", cfg: Optional[UNetConfig] = None, vae_cfg=None, **kwargs):
+        """`controlnet=ControlNetModel.from_pretrained(dir)` with the SDXL folder `path` of
+        StableDiffusionXLCustomPipeline.from_pretrained."""
+        if controlnet is None:
+            raise ValueError("StableDiffusionXLControlNetPipeline.from_pretrained needs controlnet=")
+        unet, enc, vae, _, _ = cls._load_pretrained(path, torch_dtype, device, cfg, vae_cfg)
+        return cls(unet, controlnet, prompt_encoder=enc, vae=vae)
+
+    @torch.no_grad()
+    def __call__(self, prompt: Optional[Union[str, List[str]]] = None, prompt_2=None, image=None,
+                 height: Optional[int] = None, width: Optional[int] = None, num_inference_steps: int = 50,
+                 guidance_scale: float = 5.0, negative_prompt=None, negative_prompt_2=None,
+                 num_images_per_prompt: Optional[int] = 1, eta: float = 0.0, generator=None,
+                 latents: Optional[torch.Tensor] = None, prompt_embeds: Optional[torch.Tensor] = None,
+                 negative_prompt_embeds: Optional[torch.Tensor] = None,
+                 pooled_prompt_embeds: Optional[torch.Tensor] = None,
+                 negative_pooled_prompt_embeds: Optional[torch.Tensor] = None, output_type: Optional[str] = "pil",
+                 return_dict: bool = True, callback=None, callback_steps: int = 1,
+                 cross_attention_kwargs: Optional[Dict[str, Any]] = None, controlnet_conditioning_scale: float = 1.0,
+                 guess_mode: bool = False, control_guidance_start: float = 0.0, control_guidance_end: float = 1.0,
+                 original_size: Optional[Tuple[int, int]] = None, crops_coords_top_left: Tuple[int, int] = (0, 0),
+                 target_size: Optional[Tuple[int, int]] = None, negative_original_size=None,
+                 negative_crops_coords_top_left=(0, 0), negative_target_size=None, guidance_rescale: float = 0.0,
+                 **kwargs):
+        """diffusers' parameter list: `image` is the control image (PIL image(s) or a tensor in [0, 1]); height and
+        width default to its size floored to multiples of 8.  Unknown keywords are ignored as in the text-to-image
+        pipeline, except the arguments in UNSUPPORTED, which raise IHError."""
+        from imagharmony_b200.controlnet import ControlNetCall, controlnet_keep
+        self._require_latent_unet()
+        refused = [k for k in self.UNSUPPORTED if kwargs.get(k) is not None]
+        if refused:
+            raise IHError(f"StableDiffusionXLControlNetPipeline does not implement {refused}")
+        if isinstance(controlnet_conditioning_scale, (list, tuple)) or isinstance(control_guidance_start, (list, tuple)) \
+                or isinstance(control_guidance_end, (list, tuple)):
+            raise IHError("Multi-ControlNet (lists of scales / guidance windows) is not supported")
+        if image is None:
+            raise ValueError("`image` (the control image) cannot be undefined")
+        if not 0.0 <= control_guidance_start < control_guidance_end <= 1.0:      # [3P] check_inputs
+            raise ValueError(f"control guidance window [{control_guidance_start}, {control_guidance_end}] must satisfy "
+                             "0 <= start < end <= 1")
+        if callback is not None and (not isinstance(callback_steps, int) or callback_steps <= 0):
+            raise ValueError(f"`callback_steps` has to be a positive integer but is {callback_steps}")
+        control = preprocess_control_image(image, height, width, self.vae_scale_factor)
+        height, width = control.shape[2], control.shape[3]
+        if height % 8 or width % 8:
+            raise ValueError(f"`height` and `width` have to be divisible by 8 but are {height} and {width}.")
+        do_classifier_free_guidance = guidance_scale > 1.0
+        (prompt_embeds, negative_prompt_embeds, pooled_prompt_embeds, negative_pooled_prompt_embeds) = \
+            self.encode_prompt(prompt, prompt_2, None, num_images_per_prompt, do_classifier_free_guidance,
+                               negative_prompt, negative_prompt_2, prompt_embeds, negative_prompt_embeds,
+                               pooled_prompt_embeds, negative_pooled_prompt_embeds)
+        batch = prompt_embeds.shape[0]
+        # [3P] prepare_image: repeat_interleave by the batch (one image) or by num_images_per_prompt; the CFG copy is
+        # the engine's (the embedding is computed once and duplicated)
+        control = control.repeat_interleave(batch if control.shape[0] == 1 else (num_images_per_prompt or 1), dim=0)
+        if control.shape[0] != batch:
+            raise ValueError(f"a control-image batch of {control.shape[0]} does not match the prompt batch of {batch}")
+        self.scheduler.set_timesteps(num_inference_steps)
+        lat = self.prepare_latents(batch, self.unet.config.in_channels, height, width, torch.float16, self.device,
+                                   generator, latents)
+        add_time_ids, negative_add_time_ids = self._add_time_ids(
+            batch, (original_size or (height, width), crops_coords_top_left, target_size or (height, width),
+                    negative_original_size, negative_crops_coords_top_left, negative_target_size))
+        ip_scale = self._ip_scale()
+        cn = ControlNetCall(self.controlnet, control.half(), float(controlnet_conditioning_scale), bool(guess_mode),
+                            controlnet_keep(num_inference_steps, control_guidance_start, control_guidance_end))
+        out = self.engine.run(lat, prompt_embeds, negative_prompt_embeds, pooled_prompt_embeds,
+                              negative_pooled_prompt_embeds, add_time_ids, num_inference_steps,
+                              guidance_scale=guidance_scale, ip_scale=ip_scale, guidance_rescale=guidance_rescale,
+                              callback=callback, callback_steps=callback_steps,
+                              negative_time_ids=negative_add_time_ids, generator=generator, controlnet=cn)
+        self.set_scale(ip_scale)
+        return self._output(out, output_type, return_dict)

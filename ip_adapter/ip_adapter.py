@@ -25,9 +25,10 @@ from .utils import get_generator, is_torch2_available
 
 if is_torch2_available():
     from .attention_processor import AttnProcessor2_0 as AttnProcessor
+    from .attention_processor import CNAttnProcessor2_0 as CNAttnProcessor
     from .attention_processor import IPAttnProcessor2_0 as IPAttnProcessor
 else:  # pragma: no cover
-    from .attention_processor import AttnProcessor, IPAttnProcessor
+    from .attention_processor import AttnProcessor, CNAttnProcessor, IPAttnProcessor
 
 
 DEFAULT_PROMPT = "best quality, high quality"                                           # reference :276, :441
@@ -110,9 +111,8 @@ class IPAdapter:
     # ---- reference :99-133 ------------------------------------------------------------------------------------------
     def set_ip_adapter(self):
         """One processor per attention module: plain for self-attention, decoupled image-prompt processors for the 70
-        cross-attention modules -- with the image branch switched on only inside IP_LAYER_MARKER."""
-        if hasattr(self.pipe, "controlnet"):
-            raise IHError("ControlNet pipelines are outside the SDXL IP-adapter hot path")
+        cross-attention modules -- with the image branch switched on only inside IP_LAYER_MARKER.  On a ControlNet
+        pipeline the ControlNet gets CNAttnProcessor (reference :128-133): it sees the text tokens only."""
         cfg = self.pipe.unet.config
         table = {}
         for name in self.pipe.unet.attn_processors:
@@ -128,6 +128,10 @@ class IPAdapter:
                 prm.zero_()                       # inert until load_ip_adapter fills to_k_ip / to_v_ip
             table[name] = proc
         self.pipe.unet.set_attn_processor(table)
+        if hasattr(self.pipe, "controlnet"):
+            if isinstance(self.pipe.controlnet, (list, tuple)):
+                raise IHError("Multi-ControlNet (a list of ControlNets) is not supported")
+            self.pipe.controlnet.set_attn_processor(CNAttnProcessor(num_tokens=self.num_tokens))
 
     # ---- reference :135-154 -----------------------------------------------------------------------------------------
     def load_ip_adapter(self):
