@@ -28,6 +28,15 @@ class IhCnResidual(ctypes.Structure):
                 ("channels", c_int)]
 
 
+IH_CN_MAX_NETS = 8      # include/ih_api.h
+
+
+class IhCnMultiResidual(ctypes.Structure):
+    """One entry of ih_controlnet_add_residuals_multi_f16 (include/ih_api.h)."""
+    _fields_ = [("skip", c_void_p), ("rows", c_longlong), ("skip_row0", c_longlong), ("channels", c_int),
+                ("residual", c_void_p * IH_CN_MAX_NETS)]
+
+
 def source_hash() -> str:
     """sha256 over the CUDA / header sources the library is built from (name + content, sorted)."""
     import hashlib
@@ -140,6 +149,8 @@ SIGNATURES = {
     "ih_conv3x3_small_f16": (c_int, [c_void_p, c_longlong, c_longlong, c_longlong, c_longlong, c_void_p, c_void_p,
                                      c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p]),
     "ih_controlnet_add_residuals_f16": (c_int, [ctypes.POINTER(IhCnResidual), c_int, c_void_p, c_void_p]),
+    "ih_controlnet_add_residuals_multi_f16": (c_int, [ctypes.POINTER(IhCnMultiResidual), c_int,
+                                                      ctypes.POINTER(c_void_p), c_int, c_void_p]),
 }
 
 _lib = None

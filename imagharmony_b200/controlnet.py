@@ -20,7 +20,7 @@ import torch
 import torch.nn as nn
 
 from . import ops
-from ._lib import IHError
+from ._lib import IH_CN_MAX_NETS, IHError
 from .config import ControlNetConfig
 from .unet import DownBlock, MidBlock, SDXLEncoderModel, TimestepEmbedding
 
@@ -102,7 +102,7 @@ class ControlNetModel(SDXLEncoderModel):
     def __init__(self, cfg: ControlNetConfig):
         super().__init__()
         if isinstance(cfg, (list, tuple)):
-            raise IHError("Multi-ControlNet (a list of ControlNets) is not supported")
+            raise IHError("ControlNetModel takes one config: wrap several ControlNets in MultiControlNetModel")
         if cfg.global_pool_conditions:
             raise IHError("ControlNet models with global_pool_conditions = true (shuffle-style, pooled residuals) are "
                           "not supported")
@@ -215,3 +215,43 @@ class ControlNetModel(SDXLEncoderModel):
         x = self.mid_block(x, temb_all, encoder_hidden_states)
         res = [ops.linear(t.reshape(-1, t.shape[-1]), wz, bz) for t, (wz, bz) in zip(skips + [x], self._zc)]
         return ControlNetOutput(res, scale)
+
+
+class MultiControlNetModel(nn.Module):
+    """[3P] diffusers MultiControlNetModel: several ControlNets (`.nets`) whose scaled residuals are summed, in fp16 and
+    in net order, before the UNet adds them.  DenoiseEngine does not call `forward`: it runs the nets one by one and
+    sums and injects their residuals in one kernel (ops.controlnet_add_residuals_multi), with the same rounding."""
+
+    def __init__(self, nets):
+        super().__init__()
+        nets = list(nets)
+        if not nets:
+            raise IHError("Multi-ControlNet: the list of ControlNets is empty")
+        if len(nets) > IH_CN_MAX_NETS:
+            raise IHError(f"Multi-ControlNet: {len(nets)} ControlNets, at most {IH_CN_MAX_NETS} are supported")
+        for i, net in enumerate(nets):
+            if not isinstance(net, ControlNetModel):
+                raise IHError(f"Multi-ControlNet: entry {i} is {type(net).__name__}, not a ControlNetModel")
+        boc = nets[0].config.block_out_channels
+        for i, net in enumerate(nets):
+            if net.config.block_out_channels != boc:
+                raise IHError(f"Multi-ControlNet: net {i} has block_out_channels {net.config.block_out_channels}, "
+                              f"net 0 has {boc}")
+        self.nets = nn.ModuleList(nets)
+
+    def forward(self, sample: torch.Tensor, timesteps: torch.Tensor, encoder_hidden_states: torch.Tensor,
+                controlnet_cond: Sequence[torch.Tensor], conditioning_scale: Sequence[float], guess_mode: bool = False,
+                text_embeds: Optional[torch.Tensor] = None, time_ids: Optional[torch.Tensor] = None,
+                step: Optional[torch.Tensor] = None) -> List[torch.Tensor]:
+        """The eager sum: one control image and conditioning scale per net -> the 10 summed SCALED residuals [rows, C]
+        (residual_k * scale_k of each net in its dtype, then added in net order)."""
+        if len(controlnet_cond) != len(self.nets) or len(conditioning_scale) != len(self.nets):
+            raise IHError(f"Multi-ControlNet: {len(controlnet_cond)} images and {len(conditioning_scale)} scales for "
+                          f"{len(self.nets)} nets")
+        total = None
+        for net, image, cs in zip(self.nets, controlnet_cond, conditioning_scale):
+            out = net(sample, timesteps, encoder_hidden_states, controlnet_cond=image, conditioning_scale=cs,
+                      guess_mode=guess_mode, text_embeds=text_embeds, time_ids=time_ids, step=step)
+            scaled = [(r.float() * s).to(r.dtype) for r, s in zip(out.residuals, out.scale)]
+            total = scaled if total is None else [a + b for a, b in zip(total, scaled)]
+        return total

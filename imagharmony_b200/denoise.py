@@ -20,16 +20,18 @@ gives diffusers' noise (a Philox stream inside the kernel would not reproduce to
 
 Graph lifetime: a captured graph holds raw pointers.  Everything it reads lives in buffers that are owned per shape
 and never freed while the graph exists -- the engine's static inputs (`_static`, `_inpaint_static`, `_dpm_static`,
-`_cond_static`, `_ancestral_noise`, `_cn_static`: the ControlNet's conditioning embedding and scale vector), the schedule tables (`_tables`, `_coeffs`), the processors'
+`_cond_static`, `_ancestral_noise`, `_cn_static`: each ControlNet's conditioning embedding and scale vector), the schedule tables (`_tables`, `_coeffs`), the processors'
 K/V buffers and the UNet's add-embedding buffer (per-shape dicts inside those objects), and the library's grow-only
 scratch buffers whose re-allocation bumps `ops.workspace_generation()`.  A graph is replayed only if it was captured
 under the current UNet `graph_epoch` (weights / processors unchanged) and the current workspace generation; otherwise
-it is re-captured; graphs with the ControlNet also need the ControlNet's `graph_epoch` they were captured under.
+it is re-captured; a graph with ControlNets also needs each of its nets to be the object, at the `graph_epoch`, it was
+captured with (tracked per net index, so reloading one net re-captures only the graphs that contain it).
 
-ControlNet (`run(controlnet=...)`): a step runs the ControlNet forward, then the UNet with its residuals injected
-after the mid block, then the unchanged step kernel, all in the one graph.  Steps where the ControlNet is off
-(keep[i] = 0) replay the ControlNet-free graph.  The scale vector is read from device memory, so a new
-controlnet_conditioning_scale does not re-capture.
+ControlNet (`run(controlnet=...)`): a step runs the active ControlNets' forwards in net order, then the UNet with
+their residuals summed and injected after the mid block in one launch, then the unchanged step kernel, all in the one
+graph.  There is one graph per distinct set of active nets (staggered windows of K nets give at most 2K + 1); steps
+where no net is active (keep[i] = 0 for all) replay the ControlNet-free graph.  The scale vectors are read from device
+memory, so a new controlnet_conditioning_scale does not re-capture.
 """
 from __future__ import annotations
 
@@ -39,7 +41,7 @@ import numpy as np
 import torch
 
 from . import ops
-from ._lib import IHError
+from ._lib import IH_CN_MAX_NETS, IHError
 from .controlnet import controlnet_scales
 from .scheduler import DPMSolverMultistepScheduler, EulerAncestralDiscreteScheduler, EulerDiscreteScheduler
 from .unet import UNet2DConditionModel
@@ -61,10 +63,11 @@ class DenoiseEngine:
         self._tables: Dict[Tuple[str, int], Tuple[torch.Tensor, torch.Tensor, float]] = {}
         self._coeffs: Dict[Tuple[str, int], torch.Tensor] = {}         # DPM-Solver++ / Euler Ancestral coefficients
         self._ancestral_noise: Dict[Tuple[int, int, int, int], torch.Tensor] = {}   # Euler Ancestral step noise
-        self._cn_static: Dict[Tuple, dict] = {}        # ControlNet: conditioning embedding + scale vector per shape
-        # (ControlNet, graph_epoch) the ControlNet graphs were captured for.  The model object itself is kept, not its id:
-        # a freed model's id can be reused by a new one that reaches the same epoch
-        self._cn_epoch = None
+        # ControlNet: conditioning embedding + scale vector per (net index, shape)
+        self._cn_static: Dict[Tuple, dict] = {}
+        # net index -> (ControlNet, graph_epoch) the graphs with that net were captured for.  The model object itself is
+        # kept, not its id: a freed model's id can be reused by a new one that reaches the same epoch
+        self._cn_epochs: Dict[int, Tuple] = {}
         self._epoch = getattr(unet, "graph_epoch", 0)
         self.last_launches_per_step = 0
         self.graphs_captured = 0
@@ -162,10 +165,10 @@ class DenoiseEngine:
             self._cond_static[key] = buf
         return buf
 
-    def _cn_buffers(self, b: int, h: int, w: int) -> dict:
-        """ControlNet static inputs per (ControlNet batch, h, w), never freed (the graph-lifetime rule above): the
-        conditioning embedding NHWC [b, h, w, C0] and the fp32 scale vector [10], refilled by every call."""
-        key = (b, h, w)
+    def _cn_buffers(self, net: int, b: int, h: int, w: int) -> dict:
+        """ControlNet static inputs per (net index, ControlNet batch, h, w), never freed (the graph-lifetime rule above):
+        the conditioning embedding NHWC [b, h, w, C0] and the fp32 scale vector [10], refilled by every call."""
+        key = (net, b, h, w)
         cb = self._cn_static.get(key)
         if cb is None:
             C0 = self.unet.config.block_out_channels[0]
@@ -205,11 +208,12 @@ class DenoiseEngine:
     def _step(self, st, timesteps, sigmas, guidance, use_cfg=True, rescale=0.0, ib=None, dpm=None, anc=None, cond=None,
               cn=None):
         residuals = None
-        if cn is not None:          # (ControlNet, static buffers, first image of the batch it runs on)
-            model, cb, b0 = cn
-            out = model(st["model_in"][b0:], timesteps, st["ehs"][b0:], text_embeds=st["text_embeds"][b0:],
-                        time_ids=st["time_ids"][b0:], step=st["step"], cond_embedding=cb["emb"], scale=cb["scale"])
-            residuals = (out, b0)
+        if cn is not None:          # (active net indices, [(ControlNet, static buffers)], first image they run on)
+            _, nets, b0 = cn
+            outs = [model(st["model_in"][b0:], timesteps, st["ehs"][b0:], text_embeds=st["text_embeds"][b0:],
+                          time_ids=st["time_ids"][b0:], step=st["step"], cond_embedding=cb["emb"], scale=cb["scale"])
+                    for model, cb in nets]
+            residuals = (outs[0] if len(outs) == 1 else outs, b0)
         noise = self.unet(st["model_in"], timesteps, st["ehs"], st["text_embeds"], st["time_ids"], step=st["step"],
                           cond=cond, controlnet_residuals=residuals)
         if dpm is not None:
@@ -286,7 +290,12 @@ class DenoiseEngine:
         and its scaled residuals are added to the UNet's skip connections and mid-block output; at steps with keep[i] =
         0 the step is the plain one.  The control image's embedding is computed once per call.  It works with every
         scheduler and the loop options of text-to-image, not with begin_step, inpaint, unet_cond, start_step or
-        stop_after (IHError).  It draws no random numbers."""
+        stop_after (IHError).  It draws no random numbers.
+
+        `controlnet` = a sequence of ControlNetCalls (up to 8, one per net, sharing guess_mode) is a Multi-ControlNet
+        ([3P] MultiControlNetModel): at step i the nets with keep[i] = 1 run in net order and their scaled residuals
+        are summed in fp16 and added in one launch.  diffusers runs an inactive net with scale 0; skipping it is exact
+        (fp16(acc + 0) = acc).  A list of one call is the single-net case."""
         use_cfg = guidance_scale > 1.0                                            # :223
         if use_cfg and (negative_prompt_embeds is None or negative_pooled is None):
             raise IHError("classifier-free guidance needs negative_prompt_embeds / negative_pooled")
@@ -369,30 +378,35 @@ class DenoiseEngine:
         if dpm is not None:
             dpm[0]["loop_begin"].fill_(start_step)
         self.unet.prepare_conditioning(st["ehs"], st["text_embeds"], st["time_ids"])
-        cn = None
-        keep = [1.0] * T
+        nets, keeps, b_cn0 = [], [], 0          # per ControlNet: (model, static buffers), keep list; first image
         if controlnet is not None:
-            model = controlnet.model
-            if model.config.block_out_channels != ucfg.block_out_channels:
-                raise IHError("the ControlNet's block_out_channels differ from the UNet's")
-            if controlnet.keep is not None:
-                keep = [float(k) for k in controlnet.keep]
+            calls = list(controlnet) if isinstance(controlnet, (list, tuple)) else [controlnet]
+            if not 1 <= len(calls) <= IH_CN_MAX_NETS:
+                raise IHError(f"controlnet: {len(calls)} ControlNetCalls, expected 1 .. {IH_CN_MAX_NETS}")
+            guess = bool(calls[0].guess_mode)
+            if any(bool(c.guess_mode) != guess for c in calls):
+                raise IHError("controlnet: all ControlNetCalls must share guess_mode")
+            b_cn0 = n if (use_cfg and guess) else 0                 # guess mode + CFG: the conditional half only
+            b_cn = (2 * n if use_cfg else n) - b_cn0
+            for j, call in enumerate(calls):
+                model = call.model
+                if model.config.block_out_channels != ucfg.block_out_channels:
+                    raise IHError(f"ControlNet {j}: its block_out_channels differ from the UNet's")
+                keep = [1.0] * T if call.keep is None else [float(k) for k in call.keep]
                 if len(keep) != T:
-                    raise IHError(f"controlnet keep has {len(keep)} entries for a {T}-step schedule")
-            guess = bool(controlnet.guess_mode)
-            b0 = n if (use_cfg and guess) else 0                    # guess mode + CFG: the conditional half only
-            b_cn = (2 * n if use_cfg else n) - b0
-            image = controlnet.image
-            if tuple(image.shape) != (n, model.config.conditioning_channels, 8 * h, 8 * w):
-                raise IHError(f"controlnet image: expected {(n, model.config.conditioning_channels, 8 * h, 8 * w)}, "
-                              f"got {tuple(image.shape)}")
-            cb = self._cn_buffers(b_cn, h, w)
-            model.embed_condition(image.to(self.device, torch.float16).contiguous(), out=cb["emb"][:n])
-            if b_cn > n:                                            # [3P] cat([image] * 2) under CFG
-                cb["emb"][n:].copy_(cb["emb"][:n])
-            cb["scale"].copy_(controlnet_scales(controlnet.conditioning_scale, guess))
-            model.prepare_conditioning(st["ehs"][b0:], st["text_embeds"][b0:], st["time_ids"][b0:])
-            cn = (model, cb, b0)
+                    raise IHError(f"ControlNet {j}: keep has {len(keep)} entries for a {T}-step schedule")
+                image = call.image
+                if tuple(image.shape) != (n, model.config.conditioning_channels, 8 * h, 8 * w):
+                    raise IHError(f"ControlNet {j}: image: expected "
+                                  f"{(n, model.config.conditioning_channels, 8 * h, 8 * w)}, got {tuple(image.shape)}")
+                cb = self._cn_buffers(j, b_cn, h, w)
+                model.embed_condition(image.to(self.device, torch.float16).contiguous(), out=cb["emb"][:n])
+                if b_cn > n:                                        # [3P] cat([image] * 2) under CFG
+                    cb["emb"][n:].copy_(cb["emb"][:n])
+                cb["scale"].copy_(controlnet_scales(call.conditioning_scale, guess))
+                model.prepare_conditioning(st["ehs"][b_cn0:], st["text_embeds"][b_cn0:], st["time_ids"][b_cn0:])
+                nets.append((model, cb))
+                keeps.append(keep)
         self._first_input(st, sigmas, use_cfg, dpm, anc)                               # :332-334
 
         steps = loop_T if stop_after is None else min(stop_after, loop_T)
@@ -404,20 +418,23 @@ class DenoiseEngine:
             return 0.0 if off else float(ip_scale)
 
         def cn_at(i: int):
-            return cn if (cn is not None and keep[i] > 0) else None
+            # the nets with keep[i] = 1, in net order; diffusers runs the others at scale 0, which adds exactly nothing
+            active = tuple(j for j, keep in enumerate(keeps) if keep[i] > 0)
+            return (active, [nets[j] for j in active], b_cn0) if active else None
 
         def gkey(scale: float, cn_step):
             return (n, h, w, L, T, use_cfg, float(guidance_scale), rescale, scale, self.scheduler.kind, cond is not None,
-                    ib is not None, None if cn_step is None else ("controlnet", cn_step[2] > 0))
+                    ib is not None, None if cn_step is None else ("controlnet", cn_step[2] > 0, cn_step[0]))
 
         if self.use_cuda_graph:
             if self._epoch != getattr(self.unet, "graph_epoch", 0):       # weights / processors changed since capture
                 self._graphs.clear()
                 self._epoch = getattr(self.unet, "graph_epoch", 0)
-            if cn is not None and (self._cn_epoch is None or self._cn_epoch[0] is not cn[0]
-                                   or self._cn_epoch[1] != cn[0].graph_epoch):     # another / a reloaded ControlNet
-                self._graphs = {k: v for k, v in self._graphs.items() if k[-1] is None}
-                self._cn_epoch = (cn[0], cn[0].graph_epoch)
+            for j, (model, _) in enumerate(nets):
+                seen = self._cn_epochs.get(j)
+                if seen is None or seen[0] is not model or seen[1] != model.graph_epoch:   # another / a reloaded net
+                    self._graphs = {k: v for k, v in self._graphs.items() if k[-1] is None or j not in k[-1][2]}
+                    self._cn_epochs[j] = (model, model.graph_epoch)
             needed = {}
             for i in range(start_step, steps):
                 needed.setdefault(gkey(scale_at(i), cn_at(i)), (scale_at(i), cn_at(i)))

@@ -5,6 +5,7 @@ PyTorch/CPU fallback: a CPU tensor or a missing library raises.
 """
 from __future__ import annotations
 
+import ctypes
 import os
 from typing import Optional, Tuple
 
@@ -791,3 +792,42 @@ def controlnet_add_residuals(skips, residuals, scale: torch.Tensor, skip_row0s) 
                           f"{tuple(r.shape)} at row {r0}")
         table[k] = _lib.IhCnResidual(s.data_ptr(), r.data_ptr(), rows, int(r0), C)
     check(lib.ih_controlnet_add_residuals_f16(table, n, scale.data_ptr(), _stream()), "ih_controlnet_add_residuals_f16")
+
+
+def controlnet_add_residuals_multi(skips, residuals_per_net, scales_per_net, skip_row0s) -> None:
+    """ih_controlnet_add_residuals_multi_f16: for every entry k, skips[k][rows r0 .. r0 + R) = fp16(skip + acc) in
+    place with acc = fp16(r_0 * s_0[k]), then acc = fp16(acc + fp16(r_j * s_j[k])) for the nets j = 1 .. K-1 in order
+    (diffusers' MultiControlNetModel sum, then the UNet's addition), all entries and nets in one launch.
+    residuals_per_net[j][k] is net j's residual for skip k (contiguous fp16, R rows); scales_per_net[j] is net j's
+    device float32 vector with one value per entry; skip_row0s[k] is r0."""
+    lib = _lib.load()
+    K = len(residuals_per_net)
+    n = len(skips)
+    if not 1 <= K <= _lib.IH_CN_MAX_NETS or len(scales_per_net) != K:
+        raise IHError(f"controlnet_add_residuals_multi: {K} residual lists and {len(scales_per_net)} scale vectors "
+                      f"(1 .. {_lib.IH_CN_MAX_NETS} nets)")
+    if len(skip_row0s) != n or any(len(rs) != n for rs in residuals_per_net):
+        raise IHError(f"controlnet_add_residuals_multi: {n} skips, {[len(rs) for rs in residuals_per_net]} residuals "
+                      f"per net, {len(skip_row0s)} offsets")
+    for j, sc in enumerate(scales_per_net):
+        _req(sc, f"scale[{j}]", torch.float32)
+        if sc.numel() < n or not sc.is_contiguous():
+            raise IHError(f"controlnet_add_residuals_multi: net {j} has {sc.numel()} scales for {n} entries")
+    table = (_lib.IhCnMultiResidual * n)()
+    for k, (s, r0) in enumerate(zip(skips, skip_row0s)):
+        _req(s, f"skip[{k}]")
+        C = s.shape[-1]
+        rows = residuals_per_net[0][k].numel() // C
+        for j, rs in enumerate(residuals_per_net):
+            r = rs[k]
+            _req(r, f"residual[{j}][{k}]")
+            if (not s.is_contiguous() or not r.is_contiguous() or r.shape[-1] != C or r.numel() != rows * C or r0 < 0
+                    or r0 + rows > s.numel() // C):
+                raise IHError(f"controlnet_add_residuals_multi: entry {k}: skip {tuple(s.shape)} cannot take net {j}'s "
+                              f"residual {tuple(r.shape)} at row {r0}")
+        table[k] = _lib.IhCnMultiResidual(s.data_ptr(), rows, int(r0), C,
+                                          (ctypes.c_void_p * _lib.IH_CN_MAX_NETS)(
+                                              *[rs[k].data_ptr() for rs in residuals_per_net]))
+    scales = (ctypes.c_void_p * K)(*[sc.data_ptr() for sc in scales_per_net])
+    check(lib.ih_controlnet_add_residuals_multi_f16(table, n, scales, K, _stream()),
+          "ih_controlnet_add_residuals_multi_f16")

@@ -538,7 +538,9 @@ class UNet2DConditionModel(SDXLEncoderModel):
         `controlnet_residuals` = (ControlNetOutput, row offset in images): diffusers' down_block_additional_residuals
         and mid_block_additional_residual.  Residual k, times the output's scale[k], is added to skip k (9 of them) and
         to the mid-block output, into the rows of the images from the offset on (n in guess mode: the ControlNet ran on
-        the conditional half only, the unconditional half gets nothing)."""
+        the conditional half only, the unconditional half gets nothing).  With a list of ControlNetOutputs (one per net
+        of a Multi-ControlNet, one row offset for all) the nets' scaled residuals are summed in fp16 in list order and
+        the sum is added, in one launch (ops.controlnet_add_residuals_multi)."""
         if self._w_temb is None:
             raise IHError("UNet2DConditionModel.finalize() has not been called")
         B = sample.shape[0]
@@ -565,10 +567,14 @@ class UNet2DConditionModel(SDXLEncoderModel):
             # before the up blocks pop them, so nothing sees a skip both before and after the addition
             cn, images = controlnet_residuals
             targets = skips + [x]
-            if len(cn.residuals) != len(targets):
-                raise IHError(f"controlnet_residuals: {len(cn.residuals)} residuals for {len(targets)} skip tensors")
-            ops.controlnet_add_residuals(targets, cn.residuals, cn.scale,
-                                         [images * (t.numel() // (t.shape[-1] * B)) for t in targets])
+            for out in (cn if isinstance(cn, (list, tuple)) else [cn]):
+                if len(out.residuals) != len(targets):
+                    raise IHError(f"controlnet_residuals: {len(out.residuals)} residuals for {len(targets)} skip tensors")
+            row0s = [images * (t.numel() // (t.shape[-1] * B)) for t in targets]
+            if isinstance(cn, (list, tuple)):
+                ops.controlnet_add_residuals_multi(targets, [o.residuals for o in cn], [o.scale for o in cn], row0s)
+            else:
+                ops.controlnet_add_residuals(targets, cn.residuals, cn.scale, row0s)
         for blk in self.up_blocks:
             x = blk(x, temb_all, ehs, skips)
         x = ops.groupnorm(x, self.conv_norm_out.weight, self.conv_norm_out.bias, groups=self.config.norm_num_groups,

@@ -339,6 +339,26 @@ typedef struct IhCnResidual {
 } IhCnResidual;
 int ih_controlnet_add_residuals_f16(const IhCnResidual* entries, int n_entries, const void* scale, void* stream);
 
+/* Multi-ControlNet residual injection ([3P] diffusers MultiControlNetModel, whose nets' scaled residuals are summed in
+ * fp16 in net order before the UNet adds them): for each entry e, in place on rows [skip_row0, skip_row0 + rows) of
+ * `skip` ([*, channels] contiguous fp16),
+ *   acc = fp16(r_0 * s_0[e]);  acc = fp16(acc + fp16(r_k * s_k[e])) for k = 1 .. n_nets - 1;  skip = fp16(skip + acc)
+ * with r_k = residual[k] ([rows, channels] contiguous fp16) and s_k = scales[k], net k's device fp32 vector of
+ * n_entries values.  One launch for all entries and nets; entries and scale pointers are copied into the kernel's
+ * arguments, the scale values are read from device memory at run time.  n_nets = 1 computes exactly what
+ * ih_controlnet_add_residuals_f16 computes (which stays the faster single-net path).  channels must be a multiple of 8
+ * and every pointer 16-byte aligned. */
+#define IH_CN_MAX_NETS 8
+typedef struct IhCnMultiResidual {
+  void* skip;
+  long long rows;
+  long long skip_row0;
+  int channels;
+  const void* residual[IH_CN_MAX_NETS];
+} IhCnMultiResidual;
+int ih_controlnet_add_residuals_multi_f16(const IhCnMultiResidual* entries, int n_entries, const void* const* scales,
+                                          int n_nets, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -786,42 +786,87 @@ class StableDiffusionXLControlNetPipeline(StableDiffusionXLCustomPipeline):
     Note: here `control_guidance_start` / `control_guidance_end` gate the CONTROLNET (it runs at step i only when
     i/T >= start and (i+1)/T <= end), as in diffusers' ControlNet pipeline -- not the IP-adapter scale, which the
     reference's text-to-image pipeline gates with the same names (custom_pipelines.py:326-329).  The IP scale is not
-    gated here.  Multi-ControlNet, `global_pool_conditions` models, ControlNet image-to-image / inpainting,
-    `denoising_end` and the diffusers arguments in UNSUPPORTED raise IHError."""
+    gated here.
+
+    `controlnet` may also be a list of ControlNetModels, wrapped in a MultiControlNetModel as diffusers does, or a
+    MultiControlNetModel.  Then `image` is a list with one control image per net, `controlnet_conditioning_scale` a
+    float (broadcast to every net) or a list, and `control_guidance_start` / `end` floats or lists, aligned as in
+    diffusers 0.30; each net runs only inside its own window, and the active nets' residuals are summed.
+
+    `global_pool_conditions` models, ControlNet image-to-image / inpainting, several conditionings per batch entry,
+    `denoising_end` and the diffusers arguments in UNSUPPORTED raise IHError (ValueError for nested image lists)."""
 
     UNSUPPORTED = ("denoising_end", "timesteps", "sigmas", "ip_adapter_image", "ip_adapter_image_embeds", "clip_skip",
                    "callback_on_step_end", "strength", "mask_image")
 
     def __init__(self, unet: UNet2DConditionModel, controlnet, prompt_encoder: Optional[Callable] = None,
                  vae_decode: Optional[Callable] = None, scheduler=None, vae=None):
-        if isinstance(controlnet, (list, tuple)):
-            raise IHError("Multi-ControlNet (a list of ControlNets) is not supported: pass one ControlNetModel")
+        from imagharmony_b200.controlnet import MultiControlNetModel
+        if isinstance(controlnet, (list, tuple)):          # [3P] diffusers wraps a list the same way
+            controlnet = MultiControlNetModel(controlnet)
         super().__init__(unet, prompt_encoder=prompt_encoder, vae_decode=vae_decode, scheduler=scheduler, vae=vae)
         self.controlnet = controlnet
 
     @classmethod
     def from_random(cls, cfg: UNetConfig = SDXL_BASE, controlnet_cfg: ControlNetConfig = SDXL_CONTROLNET, seed: int = 0,
                     device="cuda", vae_cfg=None):
-        """Random-init UNet and ControlNet weights (every weight random, zero convs included)."""
+        """Random-init UNet and ControlNet weights (every weight random, zero convs included).  A list of ControlNet
+        configs gives a Multi-ControlNet pipeline, net j seeded with seed + 23 + 7j."""
         from imagharmony_b200.controlnet import ControlNetModel
         from imagharmony_b200.weights import random_state_dict, shapes_of
         base = StableDiffusionXLCustomPipeline.from_random(cfg, seed=seed, device=device, vae_cfg=vae_cfg)
-        with torch.device("meta"):
-            shapes = shapes_of(ControlNetModel(controlnet_cfg))
         gen_dev = device if str(device).startswith("cuda") else "cpu"
-        cn = ControlNetModel.from_state_dict(controlnet_cfg, random_state_dict(shapes, seed + 23, device=gen_dev),
-                                             device=device)
-        return cls(base.unet, cn, vae=base.vae)
+        nets = []
+        for j, c in enumerate(controlnet_cfg if isinstance(controlnet_cfg, (list, tuple)) else [controlnet_cfg]):
+            with torch.device("meta"):
+                shapes = shapes_of(ControlNetModel(c))
+            nets.append(ControlNetModel.from_state_dict(c, random_state_dict(shapes, seed + 23 + 7 * j, device=gen_dev),
+                                                        device=device))
+        return cls(base.unet, nets if isinstance(controlnet_cfg, (list, tuple)) else nets[0], vae=base.vae)
 
     @classmethod
     def from_pretrained(cls, path: str, controlnet=None, torch_dtype=torch.float16, add_watermarker: bool = False,
                         device="cuda", cfg: Optional[UNetConfig] = None, vae_cfg=None, **kwargs):
-        """`controlnet=ControlNetModel.from_pretrained(dir)` with the SDXL folder `path` of
-        StableDiffusionXLCustomPipeline.from_pretrained."""
+        """`controlnet=ControlNetModel.from_pretrained(dir)` (or a list of them, or a MultiControlNetModel) with the
+        SDXL folder `path` of StableDiffusionXLCustomPipeline.from_pretrained."""
         if controlnet is None:
             raise ValueError("StableDiffusionXLControlNetPipeline.from_pretrained needs controlnet=")
         unet, enc, vae, _, _ = cls._load_pretrained(path, torch_dtype, device, cfg, vae_cfg)
         return cls(unet, controlnet, prompt_encoder=enc, vae=vae)
+
+    def _align_multi(self, image, scale, start, end):
+        """[3P] diffusers 0.30 for a MultiControlNetModel: scalar guidance start / end become lists (the length of the
+        other list, or one entry per net), a float scale is broadcast; `image` must be a flat list with one entry per
+        net.  -> (images, scales, starts, ends), one entry per net."""
+        k = len(self.controlnet.nets)
+        if not isinstance(image, list):
+            raise TypeError("For multiple controlnets: `image` must be type `list`")
+        if any(isinstance(i, list) for i in image):
+            raise ValueError("A single batch of multiple conditionings is not supported: pass one image (or one "
+                             "batch tensor / list of PIL images) per ControlNet, not a nested list")
+        if len(image) != k:
+            raise ValueError(f"For multiple controlnets: `image` must have one entry per ControlNet, got {len(image)} "
+                             f"images and {k} ControlNets")
+        if isinstance(scale, (list, tuple)):
+            if any(isinstance(s, (list, tuple)) for s in scale):
+                raise ValueError("A single batch of multiple conditionings is not supported: "
+                                 "`controlnet_conditioning_scale` must be a flat list")
+            if len(scale) != k:
+                raise ValueError(f"`controlnet_conditioning_scale` has {len(scale)} entries for {k} ControlNets")
+            scales = [float(s) for s in scale]
+        else:
+            scales = [float(scale)] * k
+        if not isinstance(start, (list, tuple)) and isinstance(end, (list, tuple)):
+            start = [start] * len(end)
+        elif not isinstance(end, (list, tuple)) and isinstance(start, (list, tuple)):
+            end = [end] * len(start)
+        elif not isinstance(start, (list, tuple)) and not isinstance(end, (list, tuple)):
+            start, end = [start] * k, [end] * k
+        if len(start) != len(end):
+            raise ValueError(f"`control_guidance_start` has {len(start)} entries, `control_guidance_end` {len(end)}")
+        if len(start) != k:
+            raise ValueError(f"`control_guidance_start` / `end` have {len(start)} entries for {k} ControlNets")
+        return list(image), scales, [float(s) for s in start], [float(e) for e in end]
 
     @torch.no_grad()
     def __call__(self, prompt: Optional[Union[str, List[str]]] = None, prompt_2=None, image=None,
@@ -842,23 +887,34 @@ class StableDiffusionXLControlNetPipeline(StableDiffusionXLCustomPipeline):
         """diffusers' parameter list: `image` is the control image (PIL image(s) or a tensor in [0, 1]); height and
         width default to its size floored to multiples of 8.  Unknown keywords are ignored as in the text-to-image
         pipeline, except the arguments in UNSUPPORTED, which raise IHError."""
-        from imagharmony_b200.controlnet import ControlNetCall, controlnet_keep
+        from imagharmony_b200.controlnet import ControlNetCall, MultiControlNetModel, controlnet_keep
         self._require_latent_unet()
         refused = [k for k in self.UNSUPPORTED if kwargs.get(k) is not None]
         if refused:
             raise IHError(f"StableDiffusionXLControlNetPipeline does not implement {refused}")
-        if isinstance(controlnet_conditioning_scale, (list, tuple)) or isinstance(control_guidance_start, (list, tuple)) \
-                or isinstance(control_guidance_end, (list, tuple)):
-            raise IHError("Multi-ControlNet (lists of scales / guidance windows) is not supported")
+        multi = isinstance(self.controlnet, MultiControlNetModel)
+        if not multi and (isinstance(controlnet_conditioning_scale, (list, tuple))
+                          or isinstance(control_guidance_start, (list, tuple))
+                          or isinstance(control_guidance_end, (list, tuple))):
+            raise IHError("lists of scales / guidance windows need a Multi-ControlNet (a list of ControlNets)")
         if image is None:
             raise ValueError("`image` (the control image) cannot be undefined")
-        if not 0.0 <= control_guidance_start < control_guidance_end <= 1.0:      # [3P] check_inputs
-            raise ValueError(f"control guidance window [{control_guidance_start}, {control_guidance_end}] must satisfy "
-                             "0 <= start < end <= 1")
+        if multi:
+            images, scales, starts, ends = self._align_multi(image, controlnet_conditioning_scale,
+                                                             control_guidance_start, control_guidance_end)
+        else:
+            images, scales = [image], [float(controlnet_conditioning_scale)]
+            starts, ends = [control_guidance_start], [control_guidance_end]
+        for start, end in zip(starts, ends):                                  # [3P] check_inputs
+            if not 0.0 <= start < end <= 1.0:
+                raise ValueError(f"control guidance window [{start}, {end}] must satisfy 0 <= start < end <= 1")
         if callback is not None and (not isinstance(callback_steps, int) or callback_steps <= 0):
             raise ValueError(f"`callback_steps` has to be a positive integer but is {callback_steps}")
-        control = preprocess_control_image(image, height, width, self.vae_scale_factor)
-        height, width = control.shape[2], control.shape[3]
+        controls = [preprocess_control_image(im, height, width, self.vae_scale_factor) for im in images]
+        height, width = controls[0].shape[2], controls[0].shape[3]
+        if any(tuple(c.shape[2:]) != (height, width) for c in controls):
+            raise ValueError(f"the control images come out at different sizes {[tuple(c.shape[2:]) for c in controls]}; "
+                             "pass images of one size, or height and width")
         if height % 8 or width % 8:
             raise ValueError(f"`height` and `width` have to be divisible by 8 but are {height} and {width}.")
         do_classifier_free_guidance = guidance_scale > 1.0
@@ -867,11 +923,13 @@ class StableDiffusionXLControlNetPipeline(StableDiffusionXLCustomPipeline):
                                negative_prompt, negative_prompt_2, prompt_embeds, negative_prompt_embeds,
                                pooled_prompt_embeds, negative_pooled_prompt_embeds)
         batch = prompt_embeds.shape[0]
-        # [3P] prepare_image: repeat_interleave by the batch (one image) or by num_images_per_prompt; the CFG copy is
-        # the engine's (the embedding is computed once and duplicated)
-        control = control.repeat_interleave(batch if control.shape[0] == 1 else (num_images_per_prompt or 1), dim=0)
-        if control.shape[0] != batch:
-            raise ValueError(f"a control-image batch of {control.shape[0]} does not match the prompt batch of {batch}")
+        # [3P] prepare_image, per net: repeat_interleave by the batch (one image) or by num_images_per_prompt; the CFG
+        # copy is the engine's (the embedding is computed once and duplicated)
+        for j, c in enumerate(controls):
+            controls[j] = c.repeat_interleave(batch if c.shape[0] == 1 else (num_images_per_prompt or 1), dim=0)
+            if controls[j].shape[0] != batch:
+                raise ValueError(f"a control-image batch of {controls[j].shape[0]} does not match the prompt batch of "
+                                 f"{batch}")
         self.scheduler.set_timesteps(num_inference_steps)
         lat = self.prepare_latents(batch, self.unet.config.in_channels, height, width, torch.float16, self.device,
                                    generator, latents)
@@ -879,8 +937,10 @@ class StableDiffusionXLControlNetPipeline(StableDiffusionXLCustomPipeline):
             batch, (original_size or (height, width), crops_coords_top_left, target_size or (height, width),
                     negative_original_size, negative_crops_coords_top_left, negative_target_size))
         ip_scale = self._ip_scale()
-        cn = ControlNetCall(self.controlnet, control.half(), float(controlnet_conditioning_scale), bool(guess_mode),
-                            controlnet_keep(num_inference_steps, control_guidance_start, control_guidance_end))
+        models = list(self.controlnet.nets) if multi else [self.controlnet]
+        cn = [ControlNetCall(m, c.half(), s, bool(guess_mode), controlnet_keep(num_inference_steps, start, end))
+              for m, c, s, start, end in zip(models, controls, scales, starts, ends)]
+        cn = cn if multi else cn[0]
         out = self.engine.run(lat, prompt_embeds, negative_prompt_embeds, pooled_prompt_embeds,
                               negative_pooled_prompt_embeds, add_time_ids, num_inference_steps,
                               guidance_scale=guidance_scale, ip_scale=ip_scale, guidance_rescale=guidance_rescale,

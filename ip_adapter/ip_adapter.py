@@ -20,6 +20,7 @@ from PIL import Image
 
 from imagharmony_b200._lib import IHError
 from imagharmony_b200.adapter import HarmonyAttention, ImageProjModel, Resampler  # noqa: F401
+from imagharmony_b200.controlnet import MultiControlNetModel
 
 from .utils import get_generator, is_torch2_available
 
@@ -129,9 +130,11 @@ class IPAdapter:
             table[name] = proc
         self.pipe.unet.set_attn_processor(table)
         if hasattr(self.pipe, "controlnet"):
-            if isinstance(self.pipe.controlnet, (list, tuple)):
-                raise IHError("Multi-ControlNet (a list of ControlNets) is not supported")
-            self.pipe.controlnet.set_attn_processor(CNAttnProcessor(num_tokens=self.num_tokens))
+            if isinstance(self.pipe.controlnet, MultiControlNetModel):
+                for controlnet in self.pipe.controlnet.nets:
+                    controlnet.set_attn_processor(CNAttnProcessor(num_tokens=self.num_tokens))
+            else:
+                self.pipe.controlnet.set_attn_processor(CNAttnProcessor(num_tokens=self.num_tokens))
 
     # ---- reference :135-154 -----------------------------------------------------------------------------------------
     def load_ip_adapter(self):
