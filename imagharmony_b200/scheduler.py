@@ -314,3 +314,14 @@ class DPMSolverMultistepScheduler(_FromConfig):
     @property
     def coeffs(self):
         return self.schedule.coeffs
+
+
+def randn_tensor(shape, generator, dtype: torch.dtype, device, rand_device=None) -> torch.Tensor:
+    """N(0, 1) of `shape` and `dtype` on `device`, drawn as [3P] diffusers' randn_tensor draws it, so that a seed gives
+    diffusers' numbers: with a list of generators one [1, ...] draw per row, row i with generator[i] on that generator's
+    device; otherwise one draw on the generator's device, or on `rand_device` (default `device`) when it is None."""
+    if isinstance(generator, list):
+        return torch.cat([torch.randn((1,) + tuple(shape[1:]), generator=generator[i], device=generator[i].device,
+                                      dtype=dtype).to(device) for i in range(shape[0])])
+    dev = generator.device if generator is not None else (rand_device or device)
+    return torch.randn(tuple(shape), generator=generator, device=dev, dtype=dtype).to(device)

@@ -29,7 +29,7 @@ from imagharmony_b200._lib import IHError
 from imagharmony_b200.config import SDXL_BASE, SDXL_CONTROLNET, ControlNetConfig, UNetConfig
 from imagharmony_b200.denoise import DenoiseEngine
 from imagharmony_b200.scheduler import (DPMSolverMultistepScheduler, EulerAncestralDiscreteScheduler,
-                                        EulerDiscreteScheduler)
+                                        EulerDiscreteScheduler, randn_tensor)
 from imagharmony_b200.unet import UNet2DConditionModel
 
 from .utils import is_torch2_available
@@ -201,14 +201,9 @@ class StableDiffusionXLCustomPipeline:
         """[3P] diffusers prepare_latents: randn * init_noise_sigma; a list of generators draws one sample each."""
         shape = (batch_size, num_channels_latents, height // self.vae_scale_factor, width // self.vae_scale_factor)
         if latents is None:
-            if isinstance(generator, list):
-                if len(generator) != batch_size:
-                    raise ValueError(f"got {len(generator)} generators for a batch of {batch_size}")
-                parts = [torch.randn((1,) + shape[1:], generator=g, device=g.device, dtype=torch.float32) for g in generator]
-                latents = torch.cat([p.to("cpu") for p in parts], dim=0)
-            else:
-                gdev = generator.device if generator is not None else "cpu"
-                latents = torch.randn(shape, generator=generator, device=gdev, dtype=torch.float32).to("cpu")
+            if isinstance(generator, list) and len(generator) != batch_size:
+                raise ValueError(f"got {len(generator)} generators for a batch of {batch_size}")
+            latents = randn_tensor(shape, generator, torch.float32, "cpu")
         latents = latents.to(torch.float32) * self.scheduler.init_noise_sigma
         return latents.to(dtype)
 
@@ -234,39 +229,57 @@ class StableDiffusionXLCustomPipeline:
         width = width or self.default_sample_size * self.vae_scale_factor
         original_size = original_size or (height, width)                              # :192-193
         target_size = target_size or (height, width)
-        if callback is not None and (not isinstance(callback_steps, int) or callback_steps <= 0):
-            raise ValueError(f"`callback_steps` has to be a positive integer but is {callback_steps}")   # [3P] check_inputs
+        self._check_callback_steps(callback, callback_steps)
         do_classifier_free_guidance = guidance_scale > 1.0                            # :223
-        (prompt_embeds, negative_prompt_embeds, pooled_prompt_embeds, negative_pooled_prompt_embeds) = \
-            self.encode_prompt(prompt, prompt_2, None, num_images_per_prompt, do_classifier_free_guidance,
-                               negative_prompt, negative_prompt_2, prompt_embeds, negative_prompt_embeds,
-                               pooled_prompt_embeds, negative_pooled_prompt_embeds)  # :229-247
-        batch = prompt_embeds.shape[0]
+        embeds = self.encode_prompt(prompt, prompt_2, None, num_images_per_prompt, do_classifier_free_guidance,
+                                    negative_prompt, negative_prompt_2, prompt_embeds, negative_prompt_embeds,
+                                    pooled_prompt_embeds, negative_pooled_prompt_embeds)  # :229-247
         self.scheduler.set_timesteps(num_inference_steps)                             # :250
-        lat = self.prepare_latents(batch, self.unet.config.in_channels, height, width, torch.float16, self.device,
-                                   generator, latents)                               # :255-265
+        lat = self.prepare_latents(embeds[0].shape[0], self.unet.config.in_channels, height, width, torch.float16,
+                                   self.device, generator, latents)                  # :255-265
+        sizes = (original_size, crops_coords_top_left, target_size, negative_original_size,
+                 negative_crops_coords_top_left, negative_target_size)
+        out = self._denoise_from(lat, 0, num_inference_steps, denoising_end, embeds, sizes, guidance_scale,
+                                 guidance_rescale, control_guidance_start, control_guidance_end, callback, callback_steps,
+                                 generator=generator)
+        return self._output(out, output_type, return_dict)
 
-        add_time_ids, negative_add_time_ids = self._add_time_ids(
-            batch, (original_size, crops_coords_top_left, target_size, negative_original_size,
-                    negative_crops_coords_top_left, negative_target_size))
-        loop_steps = num_inference_steps
-        if denoising_end is not None and isinstance(denoising_end, float) and 0 < denoising_end < 1:   # :307-316
+    def _denoise_from(self, lat, t_start: int, num_inference_steps: int, denoising_end, embeds, sizes, guidance_scale,
+                      guidance_rescale, control_guidance_start, control_guidance_end, callback, callback_steps,
+                      inpaint=None, generator=None, unet_cond=None, controlnet=None) -> torch.Tensor:
+        """The loop over timesteps[t_start:], truncated by denoising_end (:307-316), from the noised start latents `lat`
+        with the IP scale of the processors (:319-322); the micro-conditioning time ids are formed from `sizes`
+        (requires_aesthetics_score = False). -> final latents."""
+        add_time_ids, negative_add_time_ids = self._add_time_ids(embeds[0].shape[0], sizes)
+        loop_end = num_inference_steps
+        if denoising_end is not None and isinstance(denoising_end, float) and 0 < denoising_end < 1:
             n_train = self.scheduler.num_train_timesteps
             cutoff = int(round(n_train - denoising_end * n_train))
-            loop_steps = int(sum(1 for t in self.scheduler.timesteps if t >= cutoff))
-        conditioning_scale = self._ip_scale()                                         # :319-322
-        if loop_steps > 0:
-            out = self.engine.run(lat, prompt_embeds, negative_prompt_embeds, pooled_prompt_embeds,
-                                  negative_pooled_prompt_embeds, add_time_ids, num_inference_steps,
+            loop_end = t_start + int(sum(1 for t in self.scheduler.timesteps[t_start:] if t >= cutoff))
+        conditioning_scale = self._ip_scale()
+        if loop_end > t_start:
+            out = self.engine.run(lat, *embeds, add_time_ids, num_inference_steps,
                                   guidance_scale=guidance_scale, ip_scale=conditioning_scale,
                                   control_guidance_start=control_guidance_start,
                                   control_guidance_end=control_guidance_end, guidance_rescale=guidance_rescale,
-                                  num_loop_steps=loop_steps, callback=callback, callback_steps=callback_steps,
-                                  negative_time_ids=negative_add_time_ids, generator=generator)
+                                  num_loop_steps=loop_end, callback=callback, callback_steps=callback_steps,
+                                  negative_time_ids=negative_add_time_ids, begin_step=t_start, inpaint=inpaint,
+                                  generator=generator, unet_cond=unet_cond, controlnet=controlnet)
         else:
             out = lat.to(self.device)
         self.set_scale(conditioning_scale)
-        return self._output(out, output_type, return_dict)
+        return out
+
+    @staticmethod
+    def _check_callback_steps(callback, callback_steps) -> None:
+        if callback is not None and (not isinstance(callback_steps, int) or callback_steps <= 0):
+            raise ValueError(f"`callback_steps` has to be a positive integer but is {callback_steps}")   # [3P] check_inputs
+
+    def _refuse_unsupported(self, given: Dict[str, Any]) -> None:
+        """Raises IHError for the arguments in UNSUPPORTED that `given` sets."""
+        refused = [k for k in self.UNSUPPORTED if given.get(k) is not None]
+        if refused:
+            raise IHError(f"{type(self).__name__} does not implement {refused}")
 
     @staticmethod
     def _add_time_ids(batch: int, sizes) -> Tuple[torch.Tensor, Optional[torch.Tensor]]:
@@ -416,22 +429,23 @@ class StableDiffusionXLImg2ImgPipeline(StableDiffusionXLCustomPipeline):
         if batch_size % n_img:
             raise ValueError(f"cannot duplicate an image batch of {n_img} to a prompt batch of {batch_size}")
         moments = venc.encode_moments_nhwc(image.to(self.device, torch.float16))      # [n_img, h, w, 16]
-        L = venc.config.latent_channels
-        h, w = moments.shape[1], moments.shape[2]
-        eps_dtype = torch.float32 if getattr(venc.config, "force_upcast", True) else torch.float16
+        if isinstance(generator, list) and len(generator) != batch_size:
+            raise ValueError(f"got {len(generator)} generators for a batch of {batch_size}")
+        # with a list, every generator samples the posterior of the image of its batch slot
+        L, h, w = venc.config.latent_channels, moments.shape[1], moments.shape[2]
+        eps = self._posterior_eps(batch_size if isinstance(generator, list) else n_img, h, w, generator)
+        noise = randn_tensor((batch_size, L, h, w), generator, torch.float16, self.device, "cpu")
+        return ops.vae_posterior_noise(moments, eps, noise, L, venc.config.scaling_factor, sigma)
 
-        def draw(shape, g, dtype):
-            return torch.randn(shape, generator=g, device=g.device if g is not None else "cpu", dtype=dtype)
-        if isinstance(generator, list):
-            if len(generator) != batch_size:
-                raise ValueError(f"got {len(generator)} generators for a batch of {batch_size}")
-            eps = torch.cat([draw((1, L, h, w), g, eps_dtype).to(self.device) for g in generator])
-            noise = torch.cat([draw((1, L, h, w), g, torch.float16).to(self.device) for g in generator])
-        else:
-            eps = draw((n_img, L, h, w), generator, eps_dtype).to(self.device)
-            noise = draw((batch_size, L, h, w), generator, torch.float16).to(self.device)
-        return ops.vae_posterior_noise(moments, eps.contiguous(), noise.contiguous(), L, venc.config.scaling_factor,
-                                       sigma)
+    def _posterior_eps(self, n: int, h: int, w: int, generator) -> torch.Tensor:
+        """The posterior draw of [3P] diffusers' `_encode_vae_image(images, generator)` for n images with latents of
+        h x w: image i with generator[i] for a list, fp32 when the VAE is upcast (else fp16), on the generator's device
+        (the CPU without one); -> on the device.  For the masked images (image * (mask < 0.5) broadcast over both
+        batches) 4-channel inpainting draws and drops it (SURVEY C.31); the 9-channel path encodes with it, and with the
+        same draw of the image batch (SURVEY C.32)."""
+        cfg = self.vae_encoder.config
+        dtype = torch.float32 if getattr(cfg, "force_upcast", True) else torch.float16
+        return randn_tensor((n, cfg.latent_channels, h, w), generator, dtype, self.device, "cpu")
 
     @torch.no_grad()
     def __call__(self, prompt: Optional[Union[str, List[str]]] = None, prompt_2=None, image=None, strength: float = 0.3,
@@ -453,13 +467,9 @@ class StableDiffusionXLImg2ImgPipeline(StableDiffusionXLCustomPipeline):
         diffusers arguments in UNSUPPORTED, which raise IHError."""
         self._require_euler()
         self._require_latent_unet()
-        refused = [k for k in self.UNSUPPORTED if kwargs.get(k) is not None]
-        if refused:
-            raise IHError(f"StableDiffusionXLImg2ImgPipeline does not implement {refused}")
-        if not 0.0 <= strength <= 1.0:
-            raise ValueError(f"The value of strength should in [0.0, 1.0] but is {strength}")          # [3P] check_inputs
-        if callback is not None and (not isinstance(callback_steps, int) or callback_steps <= 0):
-            raise ValueError(f"`callback_steps` has to be a positive integer but is {callback_steps}")
+        self._refuse_unsupported(kwargs)
+        t_start = self._begin_index(num_inference_steps, strength)
+        self._check_callback_steps(callback, callback_steps)
         if image is None:
             raise ValueError("`image` input cannot be undefined")
         if self.vae_encoder is None:
@@ -470,19 +480,11 @@ class StableDiffusionXLImg2ImgPipeline(StableDiffusionXLCustomPipeline):
         original_size = original_size or (height, width)
         target_size = target_size or (height, width)
         do_classifier_free_guidance = guidance_scale > 1.0
-        (prompt_embeds, negative_prompt_embeds, pooled_prompt_embeds, negative_pooled_prompt_embeds) = \
-            self.encode_prompt(prompt, prompt_2, None, num_images_per_prompt, do_classifier_free_guidance,
-                               negative_prompt, negative_prompt_2, prompt_embeds, negative_prompt_embeds,
-                               pooled_prompt_embeds, negative_pooled_prompt_embeds)
-        batch = prompt_embeds.shape[0]
+        embeds = self.encode_prompt(prompt, prompt_2, None, num_images_per_prompt, do_classifier_free_guidance,
+                                    negative_prompt, negative_prompt_2, prompt_embeds, negative_prompt_embeds,
+                                    pooled_prompt_embeds, negative_pooled_prompt_embeds)
         self.scheduler.set_timesteps(num_inference_steps)
-        t_start = self.scheduler.img2img_begin_index(num_inference_steps, strength)
-        if num_inference_steps - t_start < 1:
-            raise ValueError(f"After adjusting the num_inference_steps by strength parameter: {strength}, the number of "
-                             f"pipeline steps is {num_inference_steps - t_start} which is < 1 and not appropriate for "
-                             "this pipeline.")
-        lat = self.prepare_img2img_latents(pixels, batch, generator, self.scheduler.add_noise_sigma(t_start))
-        embeds = (prompt_embeds, negative_prompt_embeds, pooled_prompt_embeds, negative_pooled_prompt_embeds)
+        lat = self.prepare_img2img_latents(pixels, embeds[0].shape[0], generator, self.scheduler.add_noise_sigma(t_start))
         sizes = (original_size, crops_coords_top_left, target_size, negative_original_size,
                  negative_crops_coords_top_left, negative_target_size)
         out = self._denoise_from(lat, t_start, num_inference_steps, denoising_end, embeds, sizes, guidance_scale,
@@ -494,33 +496,19 @@ class StableDiffusionXLImg2ImgPipeline(StableDiffusionXLCustomPipeline):
         """Image-to-image and inpainting noise the image latents with Euler's add_noise (x + sigma * noise) inside the
         posterior kernel; DPM-Solver++ noises in VP form (alpha * x + sigma_vp * noise), which it does not compute."""
         if isinstance(self.scheduler, DPMSolverMultistepScheduler):
-            raise IHError(f"{type(self).__name__} supports EulerDiscreteScheduler only; DPMSolverMultistepScheduler runs "
-                          "text-to-image (StableDiffusionXLCustomPipeline)")
+            raise IHError(f"{type(self).__name__} supports EulerDiscreteScheduler and EulerAncestralDiscreteScheduler; "
+                          "DPMSolverMultistepScheduler runs text-to-image (StableDiffusionXLCustomPipeline)")
 
-    def _denoise_from(self, lat, t_start: int, num_inference_steps: int, denoising_end, embeds, sizes, guidance_scale,
-                      guidance_rescale, control_guidance_start, control_guidance_end, callback, callback_steps,
-                      inpaint=None, generator=None, unet_cond=None) -> torch.Tensor:
-        """The loop over timesteps[t_start:], truncated by denoising_end, from the noised start latents `lat`; the
-        micro-conditioning time ids are formed from `sizes` (requires_aesthetics_score = False). -> final latents."""
-        add_time_ids, negative_add_time_ids = self._add_time_ids(embeds[0].shape[0], sizes)
-        loop_end = num_inference_steps
-        if denoising_end is not None and isinstance(denoising_end, float) and 0 < denoising_end < 1:
-            n_train = self.scheduler.num_train_timesteps
-            cutoff = int(round(n_train - denoising_end * n_train))
-            loop_end = t_start + int(sum(1 for t in self.scheduler.timesteps[t_start:] if t >= cutoff))
-        conditioning_scale = self._ip_scale()
-        if loop_end > t_start:
-            out = self.engine.run(lat, *embeds, add_time_ids, num_inference_steps,
-                                  guidance_scale=guidance_scale, ip_scale=conditioning_scale,
-                                  control_guidance_start=control_guidance_start,
-                                  control_guidance_end=control_guidance_end, guidance_rescale=guidance_rescale,
-                                  num_loop_steps=loop_end, callback=callback, callback_steps=callback_steps,
-                                  negative_time_ids=negative_add_time_ids, begin_step=t_start, inpaint=inpaint,
-                                  generator=generator, unet_cond=unet_cond)
-        else:
-            out = lat
-        self.set_scale(conditioning_scale)
-        return out
+    def _begin_index(self, num_inference_steps: int, strength: float) -> int:
+        """[3P] check_inputs and get_timesteps: the schedule index t_start a run of `strength` begins at."""
+        if not 0.0 <= strength <= 1.0:
+            raise ValueError(f"The value of strength should in [0.0, 1.0] but is {strength}")
+        t_start = self.scheduler.img2img_begin_index(num_inference_steps, strength)
+        if num_inference_steps - t_start < 1:
+            raise ValueError(f"After adjusting the num_inference_steps by strength parameter: {strength}, the number of "
+                             f"pipeline steps is {num_inference_steps - t_start} which is < 1 and not appropriate for "
+                             "this pipeline.")
+        return t_start
 
 
 def preprocess_mask(mask, height: int, width: int) -> torch.Tensor:
@@ -566,7 +554,7 @@ class StableDiffusionXLInpaintPipeline(StableDiffusionXLImg2ImgPipeline):
     (DenoiseEngine.run(unet_cond=...)).  At strength 1 the image itself is not encoded (SURVEY C.32).
     `padding_mask_crop` is not implemented and raises IHError, as does a UNet with any other channel count."""
 
-    UNSUPPORTED = StableDiffusionXLImg2ImgPipeline.UNSUPPORTED + ("masked_image_latents",)
+    UNSUPPORTED = StableDiffusionXLImg2ImgPipeline.UNSUPPORTED + ("masked_image_latents", "padding_mask_crop")
 
     def prepare_inpaint_latents(self, image: torch.Tensor, batch_size: int, generator, t_start: int,
                                 is_strength_max: bool) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
@@ -579,22 +567,12 @@ class StableDiffusionXLInpaintPipeline(StableDiffusionXLImg2ImgPipeline):
         if batch_size % n_img:
             raise ValueError(f"cannot duplicate an image batch of {n_img} to a prompt batch of {batch_size}")
         moments = venc.encode_moments_nhwc(image.to(self.device, torch.float16))      # [n_img, h, w, 16]
-        L = venc.config.latent_channels
-        h, w = moments.shape[1], moments.shape[2]
-        eps_dtype = torch.float32 if getattr(venc.config, "force_upcast", True) else torch.float16
-
-        def draw(shape, g, dtype):
-            return torch.randn(shape, generator=g, device=g.device if g is not None else "cpu", dtype=dtype)
-        if isinstance(generator, list):
-            if len(generator) != batch_size:
-                raise ValueError(f"got {len(generator)} generators for a batch of {batch_size}")
-            # _encode_vae_image samples the n_img images with generator[i] before the batch is tiled
-            eps = torch.cat([draw((1, L, h, w), g, eps_dtype).to(self.device) for g in generator[:n_img]])
-            noise = torch.cat([draw((1, L, h, w), g, torch.float16).to(self.device) for g in generator])
-        else:
-            eps = draw((n_img, L, h, w), generator, eps_dtype).to(self.device)
-            noise = draw((batch_size, L, h, w), generator, torch.float16).to(self.device)
-        eps, noise = eps.contiguous(), noise.contiguous()
+        if isinstance(generator, list) and len(generator) != batch_size:
+            raise ValueError(f"got {len(generator)} generators for a batch of {batch_size}")
+        L, h, w = venc.config.latent_channels, moments.shape[1], moments.shape[2]
+        # _encode_vae_image samples the n_img images with generator[i] before the batch is tiled
+        eps = self._posterior_eps(n_img, h, w, generator)
+        noise = randn_tensor((batch_size, L, h, w), generator, torch.float16, self.device, "cpu")
         sf = venc.config.scaling_factor
         image_latents = ops.vae_posterior_noise(moments, eps, torch.zeros_like(noise), L, sf, 0.0)
         if is_strength_max:
@@ -623,24 +601,18 @@ class StableDiffusionXLInpaintPipeline(StableDiffusionXLImg2ImgPipeline):
         `height`, `width` and `padding_mask_crop`.  Unknown keywords are ignored, except the diffusers arguments in
         UNSUPPORTED and a `padding_mask_crop`, which raise IHError."""
         self._require_euler()
-        refused = [k for k in self.UNSUPPORTED if kwargs.get(k) is not None]
-        if padding_mask_crop is not None:
-            refused.append("padding_mask_crop")
-        if refused:
-            raise IHError(f"StableDiffusionXLInpaintPipeline does not implement {refused}")
+        self._refuse_unsupported({**kwargs, "padding_mask_crop": padding_mask_crop})
         unet9 = self.unet.config.in_channels == 9 and self.unet.conv_in.weight.shape[1] == 9
         if self.unet.config.in_channels != 4 and not unet9:
             raise IHError(f"StableDiffusionXLInpaintPipeline supports the 4-channel UNet and the 9-channel inpainting "
                           f"UNet (this one has config.in_channels = {self.unet.config.in_channels} and a conv_in of "
                           f"{self.unet.conv_in.weight.shape[1]} input channels)")
-        if not 0.0 <= strength <= 1.0:
-            raise ValueError(f"The value of strength should in [0.0, 1.0] but is {strength}")          # [3P] check_inputs
+        t_start = self._begin_index(num_inference_steps, strength)
         height = height or self.default_sample_size * self.vae_scale_factor
         width = width or self.default_sample_size * self.vae_scale_factor
         if height % 8 != 0 or width % 8 != 0:
             raise ValueError(f"`height` and `width` have to be divisible by 8 but are {height} and {width}.")
-        if callback is not None and (not isinstance(callback_steps, int) or callback_steps <= 0):
-            raise ValueError(f"`callback_steps` has to be a positive integer but is {callback_steps}")
+        self._check_callback_steps(callback, callback_steps)
         if image is None or mask_image is None:
             raise ValueError("`image` and `mask_image` inputs cannot be undefined")
         if self.vae_encoder is None:
@@ -654,11 +626,6 @@ class StableDiffusionXLInpaintPipeline(StableDiffusionXLImg2ImgPipeline):
                                     pooled_prompt_embeds, negative_pooled_prompt_embeds)
         batch = embeds[0].shape[0]
         self.scheduler.set_timesteps(num_inference_steps)
-        t_start = self.scheduler.img2img_begin_index(num_inference_steps, strength)
-        if num_inference_steps - t_start < 1:
-            raise ValueError(f"After adjusting the num_inference_steps by strength parameter: {strength}, the number of "
-                             f"pipeline steps is {num_inference_steps - t_start} which is < 1 and not appropriate for "
-                             "this pipeline.")
         sizes = (original_size or (height, width), crops_coords_top_left, target_size or (height, width),
                  negative_original_size, negative_crops_coords_top_left, negative_target_size)
         if unet9:
@@ -672,10 +639,10 @@ class StableDiffusionXLInpaintPipeline(StableDiffusionXLImg2ImgPipeline):
         # the masked image's latents only feed a 9-channel UNet: with 4 channels diffusers encodes them unused.  That
         # encode is skipped; its posterior draw comes after the noise, so it changes only what is drawn later: the step
         # noise of Euler Ancestral, for which the draw is made and dropped (SURVEY C.31)
+        h, w = height // self.vae_scale_factor, width // self.vae_scale_factor
         if isinstance(self.scheduler, EulerAncestralDiscreteScheduler):
-            self._posterior_eps(max(pixels.shape[0], mask.shape[0]), height, width, generator)
-        mask_lat = torch.nn.functional.interpolate(mask, size=(height // self.vae_scale_factor,
-                                                               width // self.vae_scale_factor)).half()
+            self._posterior_eps(max(pixels.shape[0], mask.shape[0]), h, w, generator)
+        mask_lat = torch.nn.functional.interpolate(mask, size=(h, w)).half()
         if batch % mask_lat.shape[0]:
             raise ValueError(f"cannot duplicate a mask batch of {mask_lat.shape[0]} to a prompt batch of {batch}")
         mask_lat = mask_lat.repeat(batch // mask_lat.shape[0], 1, 1, 1).to(self.device)
@@ -702,44 +669,23 @@ class StableDiffusionXLInpaintPipeline(StableDiffusionXLImg2ImgPipeline):
                 raise ValueError(f"cannot duplicate a {what} batch of {k} to a prompt batch of {batch_size}")
         if isinstance(generator, list) and len(generator) != batch_size:
             raise ValueError(f"got {len(generator)} generators for a batch of {batch_size}")
-        height, width = image.shape[2], image.shape[3]
         L, sf = venc.config.latent_channels, venc.config.scaling_factor
-        shape = (batch_size, L, height // self.vae_scale_factor, width // self.vae_scale_factor)
-
-        def draw_noise():
-            if isinstance(generator, list):
-                return torch.cat([torch.randn((1,) + shape[1:], generator=g, device=g.device, dtype=torch.float16)
-                                  .to(self.device) for g in generator])
-            return torch.randn(shape, generator=generator, device=generator.device if generator is not None else "cpu",
-                               dtype=torch.float16).to(self.device)
+        shape = (batch_size, L, image.shape[2] // self.vae_scale_factor, image.shape[3] // self.vae_scale_factor)
         if is_strength_max:
-            latents = (draw_noise().float() * self.scheduler.init_noise_sigma).half()
+            noise = randn_tensor(shape, generator, torch.float16, self.device, "cpu")
+            latents = (noise.float() * self.scheduler.init_noise_sigma).half()
         else:
             moments = venc.encode_moments_nhwc(image.to(self.device, torch.float16))
-            eps = self._posterior_eps(n_img, height, width, generator)
-            latents = ops.vae_posterior_noise(moments, eps, draw_noise().contiguous(), L, sf,
-                                              self.scheduler.add_noise_sigma(t_start))
+            eps = self._posterior_eps(n_img, *shape[2:], generator)
+            noise = randn_tensor(shape, generator, torch.float16, self.device, "cpu")
+            latents = ops.vae_posterior_noise(moments, eps, noise, L, sf, self.scheduler.add_noise_sigma(t_start))
         masked = image * (mask < 0.5)
         moments = venc.encode_moments_nhwc(masked.to(self.device, torch.float16))
-        eps = self._posterior_eps(n_masked, height, width, generator)
+        eps = self._posterior_eps(n_masked, *shape[2:], generator)
         zeros = torch.zeros(shape, dtype=torch.float16, device=self.device)
         masked_latents = ops.vae_posterior_noise(moments, eps, zeros, L, sf, 0.0)
         mask_lat = torch.nn.functional.interpolate(mask, size=shape[2:]).half()
         return latents, mask_lat.repeat(batch_size // n_mask, 1, 1, 1).to(self.device), masked_latents
-
-    def _posterior_eps(self, n: int, height: int, width: int, generator) -> torch.Tensor:
-        """The posterior draw of [3P] diffusers' `_encode_vae_image(images, generator)` for n images: image i with
-        generator[i] for a list, fp32 when the VAE is upcast (else fp16), on the generator's device; -> on the device.
-        For the masked images (image * (mask < 0.5) broadcast over both batches) the 4-channel path draws and drops it
-        (SURVEY C.31); the 9-channel path encodes with it, and with the same draw of the image batch (SURVEY C.32)."""
-        L = self.vae_encoder.config.latent_channels
-        shape = (L, height // self.vae_scale_factor, width // self.vae_scale_factor)
-        dtype = torch.float32 if getattr(self.vae_encoder.config, "force_upcast", True) else torch.float16
-        if isinstance(generator, list):
-            return torch.cat([torch.randn((1,) + shape, generator=g, device=g.device, dtype=dtype).to(self.device)
-                              for g in generator[:n]]).contiguous()
-        return torch.randn((n,) + shape, generator=generator,
-                           device=generator.device if generator is not None else "cpu", dtype=dtype).to(self.device)
 
 
 def preprocess_control_image(image, height: Optional[int] = None, width: Optional[int] = None,
@@ -889,9 +835,7 @@ class StableDiffusionXLControlNetPipeline(StableDiffusionXLCustomPipeline):
         pipeline, except the arguments in UNSUPPORTED, which raise IHError."""
         from imagharmony_b200.controlnet import ControlNetCall, MultiControlNetModel, controlnet_keep
         self._require_latent_unet()
-        refused = [k for k in self.UNSUPPORTED if kwargs.get(k) is not None]
-        if refused:
-            raise IHError(f"StableDiffusionXLControlNetPipeline does not implement {refused}")
+        self._refuse_unsupported(kwargs)
         multi = isinstance(self.controlnet, MultiControlNetModel)
         if not multi and (isinstance(controlnet_conditioning_scale, (list, tuple))
                           or isinstance(control_guidance_start, (list, tuple))
@@ -908,8 +852,7 @@ class StableDiffusionXLControlNetPipeline(StableDiffusionXLCustomPipeline):
         for start, end in zip(starts, ends):                                  # [3P] check_inputs
             if not 0.0 <= start < end <= 1.0:
                 raise ValueError(f"control guidance window [{start}, {end}] must satisfy 0 <= start < end <= 1")
-        if callback is not None and (not isinstance(callback_steps, int) or callback_steps <= 0):
-            raise ValueError(f"`callback_steps` has to be a positive integer but is {callback_steps}")
+        self._check_callback_steps(callback, callback_steps)
         controls = [preprocess_control_image(im, height, width, self.vae_scale_factor) for im in images]
         height, width = controls[0].shape[2], controls[0].shape[3]
         if any(tuple(c.shape[2:]) != (height, width) for c in controls):
@@ -918,11 +861,10 @@ class StableDiffusionXLControlNetPipeline(StableDiffusionXLCustomPipeline):
         if height % 8 or width % 8:
             raise ValueError(f"`height` and `width` have to be divisible by 8 but are {height} and {width}.")
         do_classifier_free_guidance = guidance_scale > 1.0
-        (prompt_embeds, negative_prompt_embeds, pooled_prompt_embeds, negative_pooled_prompt_embeds) = \
-            self.encode_prompt(prompt, prompt_2, None, num_images_per_prompt, do_classifier_free_guidance,
-                               negative_prompt, negative_prompt_2, prompt_embeds, negative_prompt_embeds,
-                               pooled_prompt_embeds, negative_pooled_prompt_embeds)
-        batch = prompt_embeds.shape[0]
+        embeds = self.encode_prompt(prompt, prompt_2, None, num_images_per_prompt, do_classifier_free_guidance,
+                                    negative_prompt, negative_prompt_2, prompt_embeds, negative_prompt_embeds,
+                                    pooled_prompt_embeds, negative_pooled_prompt_embeds)
+        batch = embeds[0].shape[0]
         # [3P] prepare_image, per net: repeat_interleave by the batch (one image) or by num_images_per_prompt; the CFG
         # copy is the engine's (the embedding is computed once and duplicated)
         for j, c in enumerate(controls):
@@ -933,18 +875,13 @@ class StableDiffusionXLControlNetPipeline(StableDiffusionXLCustomPipeline):
         self.scheduler.set_timesteps(num_inference_steps)
         lat = self.prepare_latents(batch, self.unet.config.in_channels, height, width, torch.float16, self.device,
                                    generator, latents)
-        add_time_ids, negative_add_time_ids = self._add_time_ids(
-            batch, (original_size or (height, width), crops_coords_top_left, target_size or (height, width),
-                    negative_original_size, negative_crops_coords_top_left, negative_target_size))
-        ip_scale = self._ip_scale()
+        sizes = (original_size or (height, width), crops_coords_top_left, target_size or (height, width),
+                 negative_original_size, negative_crops_coords_top_left, negative_target_size)
         models = list(self.controlnet.nets) if multi else [self.controlnet]
         cn = [ControlNetCall(m, c.half(), s, bool(guess_mode), controlnet_keep(num_inference_steps, start, end))
               for m, c, s, start, end in zip(models, controls, scales, starts, ends)]
-        cn = cn if multi else cn[0]
-        out = self.engine.run(lat, prompt_embeds, negative_prompt_embeds, pooled_prompt_embeds,
-                              negative_pooled_prompt_embeds, add_time_ids, num_inference_steps,
-                              guidance_scale=guidance_scale, ip_scale=ip_scale, guidance_rescale=guidance_rescale,
-                              callback=callback, callback_steps=callback_steps,
-                              negative_time_ids=negative_add_time_ids, generator=generator, controlnet=cn)
-        self.set_scale(ip_scale)
+        # the IP scale is not gated: its window stays [0, 1]
+        out = self._denoise_from(lat, 0, num_inference_steps, None, embeds, sizes, guidance_scale, guidance_rescale,
+                                 0.0, 1.0, callback, callback_steps, generator=generator,
+                                 controlnet=cn if multi else cn[0])
         return self._output(out, output_type, return_dict)

@@ -100,21 +100,17 @@ def measure(K: int, res: int, rounds: int, replays: int) -> dict:
         engines[kind].run(*args, guidance_scale=5.0, ip_scale=1.0,
                           controlnet=ControlNetCall(cn, image.half(), 1.0, guess))
     out["launches_per_step"] = {}
-    graphs, statics = {}, {}
+    graphs = {}
     for kind, e in engines.items():
         assert len(e._graphs) == 1, (kind, list(e._graphs))
         graphs[kind] = next(iter(e._graphs.values()))[0]
-        statics[kind] = next(iter(e._static.values()))
         out["launches_per_step"][kind] = e.last_launches_per_step
     a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     times = {k: [] for k in engines}
     order = list(engines)
     for r in range(rounds):
         for kind in order[r % 3:] + order[:r % 3]:
-            st = statics[kind]
-            st["latents"].copy_(latents)
-            st["step"].fill_(0)                                # replays stay inside the K-step sigma table
-            ops.scale_model_input(st["latents"], st["model_in"], engines[kind].tables(K)[1], st["step"])
+            engines[kind]._restart(engines[kind]._loop, latents, 0)   # replays stay inside the K-step sigma table
             torch.cuda.synchronize()
             a.record()
             for _ in range(replays):

@@ -80,12 +80,9 @@ def measure(K: int, res: int, rounds: int, replays: int, karras: bool) -> dict:
     for r in range(rounds):
         for kind in (("euler", "dpm") if r % 2 == 0 else ("dpm", "euler")):
             eng = engines[kind]
-            st = next(iter(eng._static.values()))
-            st["latents"].copy_(latents)
-            st["step"].fill_(0)                                 # replays stay inside the K-step tables
+            st = eng._loop.st
             eng.unet.prepare_conditioning(st["ehs"], st["text_embeds"], st["time_ids"])
-            eng._first_input(st, eng.tables(K)[1], True,
-                             (next(iter(eng._dpm_static.values())), eng.coeffs(K)) if kind == "dpm" else None)
+            eng._restart(eng._loop, latents, 0)                 # replays stay inside the K-step tables
             torch.cuda.synchronize()
             a.record()
             for _ in range(replays):

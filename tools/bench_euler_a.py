@@ -70,12 +70,9 @@ def measure(K: int, res: int, rounds: int, replays: int) -> dict:
     for r in range(rounds):
         for kind in (("euler", "euler_a") if r % 2 == 0 else ("euler_a", "euler")):
             eng = engines[kind]
-            st = next(iter(eng._static.values()))
-            st["latents"].copy_(latents)
-            st["step"].fill_(0)                                 # replays stay inside the K-step tables
+            st = eng._loop.st
             eng.unet.prepare_conditioning(st["ehs"], st["text_embeds"], st["time_ids"])
-            anc = (eng.coeffs(K), eng._ancestral_buffer(n, lat, lat, K)) if kind == "euler_a" else None
-            eng._first_input(st, eng.tables(K)[1], True, None, anc)
+            eng._restart(eng._loop, latents, 0)                 # replays stay inside the K-step tables
             torch.cuda.synchronize()
             a.record()
             for _ in range(replays):
@@ -126,7 +123,7 @@ def measure(K: int, res: int, rounds: int, replays: int) -> dict:
 
     # ---- the per-call noise pre-draw: K draws from a CPU generator and K copies into the device buffer
     eng = engines["euler_a"]
-    buf = eng._ancestral_buffer(n, lat, lat, K)
+    buf = eng._loop.noise
     pd = []
     for r in range(rounds + 1):
         gen = torch.Generator("cpu").manual_seed(r)

@@ -84,16 +84,13 @@ def measure(strength: float, K: int, res: int, rounds: int, replays: int) -> dic
     args = (latents, pos, neg, pooled, npooled, tid, K)
     eng.run(*args, guidance_scale=5.0, ip_scale=1.0)
     eng.run(*args, guidance_scale=5.0, ip_scale=1.0, inpaint=(image_latents, noise, mask))
-    graphs = {kind: next(g for key, (g, _) in eng._graphs.items() if key[-1] == (kind == "inpaint"))
+    graphs = {kind: next(g for key, (g, _) in eng._graphs.items() if key[-2] == (kind == "inpaint"))  # the ib flag
               for kind in ("t2i", "inpaint")}
-    st = next(iter(eng._static.values()))
     a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     times = {"t2i": [], "inpaint": []}
     for r in range(rounds):
         for kind in (("t2i", "inpaint") if r % 2 == 0 else ("inpaint", "t2i")):
-            st["latents"].copy_(latents)
-            st["step"].fill_(0)                                # replays stay inside the K-step sigma table
-            ops.scale_model_input(st["latents"], st["model_in"], eng.tables(K)[1], st["step"])
+            eng._restart(eng._loop, latents, 0)                # replays stay inside the K-step sigma table
             torch.cuda.synchronize()
             a.record()
             for _ in range(replays):

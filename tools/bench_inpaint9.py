@@ -78,15 +78,11 @@ def measure(strength: float, K: int, res: int, rounds: int, replays: int) -> dic
     out["launches_per_step"] = {"t2i": launches4, "inpaint9": eng9.last_launches_per_step}
     engines = {"t2i": eng4, "inpaint9": eng9}
     graphs = {kind: next(iter(e._graphs.values()))[0] for kind, e in engines.items()}
-    statics = {kind: next(iter(e._static.values())) for kind, e in engines.items()}
     a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     times = {"t2i": [], "inpaint9": []}
     for r in range(rounds):
         for kind in (("t2i", "inpaint9") if r % 2 == 0 else ("inpaint9", "t2i")):
-            st = statics[kind]
-            st["latents"].copy_(latents)
-            st["step"].fill_(0)                                # replays stay inside the K-step sigma table
-            ops.scale_model_input(st["latents"], st["model_in"], engines[kind].tables(K)[1], st["step"])
+            engines[kind]._restart(engines[kind]._loop, latents, 0)   # replays stay inside the K-step sigma table
             torch.cuda.synchronize()
             a.record()
             for _ in range(replays):

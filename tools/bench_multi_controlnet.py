@@ -87,21 +87,17 @@ def measure(K: int, res: int, rounds: int, replays: int) -> dict:
     engines["nets1"].run(*args, guidance_scale=5.0, ip_scale=1.0, controlnet=calls[0])
     engines["nets2"].run(*args, guidance_scale=5.0, ip_scale=1.0, controlnet=calls)
     out["launches_per_step"] = {}
-    graphs, statics = {}, {}
+    graphs = {}
     for kind, e in engines.items():
         assert len(e._graphs) == 1, (kind, list(e._graphs))
         graphs[kind] = next(iter(e._graphs.values()))[0]
-        statics[kind] = next(iter(e._static.values()))
         out["launches_per_step"][kind] = e.last_launches_per_step
     a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     times = {k: [] for k in engines}
     order = list(engines)
     for r in range(rounds):
         for kind in order[r % 3:] + order[:r % 3]:
-            st = statics[kind]
-            st["latents"].copy_(latents)
-            st["step"].fill_(0)                                # replays stay inside the K-step sigma table
-            ops.scale_model_input(st["latents"], st["model_in"], engines[kind].tables(K)[1], st["step"])
+            engines[kind]._restart(engines[kind]._loop, latents, 0)   # replays stay inside the K-step sigma table
             torch.cuda.synchronize()
             a.record()
             for _ in range(replays):
@@ -113,7 +109,7 @@ def measure(K: int, res: int, rounds: int, replays: int) -> dict:
                          **{f"{k}_ms": spread(v) for k, v in times.items()},
                          **{f"{k}_minus_nets0_ms": spread([x - t for x, t in zip(times[k], times["nets0"])])
                             for k in ("nets1", "nets2")}}
-    del engines, graphs, statics
+    del engines, graphs
     torch.cuda.empty_cache()
 
     # ---- the fused injection kernel alone on the SDXL skip shapes of a CFG step, K = 1, 2, 3

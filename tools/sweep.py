@@ -56,7 +56,7 @@ def main():
                 if rank == 0:
                     print(json.dumps(rows[-1]), flush=True)
             eng.invalidate_graphs()
-            eng._static.clear()
+            eng._pool.clear()
             torch.cuda.empty_cache()
     if rank == 0:
         os.makedirs(os.path.join(ROOT, "tools_out"), exist_ok=True)
