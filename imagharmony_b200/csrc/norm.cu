@@ -41,6 +41,16 @@ __device__ __forceinline__ void store8(__half* p, const float (&x)[8]) {
 constexpr int GN_MAXG = 512;
 constexpr int GN_MAXB = 1024;
 constexpr int GN_SYNC_WORDS = 3 * GN_MAXB;   // per image: ticket (statistics), ready flag and departure counter (fused kernel)
+// The R*2*C-float statistics buffer (8*C bytes once R = 1) plus the kernels' static shared memory must fit the 48 KiB
+// a kernel gets without an opt-in; SDXL needs at most 2560 channels.
+constexpr int GN_MAXC = 4096;
+
+// The last block of an image sums the G partials of each of the 2*groups values in `slices` interleaved chains (a fixed
+// order: deterministic), keeping 2*groups*slices doubles in the statistics buffer.
+__host__ __device__ __forceinline__ int gn_slices(int threads, int groups) {
+  const int s = threads / (2 * groups);
+  return s < 1 ? 1 : (s > 4 ? 4 : s);
+}
 
 __global__ void gn_stats_kernel(const __half* __restrict__ x0, int C0, const __half* __restrict__ x1, int C1, int HW,
                                 int groups, int R, int rows_per_block, float eps, float* __restrict__ ws, int B) {
@@ -125,15 +135,13 @@ __global__ void gn_stats_kernel(const __half* __restrict__ x0, int C0, const __h
     __threadfence();
     // all threads reduce the G partials: value index v = t % (2*groups), slice = t / (2*groups); L2 (ld.cg) loads
     // are independent so they pipeline; fixed summation order keeps the result deterministic.
-    double* s_red = reinterpret_cast<double*>(s_acc);  // reuse (>= 2*C floats >= 2*groups*slices doubles)
+    double* s_red = reinterpret_cast<double*>(s_acc);  // reuse: 2*groups*slices doubles fit (checked on the host)
     const int nv = 2 * groups;
-    int slices = blockDim.x / nv;
-    if (slices < 1) slices = 1;
-    if (slices > 4) slices = 4;
+    const int slices = gn_slices(blockDim.x, groups);
     const float* pp = ws + (long long)b * GN_MAXG * nv;
     __syncthreads();
-    if ((int)threadIdx.x < nv * slices) {
-      const int v = threadIdx.x % nv, sl = threadIdx.x / nv;
+    for (int t = threadIdx.x; t < nv * slices; t += blockDim.x) {  // 2*groups may exceed the block: loop
+      const int v = t % nv, sl = t / nv;
       double a = 0.0;
 #pragma unroll 8
       for (int k = sl; k < (int)gridDim.x; k += slices) a += (double)__ldcg(pp + (long long)k * nv + v);
@@ -323,15 +331,13 @@ __global__ void gn_fused_kernel(const __half* __restrict__ x0, int C0, const __h
   __syncthreads();
   if (s_last) {
     __threadfence();
-    double* s_red = reinterpret_cast<double*>(s_acc);  // reuse (>= 2*C floats >= 2*groups*slices doubles)
+    double* s_red = reinterpret_cast<double*>(s_acc);  // reuse: 2*groups*slices doubles fit (checked on the host)
     const int nv = 2 * groups;
-    int slices = blockDim.x / nv;
-    if (slices < 1) slices = 1;
-    if (slices > 4) slices = 4;
+    const int slices = gn_slices(blockDim.x, groups);
     const float* pp = ws + (long long)b * GN_MAXG * nv;
     __syncthreads();
-    if ((int)threadIdx.x < nv * slices) {
-      const int v = threadIdx.x % nv, sl = threadIdx.x / nv;
+    for (int t = threadIdx.x; t < nv * slices; t += blockDim.x) {  // 2*groups may exceed the block: loop
+      const int v = t % nv, sl = t / nv;
       double a = 0.0;
 #pragma unroll 8
       for (int k = sl; k < (int)gridDim.x; k += slices) a += (double)__ldcg(pp + (long long)k * nv + v);
@@ -497,14 +503,17 @@ extern "C" int ih_groupnorm_f16(const void* x0, int C0, const void* x1, int C1, 
   IH_CHECK(x0 && gamma && beta && out && stats_ws, IH_ERR_ARG, "ih_groupnorm_f16: null pointer");
   if (!x1) C1 = 0;
   const int C = C0 + C1;
-  IH_CHECK(C0 % 8 == 0 && C1 % 8 == 0 && C % groups == 0 && C > 0, IH_ERR_SHAPE,
+  IH_CHECK(C0 % 8 == 0 && C1 % 8 == 0 && groups >= 1 && C > 0 && C % groups == 0, IH_ERR_SHAPE,
            "ih_groupnorm_f16: C0=%d C1=%d groups=%d unsupported", C0, C1, groups);
+  IH_CHECK(C <= GN_MAXC, IH_ERR_SHAPE, "ih_groupnorm_f16: C=%d exceeds %d", C, GN_MAXC);
+  IH_CHECK(B >= 1 && B <= GN_MAXB && HW >= 1, IH_ERR_SHAPE, "ih_groupnorm_f16: B=%d (max %d) HW=%d", B, GN_MAXB, HW);
   const int CV = C / 8;
-  IH_CHECK(CV <= 1024, IH_ERR_SHAPE, "ih_groupnorm_f16: C too large");
-  IH_CHECK(B <= GN_MAXB, IH_ERR_SHAPE, "ih_groupnorm_f16: B=%d exceeds %d", B, GN_MAXB);
   int R = 256 / CV;
   if (R < 1) R = 1;
   const int threads = CV * R;
+  // the last block's reduction reuses the statistics buffer: C > 1024 (one row lane) needs groups <= C / 2
+  IH_CHECK((size_t)2 * groups * gn_slices(threads, groups) * sizeof(double) <= (size_t)R * 2 * C * sizeof(float),
+           IH_ERR_SHAPE, "ih_groupnorm_f16: groups=%d too many for C=%d", groups, C);
   // row chunks per image: about `bps` blocks per SM overall, at most GN_MAXG per image.  Measured (tools/gn_probe.py):
   // at UNet batch 2 the kernels are launch/latency bound and 2 blocks per SM is best; from batch 16 on they are
   // bandwidth bound and 4 blocks per SM (more loads in flight) is 1.6x faster (64.5 -> 40.6 us at B16 32^2 C1280).

@@ -142,7 +142,8 @@ int ih_attention_ws_f16(const void* q, long long ldq, const void* k, long long l
 /* GroupNorm over NHWC [B, HW, C] (optionally the channel-concatenation of two tensors x0 [.., C0] and x1 [.., C1]),
  * fp32 partial sums reduced in double, optional fused SiLU.  stats_ws: ih_groupnorm_workspace_bytes(B, groups) bytes,
  * zero-initialised ONCE by the caller (the kernels leave its ticket counters at zero again) and not shared by
- * concurrently running calls.  Replaces nn.GroupNorm (+ nn.SiLU) in diffusers ResnetBlock2D / Transformer2DModel. */
+ * concurrently running calls.  C = C0 + C1 <= 4096 with C0, C1 multiples of 8, groups divides C (and groups <= C / 2
+ * when C > 1024), 1 <= B <= 1024.  Replaces nn.GroupNorm (+ nn.SiLU) in diffusers ResnetBlock2D / Transformer2DModel. */
 long long ih_groupnorm_workspace_bytes(int B, int groups);
 int ih_groupnorm_f16(const void* x0, int C0, const void* x1, int C1, const void* gamma, const void* beta, void* out,
                      void* stats_ws, int B, int HW, int groups, float eps, int silu, void* stream);

@@ -43,3 +43,25 @@ def test_argument_validation_returns_error_codes():
     assert rc < 0 and b"null" in lib.ih_last_error()
     rc = lib.ih_layernorm_f16(1, 1, 1, 1, 4, 7, 1e-5, None)   # C not a multiple of 8 (checked before any launch)
     assert rc < 0
+
+
+@pytest.mark.parametrize("C0,C1,B,HW,groups", [
+    (1280, 0, 1, 64, 1280),    # one row lane per block: 2*groups partial sums would overrun the statistics buffer
+    (2048, 0, 1, 64, 2048),
+    (1280, 1280, 2, 64, 2560),
+    (1280, 0, 1, 64, 0),       # no group count (and no division by zero on the host)
+    (1280, 0, 1, 64, 3),       # groups does not divide C
+    (4104, 0, 1, 64, 8),       # C above 4096 (the statistics buffer and 48 KiB of shared memory)
+    (4096, 8, 1, 64, 32),
+    (8192, 0, 1, 64, 32),
+    (320, 0, 0, 64, 32),       # empty batch
+    (320, 0, 1025, 64, 32),    # more images than ticket slots
+    (320, 0, 2, 0, 32),        # no pixels
+    (324, 0, 1, 64, 4),        # C0 not a multiple of 8
+])
+def test_groupnorm_rejects_unsupported_configurations(C0, C1, B, HW, groups):
+    """Checked on the host before anything is launched (fake non-null pointers never reach a kernel)."""
+    from imagharmony_b200 import _lib
+    lib = _lib.load()
+    rc = lib.ih_groupnorm_f16(1, C0, 1 if C1 else None, C1, 1, 1, 1, 1, B, HW, groups, 1e-5, 0, None)
+    assert rc < 0 and b"ih_groupnorm_f16" in lib.ih_last_error(), (rc, lib.ih_last_error())

@@ -16,7 +16,7 @@ def test_fold_layernorm_identity():
     beta = (0.2 * torch.randn(K, generator=g)).half()
     w_c, c = fold_layernorm(w, b, gamma, beta)
     assert w_c.dtype == torch.float16 and c.dtype == torch.float16
-    assert w_c.double().sum(dim=1).abs().max() < 2e-2                  # rows centred up to fp16 rounding
+    assert (w_c.double().sum(dim=1) == 0).all()                        # fp16 rows centred exactly
     mean = x.mean(dim=1, keepdim=True)
     rstd = torch.rsqrt(x.var(dim=1, unbiased=False, keepdim=True) + 1e-5)
     folded = rstd * (x @ w_c.double().t()) + c.double()
@@ -29,6 +29,24 @@ def test_fold_layernorm_identity():
     m2 = s / K
     r2 = torch.rsqrt((q / K - m2 * m2).clamp_min(0) + 1e-5)
     assert torch.allclose(m2, mean[:, 0]) and torch.allclose(r2, rstd[:, 0], rtol=1e-9)
+
+
+def test_fold_rounding_keeps_rows_summing_to_zero():
+    """The folded weight's fp16 rounding: every row sums to exactly zero (so mean(x) drops out of the GEMM at any
+    |mean| / std), and the elementwise error stays that of round-to-nearest."""
+    from imagharmony_b200.ops import _round_rows_zero_sum
+    g = torch.Generator().manual_seed(1)
+    for N, K, scale in [(1280, 1280, 1280 ** -0.5), (96, 320, 0.3), (40, 5120, 5120 ** -0.5 * 1e-3)]:
+        w = torch.randn(N, K, generator=g, dtype=torch.float64) * scale
+        w = w - w.mean(dim=1, keepdim=True)
+        h = _round_rows_zero_sum(w)
+        near = w.half()
+        assert h.dtype == torch.float16 and (h.double().sum(dim=1) == 0).all()
+        worst = (near.double() - w).abs().amax(dim=1)
+        assert ((h.double() - w).abs().amax(dim=1) <= 2 * worst).all(), "a move larger than the row's rounding steps"
+        rms = lambda t: (t.double() - w).pow(2).mean().sqrt().item()   # noqa: E731
+        assert rms(h) <= 1.01 * rms(near), (rms(h), rms(near))
+        assert (near.double().sum(dim=1) != 0).any()                   # round-to-nearest alone does not do it
 
 
 def test_vae_folded_input_conv_matches_three_separate_ops():

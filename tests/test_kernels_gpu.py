@@ -1,6 +1,9 @@
-"""GPU parity tests of every C-ABI kernel against a plain PyTorch fp32 reference of the same op (same fp16-rounded
-inputs). Tolerance: rtol = atol = 1e-3 on fp16 outputs unless a test states otherwise (BASELINE.json north_star).
-All calls go through imagharmony_b200.ops -> ctypes -> libimagharmony_sm90.so.
+"""GPU parity tests of the core C-ABI kernels (GEMM / conv, attention, norms, the Euler step and a few small kernels)
+against a plain PyTorch fp32 reference of the same op (same fp16-rounded inputs). Tolerance: rtol = atol = 1e-3 on fp16
+outputs unless a test states otherwise (BASELINE.json north_star). All calls go through imagharmony_b200.ops -> ctypes
+-> libimagharmony_sm90.so. The edge cases of the shared kernels live in test_kernel_edges_gpu.py, the feature kernels
+in their features' *_gpu.py files; test_kernel_coverage_cpu.py maps every entry point of include/ih_api.h to the tests
+that call it directly.
 """
 import math
 
