@@ -95,20 +95,13 @@ SIGNATURES = {
     "ih_gemm_prefetch_next": (None, [c_void_p, c_longlong]),
     "ih_conv2d_f16": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_longlong, c_void_p, c_void_p, c_int, c_int,
                               c_int, c_int, c_int, c_int, c_int, c_int, c_void_p]),
-    "ih_attention_f16": (c_int, [c_void_p, c_longlong, c_void_p, c_longlong, c_void_p, c_longlong, c_void_p,
-                                 c_longlong, c_int, c_int, c_int, c_int, c_int, c_float, c_void_p]),
     "ih_attention_ws_f16": (c_int, [c_void_p, c_longlong, c_void_p, c_longlong, c_void_p, c_longlong, c_void_p,
                                     c_longlong, c_int, c_int, c_int, c_int, c_int, c_float, c_void_p, c_longlong,
                                     c_void_p]),
-    "ih_xattn_q_fused_f16": (c_int, [c_void_p, c_longlong, c_void_p, c_void_p, c_void_p, c_int, c_float, c_void_p,
-                                     c_longlong, c_void_p, c_longlong, c_void_p, c_longlong, c_int, c_int, c_int, c_int,
-                                     c_int, c_float, c_int, c_void_p]),
     "ih_attention_workspace_bytes": (c_longlong, [c_int, c_int, c_int, c_int, c_int]),
-    "ih_softmax_rows_f16": (c_int, [c_void_p, c_longlong, c_longlong, c_int, c_void_p]),
     "ih_softmax_rows_masked_f16": (c_int, [c_void_p, c_longlong, c_longlong, c_int, c_int, c_void_p]),
     "ih_attention_set_split_policy": (None, [c_int]),
     "ih_attention_set_kernel": (None, [c_int]),
-    "ih_attention_set_trace": (None, [c_void_p]),
     "ih_groupnorm_f16": (c_int, [c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_int,
                                  c_int, c_int, c_float, c_int, c_void_p]),
     "ih_groupnorm_workspace_bytes": (c_longlong, [c_int, c_int]),
@@ -122,8 +115,6 @@ SIGNATURES = {
     "ih_sinusoid_f16": (c_int, [c_void_p, c_void_p, c_void_p, c_longlong, c_int, c_int, c_void_p]),
     "ih_upsample2x_f16": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
     "ih_concat_f16": (c_int, [c_void_p, c_int, c_void_p, c_int, c_void_p, c_longlong, c_void_p]),
-    "ih_conv_in_f16": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p]),
-    "ih_conv_out_f16": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p]),
     "ih_im2col3x3_nchw_f16": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p]),
     "ih_im2col3x3_nchw_cat_f16": (c_int, [c_void_p, c_int, c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_int,
                                           c_void_p]),
@@ -144,7 +135,6 @@ SIGNATURES = {
     "ih_euler_ancestral_step": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_float, c_float,
                                         c_longlong, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "ih_euler_ancestral_scale_input": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_longlong, c_int, c_void_p]),
-    "ih_scale_model_input": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_longlong, c_void_p]),
     "ih_scale_model_input_ex": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_longlong, c_int, c_void_p]),
     "ih_conv3x3_small_f16": (c_int, [c_void_p, c_longlong, c_longlong, c_longlong, c_longlong, c_void_p, c_void_p,
                                      c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p]),

@@ -538,8 +538,6 @@ using namespace ih;
 
 extern "C" void ih_attention_set_split_policy(int policy) { g_split_policy = policy; }
 extern "C" void ih_attention_set_kernel(int kernel) { g_kernel = kernel == 1 ? 1 : 0; }
-// kept for ABI compatibility: the wgmma kernels record no per-block trace
-extern "C" void ih_attention_set_trace(void* device_buffer) { (void)device_buffer; }
 
 extern "C" long long ih_attention_workspace_bytes(int B, int H, int Nq, int Nk, int n_ip) {
   if (B <= 0 || H <= 0 || Nq <= 0 || Nk <= 128 || n_ip != 0) return 0;
@@ -551,21 +549,15 @@ extern "C" long long ih_attention_workspace_bytes(int B, int H, int Nq, int Nk, 
   return (long long)(units - n_whole) * split * rows * (64 + 2) * (long long)sizeof(float);
 }
 
-extern "C" int ih_attention_f16(const void* q, long long ldq, const void* k, long long ldk, const void* v,
-                                long long ldv, void* out, long long ldo, int B, int H, int Nq, int Nk, int n_ip,
-                                float ip_scale, void* stream) {
-  return ih_attention_ws_f16(q, ldq, k, ldk, v, ldv, out, ldo, B, H, Nq, Nk, n_ip, ip_scale, nullptr, 0, stream);
-}
-
 extern "C" int ih_attention_ws_f16(const void* q, long long ldq, const void* k, long long ldk, const void* v,
                                    long long ldv, void* out, long long ldo, int B, int H, int Nq, int Nk, int n_ip,
                                    float ip_scale, void* workspace, long long workspace_bytes, void* stream) {
-  IH_CHECK(q && k && v && out, IH_ERR_ARG, "ih_attention_f16: null pointer");
-  IH_CHECK(B > 0 && H > 0 && Nq > 0 && Nk > 0, IH_ERR_SHAPE, "ih_attention_f16: bad shape");
+  IH_CHECK(q && k && v && out, IH_ERR_ARG, "ih_attention_ws_f16: null pointer");
+  IH_CHECK(B > 0 && H > 0 && Nq > 0 && Nk > 0, IH_ERR_SHAPE, "ih_attention_ws_f16: bad shape");
   IH_CHECK(ldq % 8 == 0 && ldk % 8 == 0 && ldv % 8 == 0 && ldo % 8 == 0, IH_ERR_ALIGN,
-           "ih_attention_f16: row strides must be multiples of 8 elements");
-  IH_CHECK(n_ip >= 0 && n_ip < Nk, IH_ERR_ARG, "ih_attention_f16: n_ip out of range");
-  IH_CHECK(n_ip == 0 || Nk <= 128, IH_ERR_SHAPE, "ih_attention_f16: decoupled IP path needs Nk <= 128");
+           "ih_attention_ws_f16: row strides must be multiples of 8 elements");
+  IH_CHECK(n_ip >= 0 && n_ip < Nk, IH_ERR_ARG, "ih_attention_ws_f16: n_ip out of range");
+  IH_CHECK(n_ip == 0 || Nk <= 128, IH_ERR_SHAPE, "ih_attention_ws_f16: decoupled IP path needs Nk <= 128");
 
   const int rows = n_ip == 0 ? attn_rows(Nk) : 128;
   CUtensorMap tq, tk, tv;

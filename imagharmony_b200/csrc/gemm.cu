@@ -536,12 +536,8 @@ static int pick_bn(long long m_tiles, int N, int num_kb, bool allow160) {
   if (N <= 64) return 64;
   const int sms = num_sms();
   // 128x64 tiles for launches that cannot fill the SMs with wider ones (e.g. the 1280-channel level of a 512^2 edit,
-  // M = 512): each SM then streams fewer bytes per k-block and drains one slab.  IH_BN64=0 disables.
-  static const int bn64 = [] {
-    const char* e = getenv("IH_BN64");
-    return e ? atoi(e) : 1;
-  }();
-  if (bn64 && m_tiles * ((N + 63) / 64) <= sms) return 64;
+  // M = 512): each SM then streams fewer bytes per k-block and drains one slab.
+  if (m_tiles * ((N + 63) / 64) <= sms) return 64;
   // Measured with tools/ab_probe.py tile (M = 2048, 128 tiles in one round, K = 1280 vs 5120) on an NVIDIA H100 80GB
   // HBM3 at a 400 W power limit: per k-block 0.583 / 0.706 / 0.877 / 1.161 us and fixed 3.3 / 3.7 / 3.9 / 8.8 us for
   // the 128 / 160 / 192 / 256-column tiles, here in units of the 128-column tile's k-block.  The main loop is

@@ -517,11 +517,7 @@ extern "C" int ih_groupnorm_f16(const void* x0, int C0, const void* x1, int C1, 
   // row chunks per image: about `bps` blocks per SM overall, at most GN_MAXG per image.  Measured (tools/gn_probe.py):
   // at UNet batch 2 the kernels are launch/latency bound and 2 blocks per SM is best; from batch 16 on they are
   // bandwidth bound and 4 blocks per SM (more loads in flight) is 1.6x faster (64.5 -> 40.6 us at B16 32^2 C1280).
-  static const int bps_env = [] {
-    const char* e = getenv("IH_GN_BLOCKS_PER_SM");
-    return e ? atoi(e) : 0;
-  }();
-  const int bps = bps_env > 0 ? bps_env : (B >= 8 ? 4 : 2);
+  const int bps = B >= 8 ? 4 : 2;
   int G = (bps * num_sms() + B - 1) / B;
   if (G > GN_MAXG) G = GN_MAXG;
   int rows_per_block = (HW + G - 1) / G;

@@ -120,117 +120,6 @@ __global__ void concat_kernel(const uint4* __restrict__ x0, int CV0, const uint4
 }
 
 // ---------------------------------------------------------------------------------------------------------------
-// conv_in: NCHW [B,Cin<=8,H,W] -> NHWC [B,H,W,Cout], 3x3 pad 1. thread = (pixel, 8 output channels)
-// ---------------------------------------------------------------------------------------------------------------
-__global__ void conv_in_kernel(const __half* __restrict__ x, const __half* __restrict__ w,
-                               const __half* __restrict__ bias, __half* __restrict__ out, int B, int H, int W, int Cin,
-                               int Cout) {
-  pdl_launch_dependents();
-  pdl_wait();
-  extern __shared__ __half s_w[];  // [Cin*9][Cout]
-  const int K = Cin * 9;
-  for (int i = threadIdx.x; i < K * Cout; i += blockDim.x) {
-    const int o = i / K, k = i - o * K;  // w is OIHW: [o][ci][ky][kx] -> k = ci*9 + ky*3 + kx
-    s_w[k * Cout + o] = w[i];
-  }
-  __syncthreads();
-  const int CG = Cout >> 3;
-  const long long total = (long long)B * H * W * CG;
-  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
-    const int cg = (int)(i % CG);
-    long long pix = i / CG;
-    const int xw = (int)(pix % W);
-    const int yh = (int)((pix / W) % H);
-    const int b = (int)(pix / ((long long)W * H));
-    float acc[8];
-    if (bias) ld8(bias + cg * 8, acc);
-    else {
-#pragma unroll
-      for (int e = 0; e < 8; ++e) acc[e] = 0.f;
-    }
-    for (int ci = 0; ci < Cin; ++ci)
-#pragma unroll
-      for (int t = 0; t < 9; ++t) {
-        const int yy = yh + t / 3 - 1, xx = xw + t % 3 - 1;
-        if (yy >= 0 && yy < H && xx >= 0 && xx < W) {
-          const float xv = __half2float(x[(((long long)b * Cin + ci) * H + yy) * W + xx]);
-          float wv[8];
-          ld8(s_w + (ci * 9 + t) * Cout + cg * 8, wv);
-#pragma unroll
-          for (int e = 0; e < 8; ++e) acc[e] += xv * wv[e];
-        }
-      }
-    uint4 o;
-    o.x = pack_half2(acc[0], acc[1]);
-    o.y = pack_half2(acc[2], acc[3]);
-    o.z = pack_half2(acc[4], acc[5]);
-    o.w = pack_half2(acc[6], acc[7]);
-    *reinterpret_cast<uint4*>(out + pix * Cout + cg * 8) = o;
-  }
-}
-
-// ---------------------------------------------------------------------------------------------------------------
-// conv_out: NHWC [B,H,W,Cin] -> NCHW [B,Cout<=8,H,W], 3x3 pad 1. One warp per output pixel, lanes over channels.
-// ---------------------------------------------------------------------------------------------------------------
-constexpr int CO_MAX = 8;
-__global__ void conv_out_kernel(const __half* __restrict__ x, const __half* __restrict__ w,
-                                const __half* __restrict__ bias, __half* __restrict__ out, int B, int H, int W, int Cin,
-                                int Cout) {
-  pdl_launch_dependents();
-  pdl_wait();
-  extern __shared__ __half s_w[];  // [Cout][9][Cin]
-  for (int i = threadIdx.x; i < Cout * 9 * Cin; i += blockDim.x) {
-    const int o = i / (9 * Cin);
-    const int rem = i - o * 9 * Cin;
-    const int t = rem / Cin, ci = rem - t * Cin;
-    s_w[i] = w[((long long)o * Cin + ci) * 9 + t];  // OIHW source
-  }
-  __syncthreads();
-  const int lane = threadIdx.x & 31;
-  const int warps_per_block = blockDim.x >> 5;
-  const long long npix = (long long)B * H * W;
-  const int CV = Cin >> 3;
-  for (long long pix = (long long)blockIdx.x * warps_per_block + (threadIdx.x >> 5); pix < npix;
-       pix += (long long)gridDim.x * warps_per_block) {
-    const int xw = (int)(pix % W);
-    const int yh = (int)((pix / W) % H);
-    const int b = (int)(pix / ((long long)W * H));
-    float acc[CO_MAX];
-#pragma unroll
-    for (int o = 0; o < CO_MAX; ++o) acc[o] = 0.f;
-    for (int t = 0; t < 9; ++t) {
-      const int yy = yh + t / 3 - 1, xx = xw + t % 3 - 1;
-      if (yy < 0 || yy >= H || xx < 0 || xx >= W) continue;  // warp-uniform
-      const __half* src = x + (((long long)b * H + yy) * W + xx) * Cin;
-      for (int cv = lane; cv < CV; cv += 32) {
-        float xv[8];
-        ld8(src + cv * 8, xv);
-#pragma unroll
-        for (int o = 0; o < CO_MAX; ++o) {
-          if (o < Cout) {
-            float wv[8];
-            ld8(s_w + (o * 9 + t) * Cin + cv * 8, wv);
-#pragma unroll
-            for (int e = 0; e < 8; ++e) acc[o] += xv[e] * wv[e];
-          }
-        }
-      }
-    }
-#pragma unroll
-    for (int o = 0; o < CO_MAX; ++o) {
-#pragma unroll
-      for (int s = 16; s > 0; s >>= 1) acc[o] += __shfl_xor_sync(0xffffffffu, acc[o], s);
-    }
-    if (lane == 0) {
-      for (int o = 0; o < Cout; ++o) {
-        const float bv = bias ? __half2float(bias[o]) : 0.f;
-        out[(((long long)b * Cout + o) * H + yh) * W + xw] = __float2half_rn(acc[o] + bv);
-      }
-    }
-  }
-}
-
-// ---------------------------------------------------------------------------------------------------------------
 // CFG + Euler. Rounding points follow the reference's fp16 tensor arithmetic (custom_pipelines.py:348-350) and
 // diffusers' EulerDiscreteScheduler.step (fp32 inside, result cast back to fp16).
 // ---------------------------------------------------------------------------------------------------------------
@@ -1169,30 +1058,6 @@ extern "C" int ih_concat_f16(const void* x0, int C0, const void* x1, int C1, voi
   return 0;
 }
 
-extern "C" int ih_conv_in_f16(const void* x_nchw, const void* w, const void* bias, void* out, int B, int H, int W,
-                              int Cin, int Cout, void* stream) {
-  IH_CHECK(x_nchw && w && out, IH_ERR_ARG, "ih_conv_in_f16: null pointer");
-  IH_CHECK(Cin <= 8 && Cout % 8 == 0 && Cin * 9 * Cout * 2 <= 48 * 1024, IH_ERR_SHAPE, "ih_conv_in_f16: bad shape");
-  const long long total = (long long)B * H * W * (Cout / 8);
-  IH_CUDA(launch_kernel(conv_in_kernel, dim3(grid_for(total, 256)), dim3(256), (size_t)(Cin * 9 * Cout * 2), (cudaStream_t)stream, 
-      (const __half*)x_nchw, (const __half*)w, (const __half*)bias, (__half*)out, B, H, W, Cin, Cout));
-  return 0;
-}
-
-extern "C" int ih_conv_out_f16(const void* x, const void* w, const void* bias, void* out_nchw, int B, int H, int W,
-                               int Cin, int Cout, void* stream) {
-  IH_CHECK(x && w && out_nchw, IH_ERR_ARG, "ih_conv_out_f16: null pointer");
-  IH_CHECK(Cout <= CO_MAX && Cin % 8 == 0 && Cout * 9 * Cin * 2 <= 48 * 1024, IH_ERR_SHAPE,
-           "ih_conv_out_f16: bad shape");
-  const long long npix = (long long)B * H * W;
-  long long blocks = (npix + 7) / 8;
-  const long long cap = (long long)num_sms() * 8;
-  if (blocks > cap) blocks = cap;
-  IH_CUDA(launch_kernel(conv_out_kernel, dim3((int)blocks), dim3(256), (size_t)(Cout * 9 * Cin * 2), (cudaStream_t)stream, 
-      (const __half*)x, (const __half*)w, (const __half*)bias, (__half*)out_nchw, B, H, W, Cin, Cout));
-  return 0;
-}
-
 extern "C" int ih_euler_cfg_step(const void* noise_pred, void* latents, void* model_in, const void* sigmas, void* step,
                                  float guidance, long long n_per_image, int n_images, void* stream_) {
   cudaStream_t stream = (cudaStream_t)stream_;
@@ -1298,14 +1163,9 @@ extern "C" int ih_euler_ancestral_scale_input(const void* latents, void* model_i
   return 0;
 }
 
-extern "C" int ih_scale_model_input(const void* latents, void* model_in, const void* sigmas, const void* step,
-                                    long long total, void* stream) {
-  return ih_scale_model_input_ex(latents, model_in, sigmas, step, total, 1, stream);
-}
-
 extern "C" int ih_scale_model_input_ex(const void* latents, void* model_in, const void* sigmas, const void* step,
                                        long long total, int duplicate, void* stream) {
-  IH_CHECK(latents && model_in && sigmas && step, IH_ERR_ARG, "ih_scale_model_input: null pointer");
+  IH_CHECK(latents && model_in && sigmas && step, IH_ERR_ARG, "ih_scale_model_input_ex: null pointer");
   IH_CUDA(launch_kernel(scale_model_input_kernel, dim3(grid_for(total, 256)), dim3(256), (size_t)(0), (cudaStream_t)stream, 
       (const __half*)latents, (__half*)model_in, (const float*)sigmas, (const int*)step, total, duplicate ? 1 : 0));
   return 0;
@@ -1387,16 +1247,6 @@ extern "C" int ih_mean_tokens_f16(const void* x, void* out, int B, int n, int D,
   IH_CHECK(x && out && D % 8 == 0 && n > 0, IH_ERR_ARG, "ih_mean_tokens_f16: bad arguments");
   IH_CUDA(launch_kernel(mean_tokens_kernel, dim3((D / 8 + 127) / 128, B), dim3(128), (size_t)0, (cudaStream_t)stream,
                         (const __half*)x, (__half*)out, n, D));
-  return 0;
-}
-
-extern "C" int ih_softmax_rows_f16(void* x, long long ld, long long rows, int cols, void* stream) {
-  IH_CHECK(x && rows > 0 && cols > 0, IH_ERR_ARG, "ih_softmax_rows_f16: bad arguments");
-  IH_CHECK(cols % 8 == 0 && ld % 8 == 0 && cols <= SMX_THREADS * SMX_MAXV * 8, IH_ERR_SHAPE,
-           "ih_softmax_rows_f16: cols must be a multiple of 8 and <= %d", SMX_THREADS * SMX_MAXV * 8);
-  IH_CHECK(rows <= 0x7fffffffLL, IH_ERR_SHAPE, "ih_softmax_rows_f16: too many rows");
-  IH_CUDA(launch_kernel(softmax_rows_kernel, dim3((unsigned)rows), dim3(SMX_THREADS), (size_t)0, (cudaStream_t)stream,
-                        (__half*)x, ld, cols, cols));
   return 0;
 }
 

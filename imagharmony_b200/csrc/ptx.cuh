@@ -1,5 +1,5 @@
 // Inline-PTX wrappers for sm_90a: mbarrier, TMA (cp.async.bulk.tensor), wgmma (warpgroup MMA), PDL.
-// Everything here is device-side plumbing shared by gemm.cu / attn.cu / qxattn.cu.
+// Everything here is device-side plumbing shared by gemm.cu / attn.cu.
 #pragma once
 #include <cuda.h>
 #include <cuda_fp16.h>

@@ -1,6 +1,5 @@
 // Softmax on wgmma accumulator fragments (layout: see ptx.cuh).  A query row lives in the four threads of a quad;
-// thread column pair cq = 2 (lane % 4) of every 8-column group.  Shared by attn.cu and qxattn.cu so that the fused and
-// the two-kernel cross-attention evaluate exactly the same arithmetic.
+// thread column pair cq = 2 (lane % 4) of every 8-column group.  Used by the attention kernels of attn.cu.
 #pragma once
 #include "ptx.cuh"
 

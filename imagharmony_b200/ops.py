@@ -6,7 +6,6 @@ PyTorch/CPU fallback: a CPU tensor or a missing library raises.
 from __future__ import annotations
 
 import ctypes
-import os
 from typing import Optional, Tuple
 
 import torch
@@ -105,12 +104,9 @@ def linear(x: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor] = None
     return out
 
 
-PREFETCH_WEIGHTS = os.environ.get("IH_PREFETCH", "1") != "0"
-
-
 def prefetch_next(w: Optional[torch.Tensor]) -> None:
     """Hint for the NEXT linear / conv3x3 call: while it runs, pull `w` (the weight of the launch after it) into L2."""
-    if PREFETCH_WEIGHTS and w is not None and w.is_cuda:
+    if w is not None and w.is_cuda:
         _lib.load().ih_gemm_prefetch_next(w.data_ptr(), w.numel() * w.element_size())
 
 
@@ -295,7 +291,7 @@ def attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, B: int, H: int,
               n_ip: int = 0, ip_scale: float = 1.0, out: Optional[torch.Tensor] = None,
               kv_split: bool = True) -> torch.Tensor:
     """q [B*Nq, >=H*64] / k, v [B*Nk, >=H*64] 2-D views (row stride arbitrary); returns [B*Nq, H*64].
-    kv_split=False withholds the workspace, i.e. every query tile is processed whole (ih_attention_f16 behaviour)."""
+    kv_split=False withholds the workspace, i.e. every query tile is processed whole."""
     lib = _lib.load()
     _req(q, "q"); _req(k, "k"); _req(v, "v")
     if out is None:
@@ -305,43 +301,6 @@ def attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, B: int, H: int,
                                  _rows(v, "v"), out.data_ptr(), _rows(out, "out"), B, H, Nq, Nk, n_ip,
                                  float(ip_scale), _p(ws), 0 if ws is None else ws.numel(), _stream())
     check(rc, "ih_attention_ws_f16")
-    return out
-
-
-# The fused q-projection + cross-attention kernel runs its per-head attention as a serial chain after the projection,
-# with one CTA per SM; the stand-alone attention kernel hides the same chain behind co-resident CTAs.  It has not been
-# timed against the two-kernel pipeline on the H100, so the processors use it only on request.
-USE_FUSED_XATTN = os.environ.get("IH_XATTN_FUSED", "0") == "1"
-
-
-def xattn_q_fused_ok(Nq: int, Nk: int) -> bool:
-    """Shapes the fused q-projection + short-key cross-attention kernel covers (else: linear + attention)."""
-    return Nq % 128 == 0 and 0 < Nk <= 96
-
-
-def xattn_q_fused(h: torch.Tensor, wq: torch.Tensor, k: torch.Tensor, v: torch.Tensor, B: int, H: int, Nq: int,
-                  Nk: int, *, n_ip: int = 0, ip_scale: float = 1.0, bias: Optional[torch.Tensor] = None, ln=None,
-                  out: Optional[torch.Tensor] = None) -> torch.Tensor:
-    """attention(linear(h, wq, bias, ln=ln), k, v, ...) in one kernel: h [B*Nq, K] raw rows, wq [H*64, K],
-    k / v [B*Nk, >=H*64] views; `ln=(stats, eps)` as in linear().  Returns [B*Nq, H*64]."""
-    lib = _lib.load()
-    _req(h, "h"); _req(wq, "wq"); _req(k, "k"); _req(v, "v")
-    M, K = h.shape
-    if M != B * Nq or tuple(wq.shape) != (H * 64, K) or not wq.is_contiguous():
-        raise IHError(f"xattn_q_fused: h must be [{B * Nq}, K] and wq contiguous [{H * 64}, K]")
-    ln_stats, ln_slabs, ln_eps = None, 0, 0.0
-    if ln is not None:
-        ln_stats, ln_eps = ln
-        _req(ln_stats, "ln_stats", torch.float32)
-        if ln_stats.dim() != 3 or ln_stats.shape[1] != M or ln_stats.shape[0] != (K + 63) // 64 or not ln_stats.is_contiguous():
-            raise IHError("xattn_q_fused: ln statistics must be contiguous [ceil(K/64), M, 2]")
-        ln_slabs = ln_stats.shape[0]
-    if out is None:
-        out = torch.empty((M, H * 64), dtype=torch.float16, device=h.device)
-    rc = lib.ih_xattn_q_fused_f16(h.data_ptr(), _rows(h, "h"), wq.data_ptr(), _p(bias), _p(ln_stats), ln_slabs,
-                                  float(ln_eps), k.data_ptr(), _rows(k, "k"), v.data_ptr(), _rows(v, "v"),
-                                  out.data_ptr(), _rows(out, "out"), B, H, Nq, Nk, n_ip, float(ip_scale), K, _stream())
-    check(rc, "ih_xattn_q_fused_f16")
     return out
 
 
@@ -484,16 +443,6 @@ def resize_patchify(img: torch.Tensor, size: int, patch: int, kpad: int, mean, s
     return out
 
 
-def softmax_rows_(x: torch.Tensor) -> torch.Tensor:
-    """In-place softmax over the last dimension of a 2-D fp16 matrix (row stride arbitrary, cols % 8 == 0, <= 32768)."""
-    lib = _lib.load()
-    _req(x, "x")
-    if x.dim() != 2:
-        raise IHError("softmax_rows_: 2-D matrix required")
-    check(lib.ih_softmax_rows_f16(x.data_ptr(), _rows(x, "x"), x.shape[0], x.shape[1], _stream()), "ih_softmax_rows_f16")
-    return x
-
-
 def add_bcast(a: torch.Tensor, b: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
     """a + b where b is broadcast over the leading elements of a (a.numel() % b.numel() == 0), contiguous fp16."""
     lib = _lib.load()
@@ -553,30 +502,6 @@ def concat_channels(x0: torch.Tensor, x1: torch.Tensor, out: Optional[torch.Tens
     return out
 
 
-def conv_in(x_nchw: torch.Tensor, w: torch.Tensor, bias: torch.Tensor, out: Optional[torch.Tensor] = None):
-    lib = _lib.load()
-    _req(x_nchw, "x")
-    B, Cin, H, W = x_nchw.shape
-    Cout = w.shape[0]
-    if out is None:
-        out = torch.empty((B, H, W, Cout), dtype=torch.float16, device=x_nchw.device)
-    check(lib.ih_conv_in_f16(x_nchw.data_ptr(), w.data_ptr(), _p(bias), out.data_ptr(), B, H, W, Cin, Cout,
-                             _stream()), "ih_conv_in_f16")
-    return out
-
-
-def conv_out(x: torch.Tensor, w: torch.Tensor, bias: torch.Tensor, out: Optional[torch.Tensor] = None):
-    lib = _lib.load()
-    _req(x, "x")
-    B, H, W, Cin = x.shape
-    Cout = w.shape[0]
-    if out is None:
-        out = torch.empty((B, Cout, H, W), dtype=torch.float16, device=x.device)
-    check(lib.ih_conv_out_f16(x.data_ptr(), w.data_ptr(), _p(bias), out.data_ptr(), B, H, W, Cin, Cout, _stream()),
-          "ih_conv_out_f16")
-    return out
-
-
 def im2col3x3_nchw(x_nchw: torch.Tensor, kpad: int = 64, out: Optional[torch.Tensor] = None) -> torch.Tensor:
     """[B, Cin, H, W] -> A [B*H*W, kpad] with k = ci*9 + ky*3 + kx (zero padded): conv_in as a tensor-core GEMM."""
     lib = _lib.load()
@@ -606,7 +531,8 @@ def im2col3x3_nchw_cat(x0: torch.Tensor, x1: torch.Tensor, kpad: int, out: Optio
 
 
 def softmax_rows_masked_(x: torch.Tensor, valid_cols: int) -> torch.Tensor:
-    """softmax_rows_ over the first `valid_cols` columns of each row; the remaining (padding) columns become 0."""
+    """In-place softmax of a 2-D fp16 matrix (row stride arbitrary, cols % 8 == 0, <= 32768) over the first `valid_cols`
+    columns of each row; the remaining (padding) columns become 0."""
     lib = _lib.load()
     _req(x, "x")
     if x.dim() != 2 or not 0 < valid_cols <= x.shape[1]:

@@ -18,7 +18,7 @@
 extern "C" {
 #endif
 
-#define IH_API_VERSION 1
+#define IH_API_VERSION 2
 
 /* epilogue flags for ih_gemm_f16 */
 #define IH_EPI_NONE 0
@@ -105,26 +105,15 @@ int ih_conv2d_down_f16(const void* x, const void* w, const void* bias, void* out
  *   Decoupled IP cross attention (n_ip > 0): keys/values are the concatenation [text (Nk - n_ip) ; ip (n_ip)];
  *     out = softmax_text(q k_t^T/8) v_t + ip_scale * softmax_ip(q k_ip^T/8) v_ip   (two separate softmaxes).
  * Replaces F.scaled_dot_product_attention at attention_processor.py:312-314 (self), :423-425 (text branch),
- * :440-442 + :450 (IP branch and the scale*ip axpy).  Nk <= 128 uses the single-block path. */
-int ih_attention_f16(const void* q, long long ldq, const void* k, long long ldk, const void* v, long long ldv,
-                     void* out, long long ldo, int B, int H, int Nq, int Nk, int n_ip, float ip_scale,
-                     void* stream);
-
-/* ih_attention_f16 with a caller-owned scratch buffer (>= ih_attention_workspace_bytes(...) bytes, no initialisation
- * needed).  With it the long self-attention shapes (Nk > 128, n_ip == 0) cut the query tiles that would otherwise form
- * a nearly empty last wave into KV parts that share one wave and are merged by a second small kernel (flash-decoding
- * style, fixed merge order: deterministic).  workspace == NULL behaves like ih_attention_f16. */
+ * :440-442 + :450 (IP branch and the scale*ip axpy).  Nk <= 128 uses the single-block path.
+ *   workspace: NULL, or a caller-owned scratch buffer (>= ih_attention_workspace_bytes(...) bytes, no initialisation
+ *     needed).  With it the long self-attention shapes (Nk > 128, n_ip == 0) cut the query tiles that would otherwise
+ *     form a nearly empty last wave into KV parts that share one wave and are merged by a second small kernel
+ *     (flash-decoding style, fixed merge order: deterministic).  Without it every query tile is processed whole. */
+int ih_attention_ws_f16(const void* q, long long ldq, const void* k, long long ldk, const void* v, long long ldv,
+                        void* out, long long ldo, int B, int H, int Nq, int Nk, int n_ip, float ip_scale,
+                        void* workspace, long long workspace_bytes, void* stream);
 long long ih_attention_workspace_bytes(int B, int H, int Nq, int Nk, int n_ip);
-/* Fused front half of a cross-attention layer: out = CrossAttn(LayerNorm(h) Wq^T, k, v) for short key axes (Nk <= 96,
- * Nq % 128 == 0): the q projection (K input channels -> H*64) runs as a wgmma GEMM whose epilogue performs the
- * (decoupled) attention per head, so q never goes to HBM.  h: [B*Nq, K] raw rows; wq: [H*64, K]; bias: [H*64] or NULL;
- * ln_stats/ln_slabs/ln_eps as in ih_gemm_ln_f16 (NULL: no folded LayerNorm); k, v, n_ip, ip_scale, out as in
- * ih_attention_f16.  Replaces attention_processor.py:396 (to_q) + :423-425, :440-442, :450 (IPAttnProcessor2_0) and
- * :292, :312-314 (AttnProcessor2_0 with encoder_hidden_states). */
-int ih_xattn_q_fused_f16(const void* h, long long ldh, const void* wq, const void* bias, const void* ln_stats,
-                         int ln_slabs, float ln_eps, const void* k, long long ldk, const void* v, long long ldv,
-                         void* out, long long ldo, int B, int H, int Nq, int Nk, int n_ip, float ip_scale, int K,
-                         void* stream);
 
 /* Test aid: 0 (default) = split only when the cost model predicts a gain, 1 = split every partial last wave (at
  * least 2 parts, even where they overflow into one more wave). */
@@ -133,11 +122,6 @@ void ih_attention_set_split_policy(int policy);
  * kernel, 1 = the two-CTA-per-SM kernel that also serves Nk <= 128.  Rows processed whole are bit-identical between
  * the two; the KV-split plan (and so the rows of split units) follows the selected kernel's residency. */
 void ih_attention_set_kernel(int kernel);
-/* Kept for ABI compatibility: a no-op, the attention kernels record no trace. */
-void ih_attention_set_trace(void* device_buffer);
-int ih_attention_ws_f16(const void* q, long long ldq, const void* k, long long ldk, const void* v, long long ldv,
-                        void* out, long long ldo, int B, int H, int Nq, int Nk, int n_ip, float ip_scale,
-                        void* workspace, long long workspace_bytes, void* stream);
 
 /* GroupNorm over NHWC [B, HW, C] (optionally the channel-concatenation of two tensors x0 [.., C0] and x1 [.., C1]),
  * fp32 partial sums reduced in double, optional fused SiLU.  stats_ws: ih_groupnorm_workspace_bytes(B, groups) bytes,
@@ -177,11 +161,10 @@ int ih_add_bcast_f16(const void* a, const void* b, void* out, long long n, long 
 /* out[b, :] = mean_n x[b, n, :]  -- Resampler masked_mean with an all-ones mask (resampler.py:137-138,150-158). */
 int ih_mean_tokens_f16(const void* x, void* out, int B, int n, int D, void* stream);
 
-/* In-place row softmax of an fp16 matrix [rows, cols] (row stride ld elements, fp32 statistics), cols <= 32768.  With
- * two ih_gemm_f16 calls it forms the single-head, head_dim-512 attention of the VAE decoder mid block
+/* In-place row softmax of an fp16 matrix [rows, cols] (row stride ld elements, fp32 statistics), cols <= 32768, over
+ * the first valid_cols columns of every row (valid_cols = cols: the whole row); the padding columns are written as 0.
+ * With two ih_gemm_f16 calls it forms the single-head, head_dim-512 attention of the VAE decoder mid block
  * ([3P] diffusers AutoencoderKL, called at custom_pipelines.py:373). */
-int ih_softmax_rows_f16(void* x, long long ld, long long rows, int cols, void* stream);
-/* same, with only the first valid_cols columns of every row taking part; the padding columns are written as 0. */
 int ih_softmax_rows_masked_f16(void* x, long long ld, long long rows, int cols, int valid_cols, void* stream);
 
 /* Nearest-neighbour 2x upsample NHWC [B,H,W,C] -> [B,2H,2W,C]. */
@@ -189,13 +172,6 @@ int ih_upsample2x_f16(const void* x, void* out, int B, int H, int W, int C, void
 
 /* Channel concat of two NHWC tensors: out[.., :C0] = x0, out[.., C0:] = x1. rows = B*H*W. */
 int ih_concat_f16(const void* x0, int C0, const void* x1, int C1, void* out, long long rows, void* stream);
-
-/* conv_in: NCHW latent [B,4,H,W] -> NHWC [B,H,W,Cout], 3x3 pad 1 (weight OIHW [Cout,4,3,3]). */
-int ih_conv_in_f16(const void* x_nchw, const void* w, const void* bias, void* out, int B, int H, int W, int Cin,
-                   int Cout, void* stream);
-/* conv_out: NHWC [B,H,W,Cin] -> NCHW [B,Cout,H,W], 3x3 pad 1 (weight OIHW [Cout,Cin,3,3]), Cout <= 8. */
-int ih_conv_out_f16(const void* x, const void* w, const void* bias, void* out_nchw, int B, int H, int W, int Cin,
-                    int Cout, void* stream);
 
 /* conv_in on the tensor-core GEMM: im2col of the NCHW latent into A [B*H*W, Kpad] (k = ci*9 + ky*3 + kx, zero padded),
  * to be multiplied with the OIHW weight flattened (and zero padded) to [Cout, Kpad] by ih_gemm_f16. */
@@ -307,10 +283,8 @@ int ih_euler_ancestral_step(const void* noise_pred, void* latents, void* model_i
 int ih_euler_ancestral_scale_input(const void* latents, void* model_in, const void* coeffs, const void* step,
                                    long long total, int duplicate, void* stream);
 
-/* model_in = cat([latents, latents]) / sqrt(sigma[*step]^2 + 1)   (custom_pipelines.py:332-334, first step). */
-int ih_scale_model_input(const void* latents, void* model_in, const void* sigmas, const void* step, long long total,
-                         void* stream);
-/* same with duplicate = 0: model_in = latents / sqrt(...) for the no-CFG loop (custom_pipelines.py:332 else-branch). */
+/* model_in = cat([latents, latents]) / sqrt(sigma[*step]^2 + 1)   (custom_pipelines.py:332-334, first step); with
+ * duplicate = 0, model_in = latents / sqrt(...) for the no-CFG loop (custom_pipelines.py:332 else-branch). */
 int ih_scale_model_input_ex(const void* latents, void* model_in, const void* sigmas, const void* step, long long total,
                             int duplicate, void* stream);
 

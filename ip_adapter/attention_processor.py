@@ -37,16 +37,13 @@ def _check_sdxl_case(attn, hidden_states, attention_mask):
                       "connection, rescale_output_factor == 1)")
 
 
-def _cross_attention(attn, x, kv, B, N, Nk, C, *, n_ip=0, ip_scale=1.0, ln_stats=None, ln_eps=1e-5, need_q=False):
-    """to_q + (decoupled) SDPA over the cached [K | V] rows: projection GEMM + attention kernel, or (IH_XATTN_FUSED=1,
-    slower at UNet batch 2 -- see ops.USE_FUSED_XATTN) one fused kernel.  Returns (q or None, output [B*N, C])."""
+def _cross_attention(attn, x, kv, B, N, Nk, C, *, n_ip=0, ip_scale=1.0, ln_stats=None, ln_eps=1e-5):
+    """to_q + (decoupled) SDPA over the cached [K | V] rows: projection GEMM + attention kernel.
+    Returns (q, output [B*N, C])."""
     if ln_stats is not None:
         (w, bias), ln = attn._ln, (ln_stats, ln_eps)              # norm2 folded into to_q
     else:
         w, bias, ln = attn.to_q.weight, None, None
-    if ops.USE_FUSED_XATTN and not need_q and ops.xattn_q_fused_ok(N, Nk):
-        return None, ops.xattn_q_fused(x, w, kv[:, :C], kv[:, C:], B, attn.heads, N, Nk, n_ip=n_ip, ip_scale=ip_scale,
-                                       bias=bias, ln=ln)
     ops.prefetch_next(attn.to_out[0].weight)                      # L2 hint: the out projection follows the attention
     q = ops.linear(x, w, bias, ln=ln)
     return q, ops.attention(q, kv[:, :C], kv[:, C:], B, attn.heads, N, Nk, n_ip=n_ip, ip_scale=ip_scale)
@@ -185,7 +182,7 @@ class IPAttnProcessor2_0(torch.nn.Module):
         x = hidden_states.reshape(B * N, C)
         want_map = self.keep_attn_map and not self.skip
         q, o = _cross_attention(attn, x, kv, B, N, Nk, C, n_ip=n_ip, ip_scale=float(self.scale), ln_stats=ln_stats,
-                                ln_eps=ln_eps, need_q=want_map)                   # :396, :423-450
+                                ln_eps=ln_eps)                                    # :396, :423-450
         if want_map:
             k_ip = kv.view(B, Nk, 2 * C)[:, Nk - n_ip:, :C].reshape(B, n_ip, attn.heads, 64).permute(0, 2, 1, 3)
             qh = q.reshape(B, N, attn.heads, 64).permute(0, 2, 1, 3)

@@ -17,10 +17,6 @@ def launch_count_reset():
     _count[0] = 0
 
 
-def _f(t):
-    return None if t is None else t.float()
-
-
 def fold_layernorm(w, bias, gamma, beta):
     w_g = w.double() * gamma.double()[None, :]
     w_c = (w_g - w_g.mean(dim=1, keepdim=True)).to(w.dtype).contiguous()
@@ -76,12 +72,6 @@ def attention_small(q, k, v, B, H, Nq, Nk, dqk, dv, scale, out=None):
     vf = v.float().reshape(B, Nk, H, dv).transpose(1, 2)
     o = torch.softmax(qf @ kf.transpose(-1, -2) / scale, -1) @ vf
     return o.transpose(1, 2).reshape(B * Nq, H * dv).to(q.dtype)
-
-
-def softmax_rows_(x):
-    _count[0] += 1
-    x.copy_(torch.softmax(x.float(), dim=-1).to(x.dtype))
-    return x
 
 
 def softmax_rows_masked_(x, valid_cols):
@@ -142,18 +132,6 @@ def attention(q, k, v, B, H, Nq, Nk, *, n_ip=0, ip_scale=1.0, out=None, kv_split
     return o.transpose(1, 2).reshape(B * Nq, C).to(q.dtype)
 
 
-USE_FUSED_XATTN = False
-
-
-def xattn_q_fused_ok(Nq, Nk):
-    return Nq % 128 == 0 and 0 < Nk <= 96
-
-
-def xattn_q_fused(h, wq, k, v, B, H, Nq, Nk, *, n_ip=0, ip_scale=1.0, bias=None, ln=None, out=None):
-    q = linear(h, wq, bias, ln=ln)
-    return attention(q, k, v, B, H, Nq, Nk, n_ip=n_ip, ip_scale=ip_scale)
-
-
 def groupnorm(x0, gamma, beta, *, x1=None, groups=32, eps=1e-5, silu=False, out=None, ws=None):
     _count[0] += 2
     x = x0 if x1 is None else torch.cat([x0, x1], dim=-1)
@@ -206,16 +184,6 @@ def upsample2x(x, out=None):
 def concat_channels(x0, x1, out=None):
     _count[0] += 1
     return torch.cat([x0, x1], dim=-1)
-
-
-def conv_in(x_nchw, w, bias, out=None):
-    _count[0] += 1
-    return F.conv2d(x_nchw.float(), w.float(), _f(bias), padding=1).permute(0, 2, 3, 1).to(x_nchw.dtype).contiguous()
-
-
-def conv_out(x, w, bias, out=None):
-    _count[0] += 1
-    return F.conv2d(x.float().permute(0, 3, 1, 2), w.float(), _f(bias), padding=1).to(x.dtype).contiguous()
 
 
 def euler_cfg_step(noise_pred, latents, model_in, sigmas, step, guidance):

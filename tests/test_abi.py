@@ -25,7 +25,7 @@ def test_library_exports_every_declared_symbol():
         assert hasattr(lib, name), f"{name} declared in ih_api.h but not exported"
         assert name in _lib.SIGNATURES, f"{name} has no ctypes signature in _lib.SIGNATURES"
     assert set(_lib.SIGNATURES) == set(declared)
-    assert lib.ih_version() == 1
+    assert lib.ih_version() == 2
 
 
 def test_product_path_fails_loudly_without_gpu_tensors():

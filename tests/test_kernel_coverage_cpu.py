@@ -15,7 +15,6 @@ EXEMPT = {
     "ih_launch_count": "launch counter, a diagnostic with no arithmetic",
     "ih_launch_count_reset": "launch counter, a diagnostic with no arithmetic",
     "ih_gemm_set_trace": "debug timestamps, not on the product path",
-    "ih_attention_set_trace": "no-op kept for ABI compatibility",
     "ih_gemm_prefetch_next": "L2 prefetch hint; results never depend on it",
     "ih_attention_set_split_policy": "test aid that selects the KV-split plan of ih_attention_ws_f16",
     "ih_attention_set_kernel": "test aid that selects the multi-block attention kernel of ih_attention_ws_f16",
@@ -30,10 +29,9 @@ REGISTRY = {
     "ih_conv2d_shortcut_f16": ["test_kernels_gpu::test_conv3x3_fused_shortcut"],
     "ih_conv2d_scaled_f16": ["test_kernel_edges_gpu::test_conv2d_scaled_stride2_residual"],
     "ih_conv2d_down_f16": ["test_img2img_gpu::test_conv_down_kernel"],
-    "ih_attention_f16": ["test_kernel_edges_gpu::test_attention_f16_entry"],
     "ih_attention_workspace_bytes": ["test_kernels_gpu::test_attention_kv_split"],
-    "ih_attention_ws_f16": ["test_kernels_gpu::test_attention", "test_kernels_gpu::test_attention_kv_split"],
-    "ih_xattn_q_fused_f16": ["test_kernels_gpu::test_xattn_q_fused"],
+    "ih_attention_ws_f16": ["test_kernels_gpu::test_attention", "test_kernels_gpu::test_attention_kv_split",
+                            "test_kernel_edges_gpu::test_attention_ws_f16_without_workspace"],
     "ih_groupnorm_workspace_bytes": ["test_kernel_edges_gpu::test_groupnorm_workspace_reuse_and_graph_replay"],
     "ih_groupnorm_f16": ["test_kernel_edges_gpu::test_groupnorm_group_counts",
                          "test_kernel_edges_gpu::test_groupnorm_large_group_means",
@@ -45,12 +43,10 @@ REGISTRY = {
     "ih_sinusoid_f16": ["test_kernels_gpu::test_sinusoid"],
     "ih_add_bcast_f16": ["test_kernel_edges_gpu::test_add_bcast"],
     "ih_mean_tokens_f16": ["test_kernel_edges_gpu::test_mean_tokens"],
-    "ih_softmax_rows_f16": ["test_vae_gpu::test_softmax_rows_kernel"],
-    "ih_softmax_rows_masked_f16": ["test_vae_gpu::test_softmax_rows_masked_kernel"],
+    "ih_softmax_rows_masked_f16": ["test_vae_gpu::test_softmax_rows_kernel",
+                                   "test_vae_gpu::test_softmax_rows_masked_kernel"],
     "ih_upsample2x_f16": ["test_kernels_gpu::test_upsample", "test_kernel_edges_gpu::test_upsample2x_odd"],
     "ih_concat_f16": ["test_kernel_edges_gpu::test_concat_channels"],
-    "ih_conv_in_f16": ["test_kernels_gpu::test_conv_in_out"],
-    "ih_conv_out_f16": ["test_kernels_gpu::test_conv_in_out"],
     "ih_im2col3x3_nchw_f16": ["test_inpaint9_gpu::test_im2col_cat_kernel_equals_im2col_of_the_concatenation"],
     "ih_im2col3x3_nchw_cat_f16": ["test_inpaint9_gpu::test_im2col_cat_kernel_equals_im2col_of_the_concatenation"],
     "ih_nhwc_to_nchw_f16": ["test_kernel_edges_gpu::test_nhwc_to_nchw"],
@@ -61,8 +57,8 @@ REGISTRY = {
     "ih_dpm_solver_step": ["test_dpm_gpu::test_dpm_solver_step_kernel"],
     "ih_euler_ancestral_step": ["test_euler_a_gpu::test_euler_ancestral_step_kernel"],
     "ih_euler_ancestral_scale_input": ["test_euler_a_gpu::test_first_input_equals_torch_scale_model_input"],
-    "ih_scale_model_input": ["test_kernel_edges_gpu::test_scale_model_input_entry"],
-    "ih_scale_model_input_ex": ["test_kernels_gpu::test_euler_cfg_step"],
+    "ih_scale_model_input_ex": ["test_kernels_gpu::test_euler_cfg_step",
+                                "test_kernel_edges_gpu::test_scale_model_input_entry"],
     "ih_attention_generic_f16": ["test_clip_gpu::test_attention_generic"],
     "ih_embed_tokens_f16": ["test_kernel_edges_gpu::test_embed_tokens_clamps_ids"],
     "ih_resize_patchify_f16": ["test_clip_gpu::test_embed_quickgelu_resize_kernels"],

@@ -308,18 +308,18 @@ def test_conv2d_scaled_stride2_residual(ops):
 
 
 # ------------------------------------------------------------------------------------------------------------
-# direct calls of the entry points the Python ops layer does not use
+# the attention entry without a workspace, and the first-step input scaling
 # ------------------------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("Nq,Nk,n_ip", [(256, 81, 4), (300, 300, 0)])
-def test_attention_f16_entry(ops, Nq, Nk, n_ip):
-    """ih_attention_f16 (no workspace) computes what ih_attention_ws_f16 computes without one."""
+def test_attention_ws_f16_without_workspace(ops, Nq, Nk, n_ip):
+    """ih_attention_ws_f16 with workspace == NULL processes every query tile whole, as ops.attention(kv_split=False)."""
     lib = _lib.load()
     B, H = 2, 4
     q, k, v = rnd(B * Nq, H * 64), rnd(B * Nk, H * 64, seed=1), rnd(B * Nk, H * 64, seed=2)
     out = torch.empty(B * Nq, H * 64, dtype=torch.float16, device="cuda")
-    rc = lib.ih_attention_f16(q.data_ptr(), q.stride(0), k.data_ptr(), k.stride(0), v.data_ptr(), v.stride(0),
-                              out.data_ptr(), out.stride(0), B, H, Nq, Nk, n_ip, 0.6, stream())
-    _lib.check(rc, "ih_attention_f16")
+    rc = lib.ih_attention_ws_f16(q.data_ptr(), q.stride(0), k.data_ptr(), k.stride(0), v.data_ptr(), v.stride(0),
+                                 out.data_ptr(), out.stride(0), B, H, Nq, Nk, n_ip, 0.6, None, 0, stream())
+    _lib.check(rc, "ih_attention_ws_f16")
     assert torch.equal(out, ops.attention(q, k, v, B, H, Nq, Nk, n_ip=n_ip, ip_scale=0.6, kv_split=False))
     nt = Nk - n_ip
     qd = q.double().reshape(B, Nq, H, 64).transpose(1, 2)
@@ -328,23 +328,18 @@ def test_attention_f16_entry(ops, Nq, Nk, n_ip):
     ref = (qd @ kd[:, :, :nt].transpose(-1, -2) / 8).softmax(-1) @ vd[:, :, :nt]
     if n_ip:
         ref = ref + 0.6 * ((qd @ kd[:, :, nt:].transpose(-1, -2) / 8).softmax(-1) @ vd[:, :, nt:])
-    check(out, ref.transpose(1, 2).reshape(B * Nq, H * 64), f"ih_attention_f16 {Nq}x{Nk} ip{n_ip}")
+    check(out, ref.transpose(1, 2).reshape(B * Nq, H * 64), f"ih_attention_ws_f16 no workspace {Nq}x{Nk} ip{n_ip}")
 
 
 def test_scale_model_input_entry(ops):
-    """ih_scale_model_input is ih_scale_model_input_ex with the CFG duplicate."""
-    lib = _lib.load()
+    """ih_scale_model_input_ex with the CFG duplicate: model_in = cat([x, x]) / sqrt(sigma[*step]^2 + 1)."""
     lat = rnd(3, 4, 24, 40) * 7
     sig = torch.tensor([14.6, 9.1, 0.03], device="cuda")
     step = torch.tensor([1], dtype=torch.int32, device="cuda")
     a = torch.empty(6, 4, 24, 40, dtype=torch.float16, device="cuda")
-    _lib.check(lib.ih_scale_model_input(lat.data_ptr(), a.data_ptr(), sig.data_ptr(), step.data_ptr(), lat.numel(),
-                                        stream()), "ih_scale_model_input")
-    b = torch.empty_like(a)
-    ops.scale_model_input(lat, b, sig, step)
-    assert torch.equal(a, b)
+    ops.scale_model_input(lat, a, sig, step)
     mi = r16(lat.double() / math.sqrt(sig[1].item() ** 2 + 1))
-    close_ulps(a, torch.cat([mi, mi]), "ih_scale_model_input")
+    close_ulps(a, torch.cat([mi, mi]), "ih_scale_model_input_ex")
     assert int(step.item()) == 1, "the input scaling must not advance the step counter"
 
 

@@ -275,56 +275,6 @@ def test_attention_kv_split(ops, B, H, Nq, Nk, qscale):
     assert torch.equal(split, again), "KV-split attention must be run-to-run deterministic"
 
 
-@pytest.mark.parametrize("B,H,Nq,Nk,n_ip,K,fold", [
-    (2, 20, 1024, 81, 4, 1280, True),    # the 10 IMAGHarmony layers at 1024^2 (norm2 folded into to_q)
-    (2, 20, 1024, 81, 4, 1280, False),
-    (2, 10, 4096, 77, 0, 640, True),     # text-only layer at the 640-channel level: ragged head group (10 = 4+4+2)
-    (2, 20, 256, 81, 4, 1280, True),     # 512^2
-    (1, 4, 128, 81, 4, 256, False),      # 4 k-blocks: every ring stage is reused by phase 2 right away
-    (3, 2, 384, 96, 8, 64, False),       # 1 k-block, 2 heads, full 96-key tile
-])
-def test_xattn_q_fused(ops, B, H, Nq, Nk, n_ip, K, fold):
-    """to_q projection (+ folded LayerNorm) + decoupled cross-attention in one kernel vs the two-kernel pipeline and the
-    fp32 reference of attention_processor.py:396-450."""
-    C, M = H * 64, B * Nq
-    scale = 0.7
-    wq = rnd(C, K, scale=K ** -0.5, seed=3)
-    kv = rnd(B * Nk, 2 * C, seed=4)
-    k, v = kv[:, :C], kv[:, C:]
-    if fold:
-        a = rnd(M, K, seed=5)
-        wp = rnd(K, K, scale=K ** -0.5, seed=6)
-        res = rnd(M, K, seed=7) + 0.3
-        stats = torch.empty(((K + 63) // 64, M, 2), dtype=torch.float32, device="cuda")
-        h = ops.linear(a, wp, residual=res, stats_out=stats)
-        gamma = (1 + 0.2 * rnd(K, seed=8).float()).half()
-        beta = (0.1 * rnd(K, seed=9).float()).half()
-        w_c, c = ops.fold_layernorm(wq, None, gamma, beta)
-        ln = (stats, 1e-5)
-        fused = ops.xattn_q_fused(h, w_c, k, v, B, H, Nq, Nk, n_ip=n_ip, ip_scale=scale, bias=c, ln=ln)
-        q = ops.linear(h, w_c, c, ln=ln)
-        q_ref = (F.layer_norm(h.float(), (K,), gamma.float(), beta.float(), 1e-5) @ wq.float().t()).half()
-    else:
-        h = rnd(M, K, seed=5)
-        fused = ops.xattn_q_fused(h, wq, k, v, B, H, Nq, Nk, n_ip=n_ip, ip_scale=scale)
-        q = ops.linear(h, wq)
-        q_ref = (h.float() @ wq.float().t()).half()
-    unfused = ops.attention(q, k, v, B, H, Nq, Nk, n_ip=n_ip, ip_scale=scale)
-    # same arithmetic as the two-kernel pipeline (q rounded to fp16 once, same softmax code)
-    check(fused, unfused.float(), f"xattn fused vs unfused B{B} H{H} {Nq}x{Nk}", rtol=1e-3, atol=1e-3)
-    nt = Nk - n_ip
-    qf = q_ref.float().view(B, Nq, H, 64).transpose(1, 2)
-    kf = k.float().reshape(B, Nk, H, 64).transpose(1, 2)
-    vf = v.float().reshape(B, Nk, H, 64).transpose(1, 2)
-    ref = (qf @ kf[:, :, :nt].transpose(-1, -2) / 8).softmax(-1) @ vf[:, :, :nt]
-    if n_ip:
-        ref = ref + scale * ((qf @ kf[:, :, nt:].transpose(-1, -2) / 8).softmax(-1) @ vf[:, :, nt:])
-    ref = ref.transpose(1, 2).reshape(M, C)
-    # q differs from the reference's by its fp16 rounding point when the LayerNorm is folded: 3e-3
-    tol = 3e-3 if fold else 1e-3
-    check(fused, ref, f"xattn fused B{B} H{H} {Nq}x{Nk} ip{n_ip} K{K} fold{fold}", rtol=tol, atol=tol)
-
-
 def test_attention_fused_qkv_views(ops):
     B, H, N = 2, 10, 512
     C = H * 64
@@ -427,18 +377,6 @@ def test_upsample(ops):
     out = ops.upsample2x(x)
     ref = F.interpolate(x.permute(0, 3, 1, 2).float(), scale_factor=2.0, mode="nearest").permute(0, 2, 3, 1)
     assert torch.equal(out.float(), ref)
-
-
-def test_conv_in_out(ops):
-    B, H = 2, 64
-    x = rnd(B, 4, H, H)
-    w, b = rnd(320, 4, 3, 3, scale=1 / 6), rnd(320)
-    out = ops.conv_in(x, w, b)
-    check(out, F.conv2d(x.float(), w.float(), b.float(), padding=1).permute(0, 2, 3, 1), "conv_in")
-    y = rnd(B, H, H, 320, seed=3)
-    w2, b2 = rnd(4, 320, 3, 3, scale=(9 * 320) ** -0.5), rnd(4)
-    out2 = ops.conv_out(y, w2, b2)
-    check(out2, F.conv2d(y.permute(0, 3, 1, 2).float(), w2.float(), b2.float(), padding=1), "conv_out")
 
 
 def test_euler_cfg_step(ops):

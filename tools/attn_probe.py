@@ -22,25 +22,5 @@ def main():
               f"({fl/t1/1e12:.0f} TF/s)", flush=True)
 
 
-def cross():
-    """q projection + short-key cross attention: two kernels vs the fused one."""
-    for (B, H, N, Nk, nip) in [(2, 20, 1024, 81, 4), (2, 10, 4096, 77, 0), (16, 20, 1024, 81, 4)]:
-        C = H * 64
-        h, wq, kv = r(B * N, C), r(C, C, scale=C ** -0.5), r(B * Nk, 2 * C)
-        k, v = kv[:, :C], kv[:, C:]
-        fl = 2.0 * B * N * C * C + 4.0 * B * H * N * Nk * 64
-
-        def two():
-            q = ops.linear(h, wq)
-            ops.attention(q, k, v, B, H, N, Nk, n_ip=nip, ip_scale=0.7)
-        t0 = timeit(two)
-        t1 = timeit(lambda: ops.xattn_q_fused(h, wq, k, v, B, H, N, Nk, n_ip=nip, ip_scale=0.7))
-        print(f"cross-attn front B{B} H{H} N{N} Nk{Nk}: gemm+attn {t0*1e6:.1f} us ({fl/t0/1e12:.0f} TF/s) -> fused "
-              f"{t1*1e6:.1f} us ({fl/t1/1e12:.0f} TF/s)", flush=True)
-
-
 if __name__ == "__main__":
-    if len(sys.argv) > 1 and sys.argv[1] == "cross":
-        cross()
-    else:
-        main()
+    main()

@@ -15,11 +15,10 @@ GROUPS = [
     ("tests/test_kernels_gpu.py", "test_gemm_geglu"),
     ("tests/test_kernels_gpu.py", "test_gemm_layernorm_fold"),
     ("tests/test_kernels_gpu.py", "test_attention_kv_split"),
-    ("tests/test_kernels_gpu.py", "test_xattn_q_fused"),
     ("tests/test_kernels_gpu.py", "test_conv3x3"),
     ("tests/test_kernels_gpu.py", "test_attention"),
     ("tests/test_kernels_gpu.py", "norm"),
-    ("tests/test_kernels_gpu.py", "test_linear_small or test_sinusoid or test_upsample or test_conv_in_out or test_euler"),
+    ("tests/test_kernels_gpu.py", "test_linear_small or test_sinusoid or test_upsample or test_euler"),
 ]
 
 

@@ -67,11 +67,10 @@ def main():
                              "native_tflops_incl_hoisted_flops": flops / t_nat / 1e12,
                              # FLOPs the per-step layer actually executes (to_q + decoupled attention + to_out; the K/V
                              # projections are hoisted out of the loop): what "fraction of tensor peak" must be quoted on
-                             "native_tflops_executed": (2 * 2.0 * B * N * C * C + 4.0 * B * H * N * L * 64) / t_nat / 1e12,
-                             "fused_q_xattn": os.environ.get("IH_XATTN_FUSED", "0") == "1"})
+                             "native_tflops_executed": (2 * 2.0 * B * N * C * C + 4.0 * B * H * N * L * 64) / t_nat / 1e12})
                 print(json.dumps(rows[-1]), flush=True)
     os.makedirs(os.path.join(ROOT, "tools_out"), exist_ok=True)
-    json.dump(rows, open(os.path.join(ROOT, "tools_out", "layer_head_to_head" + ("_fused" if os.environ.get("IH_XATTN_FUSED", "0") == "1" else "") + ".json"), "w"), indent=1)
+    json.dump(rows, open(os.path.join(ROOT, "tools_out", "layer_head_to_head.json"), "w"), indent=1)
 
 
 if __name__ == "__main__":
