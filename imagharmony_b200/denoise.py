@@ -50,7 +50,7 @@ from ._lib import IH_CN_MAX_NETS, IHError
 from .controlnet import controlnet_scales
 from .scheduler import (DPMSolverMultistepScheduler, EulerAncestralDiscreteScheduler, EulerDiscreteScheduler,
                         randn_tensor)
-from .unet import UNet2DConditionModel
+from .unet import UNet2DConditionModel, require_latent_size
 
 # option -> the options it cannot be combined with, and why
 _EXCLUDES = (
@@ -296,6 +296,7 @@ class DenoiseEngine:
         if (unet_cond is not None) != (ucfg.in_channels != ucfg.out_channels):
             raise IHError(f"unet_cond (mask, masked_image_latents) is required exactly for the 9-channel inpainting "
                           f"UNet; this UNet has {ucfg.in_channels} input channels")
+        require_latent_size(ucfg, h, w)
         if is_ancestral and isinstance(generator, list) and len(generator) != n:
             raise IHError(f"got {len(generator)} generators for a batch of {n}")
         loop_T = T if num_loop_steps is None else int(num_loop_steps)

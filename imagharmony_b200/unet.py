@@ -26,6 +26,16 @@ from ._lib import IHError
 from .config import UNetConfig
 
 
+def require_latent_size(cfg: UNetConfig, h: int, w: int) -> None:
+    """IHError unless an h x w latent fits the UNet: each of its len(block_out_channels) - 1 stride-2 downsamplers
+    halves the sides exactly, and every up-block upsamples to twice its input, so both sides must be divisible by
+    2 ** (len(block_out_channels) - 1) latents (4 for SDXL: images whose sides are multiples of 32 pixels)."""
+    m = 2 ** (len(cfg.block_out_channels) - 1)
+    if h % m or w % m:
+        raise IHError(f"latent size {h}x{w} ({8 * h}x{8 * w} pixels) is not supported: the UNet needs latent sides "
+                      f"divisible by {m}, i.e. image heights and widths that are multiples of {8 * m} pixels")
+
+
 class Attention(nn.Module):
     """Parameter shell with the attributes the reference processors read (attention_processor.py:374-463)."""
 
@@ -551,6 +561,7 @@ class UNet2DConditionModel(SDXLEncoderModel):
         if n_cond > 0 and (cond is None or tuple(cond.shape) != (B, n_cond) + tuple(sample.shape[2:])):
             raise IHError(f"UNet2DConditionModel: the {self.config.in_channels}-channel UNet needs `cond` of shape "
                           f"{(B, n_cond) + tuple(sample.shape[2:])}, got {None if cond is None else tuple(cond.shape)}")
+        require_latent_size(self.config, sample.shape[2], sample.shape[3])
         self._ensure_conditioning(encoder_hidden_states, text_embeds, time_ids, B)
         temb_all = self.time_embeddings(timesteps, step, B)
         Bs, _, Hs, Ws = sample.shape

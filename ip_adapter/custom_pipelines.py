@@ -229,6 +229,8 @@ class StableDiffusionXLCustomPipeline:
         width = width or self.default_sample_size * self.vae_scale_factor
         original_size = original_size or (height, width)                              # :192-193
         target_size = target_size or (height, width)
+        if height % 8 or width % 8:
+            raise ValueError(f"`height` and `width` have to be divisible by 8 but are {height} and {width}.")
         self._check_callback_steps(callback, callback_steps)
         do_classifier_free_guidance = guidance_scale > 1.0                            # :223
         embeds = self.encode_prompt(prompt, prompt_2, None, num_images_per_prompt, do_classifier_free_guidance,

@@ -1,6 +1,7 @@
-"""TEST-ONLY stand-ins for imagharmony_b200.ops implemented with plain PyTorch on the CPU (fp32).  They let the CPU test
-suite validate the *wiring* of the native UNet / processors / denoise loop (layouts, skip order, weight packing, K/V
-caching) against the oracle without a GPU.  Never imported by the product."""
+"""TEST-ONLY stand-ins for imagharmony_b200.ops implemented with plain PyTorch in fp32.  They let the CPU test suite
+validate the *wiring* of the native UNet / processors / denoise loop (layouts, skip order, weight packing, K/V caching)
+against the oracle without a GPU, and they are the per-call reference of the GPU census (tests/census.py), so they run
+on whatever device their inputs live on.  Never imported by the product."""
 import math
 
 import torch
@@ -26,10 +27,15 @@ def fold_layernorm(w, bias, gamma, beta):
     return w_c, c.to(w.dtype)
 
 
+def _up(t):
+    """fp32 compute for fp16 / fp32 operands; fp64 operands stay fp64 (the census' exact GEMM / conv references)."""
+    return t if t.dtype == torch.float64 else t.float()
+
+
 def linear(x, w, bias=None, *, residual=None, rowbias=None, rows_per_group=0, geglu=False, silu=False, gelu=False,
            out=None, tile_n=0, ln=None, stats_out=None, quick_gelu=False, alpha=1.0):
     _count[0] += 1
-    y = (x.float() @ w.float().t()) * alpha
+    y = (_up(x) @ _up(w).t()) * alpha
     if ln is not None:
         st, eps = ln
         K = x.shape[1]
@@ -104,10 +110,10 @@ def conv3x3(x, w_packed, bias=None, *, rowbias=None, residual=None, stride=1, ou
     sc_term = None
     if shortcut is not None:
         src = shortcut[0] if shortcut[1] is None else torch.cat([shortcut[0], shortcut[1]], dim=-1)
-        sc_term = src.float() @ w_packed[:, 9 * Cin:].float().t()
+        sc_term = _up(src) @ _up(w_packed[:, 9 * Cin:]).t()
         w_packed = w_packed[:, : 9 * Cin]
-    w = w_packed.reshape(Cout, 3, 3, Cin).permute(0, 3, 1, 2).float()
-    y = F.conv2d(x.float().permute(0, 3, 1, 2), w, None, stride=stride, padding=1).permute(0, 2, 3, 1) * alpha
+    w = _up(w_packed.reshape(Cout, 3, 3, Cin).permute(0, 3, 1, 2))
+    y = F.conv2d(_up(x).permute(0, 3, 1, 2), w, None, stride=stride, padding=1).permute(0, 2, 3, 1) * alpha
     if bias is not None:
         y = y + bias.float()
     if rowbias is not None:
@@ -168,7 +174,7 @@ def sinusoid(t, dim, n, *, step=None, out=None):
     _count[0] += 1
     half = dim // 2
     tv = t[step.long()].expand(n) if step is not None else t[:n]
-    f = torch.exp(-math.log(10000.0) * torch.arange(half, dtype=torch.float32) / half)
+    f = torch.exp(-math.log(10000.0) * torch.arange(half, dtype=torch.float32, device=t.device) / half)
     a = tv.float().reshape(-1, 1) * f.reshape(1, -1)
     return torch.cat([a.cos(), a.sin()], -1).to(torch.float32 if FP32 else torch.float16)
 
@@ -259,7 +265,7 @@ def attention_generic(q, k, v, B, H, Nq, Nk, dqk, dv, scale, causal=False, out=N
     vh = v[:, :H * dv].float().reshape(B, Nk, H, dv).permute(0, 2, 1, 3)
     s = qh @ kh.transpose(-1, -2) * scale
     if causal:
-        mask = torch.ones(Nq, Nk, dtype=torch.bool).tril(Nk - Nq)
+        mask = torch.ones(Nq, Nk, dtype=torch.bool, device=q.device).tril(Nk - Nq)
         s = s.masked_fill(~mask, float("-inf"))
     o = (s.softmax(-1) @ vh).permute(0, 2, 1, 3).reshape(B * Nq, H * dv).to(q.dtype)
     if out is not None:

@@ -4,7 +4,7 @@ across scheduler swaps and batch sizes, SDXL-base trajectories, and IPAdapterXL.
 import pytest
 import torch
 
-from test_kernels_gpu import check, ops  # noqa: F401  (fixture)
+from test_kernels_gpu import STEP_BUCKETS, check, ops  # noqa: F401  (fixture)
 from test_unet_gpu import _errs, _inputs, _make_pair, sdxl_pair  # noqa: F401  (fixture)
 
 pytestmark = pytest.mark.gpu
@@ -12,15 +12,18 @@ pytestmark = pytest.mark.gpu
 
 @pytest.mark.parametrize("karras", [False, True])
 @pytest.mark.parametrize("n", [1, 3])
-@pytest.mark.parametrize("use_cfg,rescale", [(True, 0.0), (False, 0.0), (True, 0.7)])
-def test_dpm_solver_step_kernel(ops, use_cfg, rescale, n, karras):  # noqa: F811
+@pytest.mark.parametrize("use_cfg,rescale,hw", [
+    pytest.param(True, 0.0, (64, 48), id="True-0.0"), pytest.param(False, 0.0, (64, 48), id="False-0.0"),
+    pytest.param(True, 0.7, (64, 48), id="True-0.7"),
+] + [pytest.param(True, 0.7, hw, id=f"True-0.7-{hw[0]}x{hw[1]}") for hw in STEP_BUCKETS])
+def test_dpm_solver_step_kernel(ops, use_cfg, rescale, n, karras, hw):  # noqa: F811
     """First order at loop_begin (index 0, and mid-schedule with loop_begin there), second order mid-schedule, and the
     final step to sigma 0, which must return x0 exactly.  Without rescale bit-exact against diffusers' expressions
     on the same fp16 CUDA tensors and 0-dim CPU scalars; with rescale the bar of test_kernels_gpu.py::test_euler_step_ex
     (the per-image std is a reduction in another order than torch's)."""
     from dpm_ref import dpm_step_ref
     from imagharmony_b200.scheduler import DPMSolverMultistepScheduler
-    T, h, w = 10, 64, 48
+    T, (h, w) = 10, hw
     s = DPMSolverMultistepScheduler(use_karras_sigmas=karras)
     s.set_timesteps(T)
     coeffs = torch.from_numpy(s.coeffs).cuda()

@@ -5,7 +5,7 @@ resume, an SDXL-base trajectory, and IPAdapterXL.generate over an Euler A pipeli
 import pytest
 import torch
 
-from test_kernels_gpu import check, ops  # noqa: F401  (fixture)
+from test_kernels_gpu import STEP_BUCKETS, check, ops  # noqa: F401  (fixture)
 from test_unet_gpu import _errs, _inputs, _make_pair, sdxl_pair  # noqa: F401  (fixture)
 
 pytestmark = pytest.mark.gpu
@@ -19,12 +19,15 @@ def _table(T):
 
 
 @pytest.mark.parametrize("n", [1, 3])
-@pytest.mark.parametrize("use_cfg,rescale", [(True, 0.0), (False, 0.0), (True, 0.7)])
-def test_euler_ancestral_step_kernel(ops, use_cfg, rescale, n):  # noqa: F811
+@pytest.mark.parametrize("use_cfg,rescale,hw", [
+    pytest.param(True, 0.0, (64, 48), id="True-0.0"), pytest.param(False, 0.0, (64, 48), id="False-0.0"),
+    pytest.param(True, 0.7, (64, 48), id="True-0.7"),
+] + [pytest.param(True, 0.7, hw, id=f"True-0.7-{hw[0]}x{hw[1]}") for hw in STEP_BUCKETS])
+def test_euler_ancestral_step_kernel(ops, use_cfg, rescale, n, hw):  # noqa: F811
     """First, middle and last index.  Without rescale bit-exact against diffusers' expressions on the same fp16 CUDA
     tensors, 0-dim CPU scalars and noise; with rescale the bar of test_kernels_gpu.py::test_euler_step_ex."""
     from euler_a_ref import euler_a_step_ref
-    T, h, w = 10, 64, 48
+    T, (h, w) = 10, hw
     s, coeffs = _table(T)
     b = 2 * n if use_cfg else n
     g = torch.Generator().manual_seed(100 * n + 10 * int(use_cfg) + int(rescale > 0))

@@ -7,22 +7,25 @@ import pytest
 import torch
 
 from test_img2img_gpu import _pipe_and_oracles
-from test_kernels_gpu import check, ops  # noqa: F401  (fixture)
+from test_kernels_gpu import STEP_BUCKETS, check, ops  # noqa: F401  (fixture)
 
 pytestmark = pytest.mark.gpu
 
 
 @pytest.mark.parametrize("frac", [False, True])
 @pytest.mark.parametrize("n", [1, 3])
-@pytest.mark.parametrize("use_cfg,rescale", [(True, 0.0), (False, 0.0), (True, 0.7)])
-def test_euler_inpaint_step_kernel(ops, use_cfg, rescale, n, frac):  # noqa: F811
+@pytest.mark.parametrize("use_cfg,rescale,hw", [
+    pytest.param(True, 0.0, (64, 48), id="True-0.0"), pytest.param(False, 0.0, (64, 48), id="False-0.0"),
+    pytest.param(True, 0.7, (64, 48), id="True-0.7"),
+] + [pytest.param(True, 0.7, hw, id=f"True-0.7-{hw[0]}x{hw[1]}") for hw in STEP_BUCKETS])
+def test_euler_inpaint_step_kernel(ops, use_cfg, rescale, n, frac, hw):  # noqa: F811
     """Steps at the start, in the middle, at blend_end - 1 (the last step of a denoising_end loop: blends with the clean
     latents although sigma[i+1] > 0) and at the end of a 10-step schedule.  Without rescale bit-exact (no fast math:
     IEEE division and sqrt; FMA contraction restated); with rescale the bar of test_kernels_gpu.py::test_euler_step_ex,
     since the per-image std is a reduction in another order than torch's."""
     from imagharmony_b200.scheduler import EulerDiscreteScheduler
     from inpaint_ref import inpaint_step_ref
-    T, h, w = 10, 64, 48
+    T, (h, w) = 10, hw
     sig_np = EulerDiscreteScheduler().set_timesteps(T).sigmas
     sig = torch.from_numpy(sig_np).cuda()
     b = 2 * n if use_cfg else n

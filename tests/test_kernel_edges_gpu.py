@@ -15,6 +15,7 @@ import pytest
 import torch
 import torch.nn.functional as F
 
+from fp16_ulps import close_ulps, ulp16
 from imagharmony_b200 import _lib
 from imagharmony_b200._lib import IHError
 from test_kernels_gpu import check, ops, rnd  # noqa: F401  (fixture)
@@ -36,26 +37,6 @@ def qrnd(*shape, step=0.125, scale=1.0, seed=0):
     exact in fp32 for the sizes used here."""
     g = torch.Generator(device="cpu").manual_seed(seed + 7 * sum(shape))
     return (torch.round(torch.randn(*shape, generator=g, dtype=torch.float64) * scale / step) * step).half().cuda()
-
-
-def ulp16(x):
-    a = x.abs().double().clamp_min(2.0 ** -14)
-    return torch.exp2(torch.floor(torch.log2(a)) - 10)
-
-
-def close_ulps(out, ref, what, ulps=1.0, slack=None):
-    """|out - ref| <= ulps * ulp16(max(|out|, |ref|)) (+ slack: the fp32 accumulation-order allowance)."""
-    out, ref = out.double(), ref.double()
-    assert out.shape == ref.shape, (what, out.shape, ref.shape)
-    assert torch.isfinite(out).all(), f"{what}: non-finite output"
-    err = (out - ref).abs()
-    tol = ulps * ulp16(torch.maximum(out.abs(), ref.abs()))
-    if slack is not None:
-        tol = tol + slack
-    bad = err > tol
-    print(f"[{what}] max_abs_err={err.max().item():.3e} max_err/ulp={(err / ulp16(ref)).max().item():.2f}")
-    assert not bad.any(), (f"{what}: {int(bad.sum())} of {bad.numel()} elements beyond {ulps} ulp, "
-                           f"max err {err.max().item():.3e}")
 
 
 def stream():

@@ -403,18 +403,26 @@ def test_euler_cfg_step(ops):
     check(m2, torch.cat([mi, mi]), "scale_model_input")
 
 
-@pytest.mark.parametrize("use_cfg,rescale", [(False, 0.0), (True, 0.7), (True, 1.0)])
-def test_euler_step_ex(ops, use_cfg, rescale):
+# latent sizes of SDXL buckets (832x1216, 640x1536, 768x1344): the per-image rescale reduction over 4*h*w elements that
+# are not a power of two
+STEP_BUCKETS = [(104, 152), (80, 192), (96, 168)]
+
+
+@pytest.mark.parametrize("use_cfg,rescale,n,h,w", [
+    pytest.param(False, 0.0, 3, 64, 64, id="False-0.0"),
+    pytest.param(True, 0.7, 3, 64, 64, id="True-0.7"),
+    pytest.param(True, 1.0, 3, 64, 64, id="True-1.0"),
+] + [pytest.param(True, 0.7, n, h, w, id=f"True-0.7-n{n}-{h}x{w}") for n in (1, 3) for h, w in STEP_BUCKETS])
+def test_euler_step_ex(ops, use_cfg, rescale, n, h, w):
     """ih_euler_step_ex: no-CFG (custom_pipelines.py:223) and guidance_rescale (:352-354) variants of the transition,
     against the fp16 tensor arithmetic of the reference loop (oracle/scheduler_ref.py rescale_noise_cfg)."""
     from oracle.scheduler_ref import rescale_noise_cfg
-    n, H = 3, 64
     b = 2 * n if use_cfg else n
-    lat = rnd(n, 4, H, H) * 5
-    noise = rnd(b, 4, H, H, seed=2)
+    lat = rnd(n, 4, h, w) * 5
+    noise = rnd(b, 4, h, w, seed=2)
     sig = torch.tensor([13.1204, 11.6761, 10.4250, 0.0], device="cuda")
     step = torch.tensor([1], dtype=torch.int32, device="cuda")
-    model_in = torch.empty(b, 4, H, H, dtype=torch.float16, device="cuda")
+    model_in = torch.empty(b, 4, h, w, dtype=torch.float16, device="cuda")
     lat_ref = lat.clone()
     ops.euler_step(noise, lat, model_in, sig, step, 5.0, use_cfg=use_cfg, guidance_rescale=rescale)
     if use_cfg:

@@ -65,6 +65,7 @@ def _refused_calls(T, n, lat, nets):
         ("euler", dict(controlnet=[a, ControlNetCall(wide, img, 1.0, False)]), "block_out_channels"),
         ("euler", dict(controlnet=ControlNetCall(a.model, img, 1.0, False, [1.0] * (T - 1))), "keep"),
         ("euler", dict(controlnet=[a, ControlNetCall(b.model, _image(n, 8 * lat + 8), 1.0, False)]), "image"),
+        ("euler", dict(latents=torch.zeros(n, 4, lat + 2, lat)), "latent size"),    # the stride-2 convs need h % 4 == 0
     ]
     return calls
 
@@ -86,7 +87,7 @@ def test_refused_calls_do_no_work(mcp):  # noqa: F811
                   "dpm": DPMSolverMultistepScheduler}
     engines = {k: DenoiseEngine(pipe.unet, use_cuda_graph=False, scheduler=s()) for k, s in schedulers.items()}
     calls = _refused_calls(T, n, lat, pipe.controlnet.nets)
-    assert len(calls) == sum(len(v) for v in EXCLUDES.values()) + 16
+    assert len(calls) == sum(len(v) for v in EXCLUDES.values()) + 17
     kv = _kv_buffers(models)
     for kind, kw, words in calls:
         eng = engines[kind]
@@ -102,3 +103,24 @@ def test_refused_calls_do_no_work(mcp):  # noqa: F811
     with _Empty32():
         engines["euler"].run(**args, controlnet=ControlNetCall(pipe.controlnet.nets[0], _image(n, 8 * lat), 1.0, False))
     assert ops.launch_count() > launches and engines["euler"]._pool and _kv_buffers(models) > kv
+
+
+@pytest.mark.parametrize("height,width,error", [(1001, 1024, ValueError), (1000, 1000, "IHError"),
+                                                (1016, 1024, "IHError")])
+def test_pipeline_refuses_sizes_the_unet_cannot_run(patched, height, width, error):  # noqa: F811
+    """Text-to-image at a size that is not a multiple of 8 is a ValueError (as diffusers' check_inputs), and at a
+    multiple of 8 that is not one of 32 (the UNet's two stride-2 convs halve the latent twice) an IHError from the
+    engine, before it launches anything or allocates a static buffer."""
+    from imagharmony_b200 import ops
+    from imagharmony_b200._lib import IHError
+    from imagharmony_b200.config import TINY
+    from ip_adapter.custom_pipelines import StableDiffusionXLCustomPipeline
+    pipe = StableDiffusionXLCustomPipeline.from_random(TINY, seed=0, device="cpu")
+    pe, pooled = torch.randn(1, 81, TINY.cross_attention_dim).half(), torch.randn(1, TINY.pooled_embed_dim).half()
+    launches = ops.launch_count()
+    with pytest.raises(IHError if error == "IHError" else error, match="divisible by"):
+        pipe(prompt_embeds=pe, negative_prompt_embeds=pe, pooled_prompt_embeds=pooled,
+             negative_pooled_prompt_embeds=pooled, num_inference_steps=4, output_type="latent", height=height,
+             width=width)
+    assert ops.launch_count() == launches
+    assert not pipe.engine._pool and not pipe.engine._schedules
