@@ -45,9 +45,11 @@ def _fp16_representable(m):
     return m
 
 
-def resize_patchify_ref(img: torch.Tensor, size: int, patch: int, kpad: int, mean, std) -> torch.Tensor:
-    """img [B, 3, H, W] fp32 in [-1, 1] -> area-average to size x size (exact box filter with fractional pixel
-    coverage) -> [0, 1] clamp -> (v - mean) / std -> patch rows [B * (size/patch)^2, kpad], k = c*P*P + py*P + px."""
+def resize_patchify_ref(img: torch.Tensor, size: int, patch: int, kpad: int, mean, std,
+                        dtype: torch.dtype = torch.float32) -> torch.Tensor:
+    """img [B, 3, H, W] in [-1, 1] on the CPU -> area-average to size x size (exact box filter with fractional pixel
+    coverage) -> [0, 1] clamp -> (v - mean) / std -> patch rows [B * (size/patch)^2, kpad], k = c*P*P + py*P + px,
+    computed in `dtype` (fp32; fp64 for the per-call kernel census)."""
     B, C, H, W = img.shape
 
     def weights(n_in: int) -> torch.Tensor:          # [size, n_in] coverage of input pixel x by output pixel o
@@ -55,13 +57,13 @@ def resize_patchify_ref(img: torch.Tensor, size: int, patch: int, kpad: int, mea
         o = torch.arange(size, dtype=torch.float64)[:, None]
         x = torch.arange(n_in, dtype=torch.float64)[None, :]
         w = (torch.minimum((o + 1) * f, x + 1) - torch.maximum(o * f, x)).clamp_min(0)
-        return (w / w.sum(dim=1, keepdim=True)).float()
+        return (w / w.sum(dim=1, keepdim=True)).to(dtype)
     wy, wx = weights(H), weights(W)
-    small = torch.einsum("oy,bcyx,px->bcop", wy, img.float(), wx)
+    small = torch.einsum("oy,bcyx,px->bcop", wy, img.to(dtype), wx)
     v = (small * 0.5 + 0.5).clamp(0, 1)
-    v = (v - torch.tensor(mean).view(1, 3, 1, 1)) / torch.tensor(std).view(1, 3, 1, 1)
+    v = (v - torch.tensor(mean, dtype=dtype).view(1, 3, 1, 1)) / torch.tensor(std, dtype=dtype).view(1, 3, 1, 1)
     g = size // patch
     rows = v.reshape(B, C, g, patch, g, patch).permute(0, 2, 4, 1, 3, 5).reshape(B * g * g, C * patch * patch)
-    out = torch.zeros((B * g * g, kpad), dtype=torch.float32)
+    out = torch.zeros((B * g * g, kpad), dtype=dtype)
     out[:, : rows.shape[1]] = rows
     return out

@@ -29,27 +29,91 @@ plus the magnitudes the bars need.  Bars (max err / bar <= 1 passes):
   (resp. sum x^2): any fp32 summation order of N terms;
 * attention: P is packed to fp16 before the PV MMA (half an fp16 ulp of every p) and exp / the score sums in fp32 stay
   below another half: 1 ulp + 2^-10 * (P @ |V|), the IP part weighted by |ip_scale|;
-* norms, linear_small, sinusoid, masked softmax: the bars of their existing kernel tests, against unrounded fp32.
+* norms, linear_small, sinusoid, masked softmax: the bars of their existing kernel tests, against unrounded fp32;
+* conv3x3_down (the VAE encoder's bottom/right-padded stride-2 conv, conv_impl on the same wgmma main loop): the
+  conv3x3 bar with K = 9 Cin, against F.pad(x, (0, 1, 0, 1)) and a stride-2, pad-0 conv in fp64;
+* conv3x3_small (one thread per output, a sequential fp32 fmaf over the 9 Cin products in tap order, + bias, SiLU as
+  acc / (1 + __expf(-acc)), one fp16 rounding), against fp64: half an ulp, plus (9 Cin + 1) 2^-24 (conv |x| * |w| + |b|)
+  for the 9 Cin fma roundings and the bias add (round-to-nearest loses at most 2^-24 of a running sum, which never
+  exceeds the magnitude), times SLOPE under SiLU, plus EPI |out| for __expf and the divide (a relative error e of
+  __expf moves SiLU by at most e |SiLU|);
+* attention_generic (fp32 scores by a sequential fma over dqk, times scale; fp32 softmax with __expf; fp32 PV by a
+  sequential fma over the live keys; times 1 / sum; one fp16 rounding), against fp64 with the causal mask: half an
+  ulp, plus (P @ |V|) times
+  - 2 max_j ds_j, the score error ds_j = (dqk + 1) 2^-24 (|q| . |k_j|) scale carried through the softmax (a score
+    move ds_j changes p_j by a factor within exp(+-2 max ds)),
+  - 2 (2^-21 + 2^-24 max_j |s_j - s_max|) for __expf (ex2.approx and the rounding of its scaled argument),
+  - (2 Nk + 3) 2^-24 for the two fp32 sums of Nk terms, 1 / sum and the final product;
+* attention_small (fp32 q . k rounded to fp16, divided by the fp32 scale, rounded to fp16 again -- both the
+  reference's rounding points, attention_processor.py:45 --; fp32 softmax with __expf; each p stored as fp16 before
+  the fp32 PV): the reference takes the same two fp16 roundings of the fp64 dot product.  The kernel's fp32 dot product
+  may round to the neighbouring fp16 score, so every score may be 1 fp16 ulp off: with d = max_j ulp16(s_j) each p_j
+  moves by a factor within exp(+-2d), and as sum p_j = 1 on both sides that costs (e^{2d} - 1) (P @ |V - out|).  Then
+  the fp16 store of p (2^-11 p_j, or 2^-25 below the fp16 normal range) and the fp32 arithmetic before it (__expf and the
+  sum, as for attention_generic), over P @ |V| resp. sum |V|; plus (Nk + 1) 2^-24 (P @ |V|) for the PV sum, and half an
+  ulp of the output;
+* embed_tokens, add_bcast: bit-exact against (a.float() + b.float()).half() (embed_tokens with the ids clamped to the
+  vocabulary as the kernel clamps them): fp32 carries at least 2 * 11 + 2 significant bits, so rounding the exact sum
+  of two fp16 values first to fp32 and then to fp16 gives the same fp16 value as rounding it once;
+* mean_tokens (a sequential fp32 sum of n terms, times the fp32 reciprocal of n, one fp16 rounding), against fp64:
+  half an ulp, plus n 2^-24 mean|x| for the sum, plus 2 2^-24 |out| for the reciprocal and the product;
+* resize_patchify (area average in fp32, [0, 1], (v - mean) / std), against oracle.clip_ref.resize_patchify_ref in
+  fp64, per element: the pixel-boundary products oy * fy round twice (fy, then the product), so each boundary moves by
+  at most Hin 2^-23; only the two edge rows and columns of a window carry a boundary, so the area-weighted average
+  moves by at most 2 max|x| (2 fx Hin 2^-23 + 2 fy Win 2^-23) / (fy fx) = max|x| S 2^-20, plus 2 max|x| 2^-24 for the
+  wy * wx products and 2 n_px 2^-24 max|x| for the two fma sums over the window's n_px pixels, 2^-24 for the divide;
+  then * 0.5 + 0.5, - mean and / std add four fp32 roundings of values below 1 + max|x| and the / std multiplies the
+  error by up to 1 / min(std) = 3.8; plus half an ulp of the output;
+* im2col3x3_nchw_cat, controlnet_add_residuals(_multi): bit-exact against the stand-ins (tests/fake_ops_inpaint9.py,
+  tests/fake_ops_controlnet.py, tests/fake_ops_multi_controlnet.py), which round where the kernels round.  The two
+  injection ops add into `skips` in place: the reference applies the stand-in to a snapshot taken before the call and
+  compares every skip tensor after it, rows outside the injected window included;
+* vae_posterior_noise: the bar of test_img2img_gpu.py::test_posterior_noise_kernel, 1 fp16 ulp against
+  img2img_ref.posterior_noise_ref (the same rounding points; the fp32 exp may differ in the last bit), and overflow to
+  inf at the same elements.
+
+The scheduler step kernels and the model-input scaling are not model ops: STEP_KERNELS names the bit-exact test that
+checks each at SDXL bucket latent sizes.
 """
 import inspect
+import math
 
 import torch
 import torch.nn.functional as F
 
 import fake_ops
-from fp16_ulps import ulp_err_tol
+import fake_ops_controlnet
+import fake_ops_img2img
+import fake_ops_inpaint9
+import fake_ops_multi_controlnet
+from fp16_ulps import ulp16, ulp_err_tol
 
-EXEMPT = {"prefetch_next", "fold_layernorm", "pack_conv3x3_weight", "workspace_generation", "launch_count"}
+EXEMPT = {"prefetch_next", "fold_layernorm", "pack_conv3x3_weight", "workspace_generation", "launch_count",
+          "launch_count_reset"}
+STEP_KERNELS = {       # op -> the test that checks it bit-exactly at SDXL bucket latent sizes
+    "euler_cfg_step": "test_kernels_gpu.py::test_euler_cfg_step",
+    "euler_step": "test_kernels_gpu.py::test_euler_step_ex",
+    "euler_inpaint_step": "test_inpaint_gpu.py::test_euler_inpaint_step_kernel",
+    "dpm_solver_step": "test_dpm_gpu.py::test_dpm_solver_step_kernel",
+    "euler_ancestral_step": "test_euler_a_gpu.py::test_euler_ancestral_step_kernel",
+    "scale_model_input": "test_kernel_edges_gpu.py::test_scale_model_input_entry",
+    "euler_ancestral_scale_input": "test_euler_a_gpu.py::test_first_input_equals_torch_scale_model_input",
+}
 ACC_STEP = 2.0 ** -23     # one rounding of the fp32 accumulator per k16 MMA step, relative to |A| @ |W|^T
 EPI = 2.0 ** -21          # the fp32 epilogue, relative to the values it forms
 SLOPE = 1.13              # max |d act / dx| of GELU(erf) (1.129); SiLU and quick-GELU peak at 1.100
 U32 = 2.0 ** -24
 
 
+def _is_stand_in(module_name):
+    return module_name.rsplit(".", 1)[-1].startswith("fake_ops")     # tests/fake_ops.py and every tests/fake_ops_*.py
+
+
 def op_names(ops):
     """Public functions of the ops module (or of the stand-ins patched into it), without its imports."""
     return sorted(n for n, f in vars(ops).items()
-                  if not n.startswith("_") and inspect.isfunction(f) and f.__module__ in (ops.__name__, fake_ops.__name__))
+                  if not n.startswith("_") and inspect.isfunction(f)
+                  and (f.__module__ == ops.__name__ or _is_stand_in(f.__module__)))
 
 
 # ---------------------------------------------------------------------------------------------------------------------
@@ -208,6 +272,140 @@ def _exact(fn, *names):
     return lambda res, p: exact_ratio(res, fn(*(p[n] for n in names)))
 
 
+def _w4(w_packed, Cin):
+    """Tap-major [Cout, 9 Cin] -> OIHW [Cout, Cin, 3, 3] in fp64."""
+    return w_packed.double().reshape(w_packed.shape[0], 3, 3, Cin).permute(0, 3, 1, 2)
+
+
+def ref_conv3x3_down(res, p):
+    x = p["x"].double()
+    w = _w4(p["w_packed"], x.shape[-1])
+
+    def conv(x, w, alpha):
+        return F.conv2d(F.pad(x.permute(0, 3, 1, 2), (0, 1, 0, 1)), w, stride=2).permute(0, 2, 3, 1) * alpha
+    ref = conv(x, w, p["alpha"]) + (0.0 if p["bias"] is None else p["bias"].double())
+    mag = conv(x.abs(), w.abs(), abs(p["alpha"]))
+    return ulp_ratio(res, ref, 0.5, acc_allowance(9 * x.shape[-1]) * mag + 2 * EPI * ref.abs())
+
+
+def ref_conv3x3_small(res, p):
+    x = p["x"].double()
+    x = x if p["nchw"] else x.permute(0, 3, 1, 2)
+    Cin = x.shape[1]
+    w = _w4(p["w_packed"], Cin)
+    b = None if p["bias"] is None else p["bias"].double()
+    pre = F.conv2d(x, w, b, stride=p["stride"], padding=1)
+    s = (9 * Cin + 1) * U32 * F.conv2d(x.abs(), w.abs(), None if b is None else b.abs(), stride=p["stride"], padding=1)
+    ref = pre
+    if p["silu"]:
+        ref = F.silu(pre)
+        s = SLOPE * s + EPI * ref.abs()
+    return ulp_ratio(res, ref.permute(0, 2, 3, 1), 0.5, s.permute(0, 2, 3, 1))
+
+
+def _heads(t, B, N, H, d):
+    return t[:, :H * d].double().reshape(B, N, H, d).transpose(1, 2)
+
+
+def _flat(t):
+    B, H, N, d = t.shape
+    return t.transpose(1, 2).reshape(B * N, H * d)
+
+
+def ref_attention_generic(res, p):
+    B, H, Nq, Nk, dqk, dv, scale = (p[n] for n in ("B", "H", "Nq", "Nk", "dqk", "dv", "scale"))
+    q, k, v = _heads(p["q"], B, Nq, H, dqk), _heads(p["k"], B, Nk, H, dqk), _heads(p["v"], B, Nk, H, dv)
+    s = q @ k.transpose(-1, -2) * scale
+    smag = q.abs() @ k.abs().transpose(-1, -2) * abs(scale)
+    live = torch.ones(Nq, Nk, dtype=torch.bool, device=s.device)
+    if p["causal"]:
+        live = live.tril(Nk - Nq)
+    s = s.masked_fill(~live, float("-inf"))
+    P = s.softmax(-1)
+    ds = (dqk + 1) * U32 * smag.masked_fill(~live, 0).amax(-1, keepdim=True)
+    spread = (s.amax(-1, keepdim=True) - s).masked_fill(~live, 0).amax(-1, keepdim=True)
+    rel = 2 * ds + 2 * (2.0 ** -21 + U32 * spread) + (2 * Nk + 3) * U32
+    return ulp_ratio(res, _flat(P @ v), 0.5, _flat(rel * (P @ v.abs())))
+
+
+def ref_attention_small(res, p):
+    B, H, Nq, Nk, dqk, dv = (p[n] for n in ("B", "H", "Nq", "Nk", "dqk", "dv"))
+    q, k, v = _heads(p["q"], B, Nq, H, dqk), _heads(p["k"], B, Nk, H, dqk), _heads(p["v"], B, Nk, H, dv)
+    scale32 = float(torch.tensor(p["scale"], dtype=torch.float32))        # the kernel divides by the fp32 value
+    qk16 = (q @ k.transpose(-1, -2)).half().double()
+    s16 = (qk16 / scale32).half().double()
+    P = s16.softmax(-1)
+    out = P @ v
+    # a neighbouring fp16 q.k moves the quotient by ulp16(q.k) / scale before its own rounding
+    d = (ulp16(qk16) / scale32 + ulp16(s16)).amax(-1, keepdim=True)
+    grow = torch.exp(2 * d)
+    spread = (s16.amax(-1, keepdim=True) - s16).amax(-1, keepdim=True)
+    pre = 2.0 ** -21 + U32 * spread + (Nk + 2) * U32                      # __expf, the fp32 sum, 1 / sum, p * inv
+    pv = grow * (P @ v.abs())
+    centred = (P[..., None] * (v[:, :, None] - out[:, :, :, None]).abs()).sum(-2)      # sum_j p_ij |v_j - out_i|
+    slack = ((grow - 1) * centred + (2.0 ** -11 + pre + (Nk + 1) * U32) * pv
+             + 2.0 ** -25 * v.abs().sum(-2, keepdim=True))
+    return ulp_ratio(res, _flat(out), 0.5, _flat(slack))
+
+
+def ref_embed_tokens(res, p):
+    ids, tok, pos = p["ids"], p["tok_emb"], p["pos_emb"]
+    B, T = ids.shape
+    rows = tok[ids.long().clamp(0, tok.shape[0] - 1)]
+    return exact_ratio(res, (rows.float() + pos[:T].float()[None]).to(tok.dtype).reshape(B * T, -1))
+
+
+def ref_add_bcast(res, p):
+    a, b = p["a"], p["b"]
+    return exact_ratio(res, (a.float().reshape(-1, b.numel()) + b.float().reshape(1, -1)).to(a.dtype).reshape(a.shape))
+
+
+def ref_mean_tokens(res, p):
+    x = p["x"].double()
+    ref = x.mean(dim=1)
+    return ulp_ratio(res, ref, 0.5, x.shape[1] * U32 * x.abs().mean(dim=1) + 2 * U32 * ref.abs())
+
+
+def ref_resize_patchify(res, p):
+    from oracle.clip_ref import resize_patchify_ref
+    img, S = p["img"], p["size"]
+    _, _, Hin, Win = img.shape
+    ref = resize_patchify_ref(img.cpu().double(), S, p["patch"], p["kpad"], p["mean"], p["std"], dtype=torch.float64)
+    A = float(img.abs().max())
+    n_px = (math.ceil(Hin / S) + 2) * (math.ceil(Win / S) + 2)
+    d_avg = A * (S * 2.0 ** -20 + 2 * U32 + 2 * n_px * U32 + U32)
+    d = (0.5 * d_avg + 4 * U32 * (1 + A)) / min(float(s) for s in p["std"])
+    return ulp_ratio(res.cpu(), ref, 0.5, d + U32 * ref.abs())
+
+
+def _injection_ratio(res, p, inject):
+    """Every skip tensor after an in-place injection against the stand-in applied to the pre-call snapshot."""
+    want = [s.clone() for s in p["skips"]]
+    inject(want)
+    if len(res) != len(want):
+        return float("inf")
+    return max(exact_ratio(r, w) for r, w in zip(res, want))
+
+
+def ref_controlnet_add_residuals(res, p):
+    return _injection_ratio(res, p, lambda sk: fake_ops_controlnet.controlnet_add_residuals(
+        sk, p["residuals"], p["scale"], p["skip_row0s"]))
+
+
+def ref_controlnet_add_residuals_multi(res, p):
+    return _injection_ratio(res, p, lambda sk: fake_ops_multi_controlnet.controlnet_add_residuals_multi(
+        sk, p["residuals_per_net"], p["scales_per_net"], p["skip_row0s"]))
+
+
+def ref_vae_posterior_noise(res, p):
+    ref = fake_ops_img2img.vae_posterior_noise(p["moments"], p["eps"], p["noise"], p["channels"], p["scaling_factor"],
+                                               p["sigma"])
+    fin = torch.isfinite(ref)
+    if res.shape != ref.shape or not torch.equal(torch.isfinite(res), fin) or not torch.equal(res[~fin], ref[~fin]):
+        return float("inf")
+    return ulp_ratio(res[fin], ref[fin], 1.0)                              # test_posterior_noise_kernel's bar
+
+
 REFERENCES = {
     "linear": ref_linear,
     "conv3x3": ref_conv3x3,
@@ -221,8 +419,22 @@ REFERENCES = {
     "concat_channels": _exact(fake_ops.concat_channels, "x0", "x1"),
     "im2col3x3_nchw": _exact(fake_ops.im2col3x3_nchw, "x_nchw", "kpad"),
     "nhwc_to_nchw": _exact(fake_ops.nhwc_to_nchw, "x", "C"),
+    "conv3x3_down": ref_conv3x3_down,
+    "conv3x3_small": ref_conv3x3_small,
+    "attention_generic": ref_attention_generic,
+    "attention_small": ref_attention_small,
+    "embed_tokens": ref_embed_tokens,
+    "add_bcast": ref_add_bcast,
+    "mean_tokens": ref_mean_tokens,
+    "resize_patchify": ref_resize_patchify,
+    "im2col3x3_nchw_cat": _exact(fake_ops_inpaint9.im2col3x3_nchw_cat, "x0", "x1", "kpad"),
+    "controlnet_add_residuals": ref_controlnet_add_residuals,
+    "controlnet_add_residuals_multi": ref_controlnet_add_residuals_multi,
+    "vae_posterior_noise": ref_vae_posterior_noise,
 }
-IN_PLACE = {"softmax_rows_masked_": "x"}       # op -> the argument it overwrites (and returns)
+# op -> the argument it overwrites: an op that returns it gets it back; for one that returns None (the ControlNet
+# injections) the reference receives the argument itself, after the call, as the result
+IN_PLACE = {"softmax_rows_masked_": "x", "controlnet_add_residuals": "skips", "controlnet_add_residuals_multi": "skips"}
 OUTPUTS = {"out", "stats_out"}                  # written by the op: compared after the call, never snapshotted
 NOT_KEYED = {"ws"}                            # persistent scratch: its size does not change what the op computes
 
@@ -264,6 +476,21 @@ def _label(name, p):
     if name == "groupnorm":
         c1 = 0 if p["x1"] is None else p["x1"].shape[-1]
         return f"{dims(p['x0'])}+{c1} g{p['groups']}{' silu' if p['silu'] else ''}"
+    if name in ("attention_generic", "attention_small"):
+        causal = " causal" if p.get("causal") else ""
+        return f"B{p['B']} H{p['H']} {p['Nq']}x{p['Nk']} d{p['dqk']}/{p['dv']}{causal}"
+    if name == "conv3x3_small":
+        return (f"{dims(p['x'])}{' nchw' if p['nchw'] else ''}->{p['w_packed'].shape[0]} s{p['stride']}"
+                f"{' silu' if p['silu'] else ''}")
+    if name == "conv3x3_down":
+        return f"{dims(p['x'])}->{p['w_packed'].shape[0]}" + ("" if p["alpha"] == 1.0 else f" alpha={p['alpha']:g}")
+    if name == "resize_patchify":
+        return f"{dims(p['img'])}->{p['size']}"
+    if name == "vae_posterior_noise":
+        return f"moments {dims(p['moments'])} eps {dims(p['eps'])} {p['eps'].dtype} noise {dims(p['noise'])}"
+    if name in IN_PLACE and name != "softmax_rows_masked_":
+        nets = f" K{len(p['residuals_per_net'])}" if "residuals_per_net" in p else ""
+        return f"{len(p['skips'])} skips {dims(p['skips'][0])} row0 {p['skip_row0s'][0]}{nets}"
     tensors = [v for v in p.values() if isinstance(v, torch.Tensor)]
     return dims(tensors[0]) if tensors else ""
 
@@ -307,7 +534,8 @@ class Census:
                 snap = {n: (v if n in OUTPUTS else _snapshot(v)) for n, v in p.items()}
             res = orig(*a, **k)
             row["checked"] += 1
-            row["worst"] = max(row["worst"], ref(res, snap))
+            got = p[IN_PLACE[name]] if res is None and name in IN_PLACE else res
+            row["worst"] = max(row["worst"], ref(got, snap))
             return res
         wrapped.__wrapped_op__ = orig
         return wrapped
