@@ -13,7 +13,7 @@ from __future__ import annotations
 
 import json
 import os
-from dataclasses import dataclass, fields
+from dataclasses import dataclass
 from typing import List, Optional, Sequence
 
 import torch
@@ -21,7 +21,7 @@ import torch.nn as nn
 
 from . import ops
 from ._lib import IH_CN_MAX_NETS, IHError
-from .config import ControlNetConfig
+from .config import ControlNetConfig, config_from_diffusers
 from .unet import DownBlock, MidBlock, SDXLEncoderModel, TimestepEmbedding
 
 
@@ -128,7 +128,7 @@ class ControlNetModel(SDXLEncoderModel):
         self.down_blocks = nn.ModuleList(downs)
         self.controlnet_down_blocks = nn.ModuleList([nn.Conv2d(c, c, 1) for c in res_ch])
         self.controlnet_mid_block = nn.Conv2d(boc[-1], boc[-1], 1)
-        self.mid_block = MidBlock(cfg, boc[-1], tl[-1])
+        self.mid_block = MidBlock(cfg, boc[-1], cfg.mid_depth)
         self._zc = None
 
     # ------------------------------------------------------------------------------------------------------------
@@ -140,23 +140,7 @@ class ControlNetModel(SDXLEncoderModel):
             meta = json.load(f)
         if meta.get("global_pool_conditions", False):
             raise IHError("ControlNet models with global_pool_conditions = true are not supported")
-        cfg = ControlNetConfig()
-        names = {f.name for f in fields(ControlNetConfig)}
-        # attention_head_dim is a per-level head count in diffusers' SDXL configs; the head width here is fixed at 64
-        upd = {k: (tuple(v) if isinstance(v, list) else v) for k, v in meta.items()
-               if k in names and k != "attention_head_dim"}
-        if "projection_class_embeddings_input_dim" in meta:
-            upd["pooled_embed_dim"] = int(meta["projection_class_embeddings_input_dim"]) - 6 * int(
-                meta.get("addition_time_embed_dim", cfg.addition_time_embed_dim))
-        tl = upd.get("transformer_layers_per_block", cfg.transformer_layers_per_block)
-        if isinstance(tl, int):
-            upd["transformer_layers_per_block"] = (tl,) * len(upd.get("block_out_channels", cfg.block_out_channels))
-        dbt = meta.get("down_block_types")
-        if dbt is not None:      # diffusers lists DownBlock2D for the attention-free levels; depth 0 here
-            upd["transformer_layers_per_block"] = tuple(0 if not t.startswith("CrossAttn") else d
-                                                        for t, d in zip(dbt, upd["transformer_layers_per_block"]))
-        import dataclasses
-        cfg = dataclasses.replace(cfg, **upd)
+        cfg = config_from_diffusers(meta, ControlNetConfig)
         for name in ("diffusion_pytorch_model.safetensors", "diffusion_pytorch_model.fp16.safetensors"):
             f = os.path.join(path, name)
             if os.path.exists(f):

@@ -156,7 +156,7 @@ class DenoiseEngine:
                 "model_in": self._buf("model_in", key, (b, cfg.out_channels, h, w)),
                 "ehs": self._buf("ehs", key, (b, L, cfg.cross_attention_dim)),
                 "text_embeds": self._buf("text_embeds", key, (b, cfg.pooled_embed_dim)),
-                "time_ids": self._buf("time_ids", key, (b, 6), torch.float32),
+                "time_ids": self._buf("time_ids", key, (b, cfg.num_time_ids), torch.float32),
                 "step": self._buf("step", key, (1,), torch.int32, zero=True)}
 
     def _draw_ancestral_noise(self, buf: torch.Tensor, generator, begin: int, end: int) -> None:

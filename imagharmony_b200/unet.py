@@ -433,7 +433,10 @@ class SDXLEncoderModel(nn.Module):
         for name, attn in self._attn_modules():
             if attn.is_cross and hasattr(attn.processor, "prepare"):
                 attn.processor.prepare(attn, ehs, text_only=text_only)
-        tid = ops.sinusoid(time_ids.reshape(-1).float().contiguous(), cfg.addition_time_embed_dim, B * 6)
+        if time_ids.numel() != B * cfg.num_time_ids:
+            raise IHError(f"time_ids: {cfg.num_time_ids} micro-conditioning ids per image expected, got a tensor of shape "
+                          f"{tuple(time_ids.shape)} for {B} images")
+        tid = ops.sinusoid(time_ids.reshape(-1).float().contiguous(), cfg.addition_time_embed_dim, B * cfg.num_time_ids)
         add_in = torch.cat([text_embeds.to(torch.float16), tid.reshape(B, -1)], dim=-1).contiguous()
         h = ops.linear_small(add_in, self.add_embedding.linear_1.weight, self.add_embedding.linear_1.bias, act_out=True)
         buf = self._aug_bufs.get(B)                            # one buffer per batch size, never freed or moved
@@ -500,14 +503,20 @@ class UNet2DConditionModel(SDXLEncoderModel):
             ups.append(UpBlock(cfg, prev, skip_ch, co, rtl[i], add_up=i < len(rev) - 1))
             prev = co
         self.up_blocks = nn.ModuleList(ups)
-        self.mid_block = MidBlock(cfg, boc[-1], tl[-1])
+        self.mid_block = MidBlock(cfg, boc[-1], cfg.mid_depth)
         self.conv_norm_out = nn.GroupNorm(cfg.norm_num_groups, boc[0], eps=1e-5)
         self.conv_out = nn.Conv2d(boc[0], cfg.out_channels, 3, padding=1)
 
     def install_default_processors(self, scale: float = 1.0):
-        """IPAdapter.set_ip_adapter (ip_adapter.py:99-125) for this UNet; IP weights are zero until loaded."""
-        from ip_adapter.attention_processor import AttnProcessor2_0, IPAttnProcessor2_0
+        """IPAdapter.set_ip_adapter (ip_adapter.py:99-125) for this UNet; IP weights are zero until loaded.  A UNet
+        without image-prompt tokens (num_ip_tokens = 0, the refiner) gets diffusers' default instead: every
+        cross-attention attends to all text tokens (CNAttnProcessor2_0 with num_tokens = 0, as on the ControlNet)."""
+        from ip_adapter.attention_processor import AttnProcessor2_0, CNAttnProcessor2_0, IPAttnProcessor2_0
         cfg = self.config
+        if cfg.num_ip_tokens == 0:
+            procs = CNAttnProcessor2_0(num_tokens=0)
+            self.set_attn_processor(procs)
+            return self.attn_processors
         procs = {}
         dev = self.conv_in.weight.device
         for name, attn in self._attn_modules():

@@ -18,6 +18,7 @@ pipeline owns one (`from_random`, or `from_pretrained` with a `vae/` folder); a 
 from __future__ import annotations
 
 import hashlib
+import json
 import os
 from dataclasses import dataclass
 from typing import Any, Callable, Dict, List, Optional, Tuple, Union
@@ -26,11 +27,11 @@ import torch
 
 from imagharmony_b200 import ops
 from imagharmony_b200._lib import IHError
-from imagharmony_b200.config import SDXL_BASE, SDXL_CONTROLNET, ControlNetConfig, UNetConfig
+from imagharmony_b200.config import SDXL_BASE, SDXL_CONTROLNET, ControlNetConfig, UNetConfig, config_from_diffusers
 from imagharmony_b200.denoise import DenoiseEngine
 from imagharmony_b200.scheduler import (DPMSolverMultistepScheduler, EulerAncestralDiscreteScheduler,
                                         EulerDiscreteScheduler, randn_tensor)
-from imagharmony_b200.unet import UNet2DConditionModel
+from imagharmony_b200.unet import UNet2DConditionModel, require_latent_size
 
 from .utils import is_torch2_available
 
@@ -62,13 +63,40 @@ class SyntheticPromptEncoder:
         return torch.stack(hs).half(), torch.stack(pooled).half()
 
 
+def _fraction(value) -> bool:
+    """[3P] diffusers' denoising_value_valid: denoising_start / denoising_end take effect only as a float in (0, 1)."""
+    return isinstance(value, float) and 0 < value < 1
+
+
+def denoising_start_begin_step(timesteps, num_train_timesteps: int, denoising_start: float) -> int:
+    """[3P] StableDiffusionXLImg2ImgPipeline.get_timesteps with a valid `denoising_start` (first-order schedulers): the
+    loop runs the n timesteps below int(round(N - denoising_start * N)), the last n of the schedule, so it begins at
+    index len(timesteps) - n.  A base run with denoising_end = denoising_start keeps the timesteps at or above the same
+    cutoff, so it ends at that same index: the handoff repeats and skips no step."""
+    cutoff = int(round(num_train_timesteps - denoising_start * num_train_timesteps))
+    return len(timesteps) - int(sum(1 for t in timesteps if t < cutoff))
+
+
+def _read_json(path: str, *parts: str) -> dict:
+    f = os.path.join(path, *parts)
+    if not os.path.exists(f):
+        return {}
+    with open(f) as fh:
+        return json.load(fh)
+
+
 class StableDiffusionXLCustomPipeline:
     vae_scale_factor = 8
-    force_zeros_for_empty_prompt = True     # [3P] SDXL-base pipeline config
+    force_zeros_for_empty_prompt = True     # [3P] SDXL-base pipeline config; from_pretrained reads model_index.json
+    TIME_IDS = (6,)                         # the UNet micro-conditioning id counts this pipeline forms
 
     def __init__(self, unet: UNet2DConditionModel, prompt_encoder: Optional[Callable] = None,
                  vae_decode: Optional[Callable] = None,
                  scheduler: Optional[Union[EulerDiscreteScheduler, DPMSolverMultistepScheduler]] = None, vae=None):
+        if unet.config.num_time_ids not in self.TIME_IDS:
+            raise IHError(f"{type(self).__name__} needs a UNet with {' or '.join(map(str, self.TIME_IDS))} "
+                          f"micro-conditioning ids; this one has {unet.config.num_time_ids} (a UNet that requires an "
+                          "aesthetics score, the SDXL refiner, runs in StableDiffusionXLImg2ImgPipeline)")
         self.unet = unet
         self.vae = vae                      # imagharmony_b200.vae.AutoencoderKLDecoder or None
         self.scheduler = scheduler or EulerDiscreteScheduler()
@@ -100,14 +128,25 @@ class StableDiffusionXLCustomPipeline:
     def from_pretrained(cls, path: str, torch_dtype=torch.float16, add_watermarker: bool = False, device="cuda",
                         cfg: Optional[UNetConfig] = None, vae_cfg=None, **kwargs):
         """test.py:68-72.  Loads `<path>/unet/diffusion_pytorch_model.safetensors` (diffusers key names are the native
-        UNet's key names, so no key map is needed).  Without `cfg` the UNet is SDXL-base with the input channel count
-        of the checkpoint's conv_in (4, or 9 for the inpainting UNet)."""
-        unet, enc, vae, _, _ = cls._load_pretrained(path, torch_dtype, device, cfg, vae_cfg)
-        return cls(unet, prompt_encoder=enc, vae=vae)
+        UNet's key names, so no key map is needed).  Without `cfg` the UNet's architecture comes from
+        `<path>/unet/config.json` when there is one (see _load_pretrained), else it is SDXL-base with the input channel
+        count of the checkpoint's conv_in (4, or 9 for the inpainting UNet)."""
+        unet, enc, vae, _, _, index = cls._load_pretrained(path, torch_dtype, device, cfg, vae_cfg)
+        return cls(unet, prompt_encoder=enc, vae=vae)._configure(index)
+
+    def _configure(self, index: dict):
+        """Per-checkpoint pipeline settings from model_index.json: force_zeros_for_empty_prompt (true for the base,
+        false for the refiner: an absent negative prompt is then encoded as "")."""
+        if "force_zeros_for_empty_prompt" in index:
+            self.force_zeros_for_empty_prompt = bool(index["force_zeros_for_empty_prompt"])
+        return self
 
     @staticmethod
     def _load_pretrained(path: str, torch_dtype, device, cfg: Optional[UNetConfig], vae_cfg):
-        """-> (unet, prompt encoder or None, VAE decoder or None, VAE state dict or None, VAE config or None)."""
+        """-> (unet, prompt encoder or None, VAE decoder or None, VAE state dict or None, VAE config or None,
+        model_index.json as a dict, {} without one).  Without `cfg` the UNet's architecture comes from unet/config.json
+        (with model_index.json's requires_aesthetics_score: 5 time ids when true) or, without that file, is SDXL-base
+        with the input channel count of the checkpoint's conv_in."""
         from safetensors.torch import load_file
         f = os.path.join(path, "unet", "diffusion_pytorch_model.safetensors")
         if not os.path.exists(f):
@@ -115,6 +154,10 @@ class StableDiffusionXLCustomPipeline:
         if not os.path.exists(f):
             raise FileNotFoundError(f"no SDXL UNet weights under {path}/unet (safetensors)")
         usd = load_file(f)
+        index = _read_json(path, "model_index.json")
+        meta = _read_json(path, "unet", "config.json")
+        if cfg is None and meta:
+            cfg = config_from_diffusers(meta, UNetConfig, bool(index.get("requires_aesthetics_score", False)))
         if cfg is None:
             cfg = SDXL_BASE
             if "conv_in.weight" in usd and usd["conv_in.weight"].shape[1] != cfg.in_channels:
@@ -144,7 +187,7 @@ class StableDiffusionXLCustomPipeline:
         from .encoders import ClipPromptEncoder
         if ClipPromptEncoder.available(path):
             enc = ClipPromptEncoder.from_pretrained(path, device=device, dtype=torch_dtype)
-        return unet, enc, vae, vsd, vcfg
+        return unet, enc, vae, vsd, vcfg, index
 
     def to(self, device=None, *args, **kwargs):
         """Weights live on the device the UNet was built on (from_random / from_pretrained take `device=`); moving 5 GB
@@ -248,11 +291,11 @@ class StableDiffusionXLCustomPipeline:
 
     def _denoise_from(self, lat, t_start: int, num_inference_steps: int, denoising_end, embeds, sizes, guidance_scale,
                       guidance_rescale, control_guidance_start, control_guidance_end, callback, callback_steps,
-                      inpaint=None, generator=None, unet_cond=None, controlnet=None) -> torch.Tensor:
+                      inpaint=None, generator=None, unet_cond=None, controlnet=None, aesthetic=None) -> torch.Tensor:
         """The loop over timesteps[t_start:], truncated by denoising_end (:307-316), from the noised start latents `lat`
-        with the IP scale of the processors (:319-322); the micro-conditioning time ids are formed from `sizes`
-        (requires_aesthetics_score = False). -> final latents."""
-        add_time_ids, negative_add_time_ids = self._add_time_ids(embeds[0].shape[0], sizes)
+        with the IP scale of the processors (:319-322); the micro-conditioning time ids are formed from `sizes`, and
+        from `aesthetic` = (aesthetic_score, negative_aesthetic_score) for a 5-id UNet. -> final latents."""
+        add_time_ids, negative_add_time_ids = self._add_time_ids(embeds[0].shape[0], sizes, aesthetic)
         loop_end = num_inference_steps
         if denoising_end is not None and isinstance(denoising_end, float) and 0 < denoising_end < 1:
             n_train = self.scheduler.num_train_timesteps
@@ -284,14 +327,21 @@ class StableDiffusionXLCustomPipeline:
             raise IHError(f"{type(self).__name__} does not implement {refused}")
 
     @staticmethod
-    def _add_time_ids(batch: int, sizes) -> Tuple[torch.Tensor, Optional[torch.Tensor]]:
+    def _add_time_ids(batch: int, sizes, aesthetic=None) -> Tuple[torch.Tensor, Optional[torch.Tensor]]:
         """:277-294 [3P] _get_add_time_ids: (positive, negative or None) micro-conditioning ids [batch, 6] from `sizes` =
         (original_size, crops_coords_top_left, target_size, negative_original_size, negative_crops_coords_top_left,
-        negative_target_size); requires_aesthetics_score = False."""
+        negative_target_size); requires_aesthetics_score = False.  With `aesthetic` = (aesthetic_score,
+        negative_aesthetic_score) it is the image-to-image requires_aesthetics_score = True form, [batch, 5] each:
+        original_size + crops + (aesthetic_score,) and negative_original_size (default: original_size) +
+        negative_crops + (negative_aesthetic_score,)."""
         original_size, crops, target_size, neg_original_size, neg_crops, neg_target_size = sizes
 
         def time_ids(size, crop, target):
             return torch.tensor([list(size) + list(crop) + list(target)], dtype=torch.float32).repeat(batch, 1)
+        if aesthetic is not None:
+            score, neg_score = aesthetic
+            return (time_ids(original_size, crops, [score]),
+                    time_ids(neg_original_size or original_size, neg_crops, [neg_score]))
         negative = None
         if neg_original_size is not None and neg_target_size is not None:
             negative = time_ids(neg_original_size, neg_crops, neg_target_size)
@@ -378,11 +428,23 @@ class StableDiffusionXLImg2ImgPipeline(StableDiffusionXLCustomPipeline):
     prompt batch with torch.cat (prompt slot b gets image b % n_images, while num_images_per_prompt repeats prompts
     in place), with a list of generators each slot encodes image b % n_images with its own generator.
     The SDXL-base configuration has requires_aesthetics_score = False: `aesthetic_score` / `negative_aesthetic_score`
-    are accepted and unused."""
+    are accepted and unused.  A UNet with 5 micro-conditioning ids (the SDXL refiner, unet.config.num_time_ids = 5)
+    requires them: its time ids are original_size + crops + (aesthetic_score,) for the positive half and
+    negative_original_size + negative_crops + (negative_aesthetic_score,) for the negative one.
+
+    Ensemble of experts ([3P] diffusers `denoising_start`): the base runs with `denoising_end=d, output_type="latent"`,
+    and this pipeline (usually on the refiner) finishes with `image=<those latents>, denoising_start=d`.  A [B, 4, h, w]
+    `image` is taken as latents: not encoded, scaled or noised, no random draw, tiled to the prompt batch like encoded
+    latents; the loop runs the last n timesteps, those below the cutoff int(round(1000 - d * 1000)), on the same engine
+    and graphs (DenoiseEngine.run(begin_step=T - n)), and returns the latents unchanged when n = 0.  `strength` is
+    validated and unused.  Latents need a valid `denoising_start` (a float in (0, 1); other values are ignored, as in
+    diffusers), and `denoising_start` needs latents: a pixel image with it (encoded without noise) is not implemented;
+    both raise IHError."""
 
     # diffusers arguments that change the result and have no native implementation: refused, never ignored
-    UNSUPPORTED = ("denoising_start", "timesteps", "sigmas", "latents", "ip_adapter_image", "ip_adapter_image_embeds",
+    UNSUPPORTED = ("timesteps", "sigmas", "latents", "ip_adapter_image", "ip_adapter_image_embeds",
                    "clip_skip", "callback_on_step_end")
+    TIME_IDS = (5, 6)
 
     def __init__(self, unet: UNet2DConditionModel, prompt_encoder: Optional[Callable] = None,
                  vae_decode: Optional[Callable] = None,
@@ -410,12 +472,12 @@ class StableDiffusionXLImg2ImgPipeline(StableDiffusionXLCustomPipeline):
     def from_pretrained(cls, path: str, torch_dtype=torch.float16, add_watermarker: bool = False, device="cuda",
                         cfg: Optional[UNetConfig] = None, vae_cfg=None, **kwargs):
         """As StableDiffusionXLCustomPipeline.from_pretrained; the VAE checkpoint also provides the encoder."""
-        unet, enc, vae, vsd, vcfg = cls._load_pretrained(path, torch_dtype, device, cfg, vae_cfg)
+        unet, enc, vae, vsd, vcfg, index = cls._load_pretrained(path, torch_dtype, device, cfg, vae_cfg)
         vae_encoder = None
         if vsd is not None:
             from imagharmony_b200.vae import AutoencoderKLEncoder
             vae_encoder = AutoencoderKLEncoder.from_state_dict(vcfg, vsd, device=device)
-        return cls(unet, prompt_encoder=enc, vae=vae, vae_encoder=vae_encoder)
+        return cls(unet, prompt_encoder=enc, vae=vae, vae_encoder=vae_encoder)._configure(index)
 
     def enable_vae_tiling(self):
         super().enable_vae_tiling()
@@ -438,6 +500,15 @@ class StableDiffusionXLImg2ImgPipeline(StableDiffusionXLCustomPipeline):
         eps = self._posterior_eps(batch_size if isinstance(generator, list) else n_img, h, w, generator)
         noise = randn_tensor((batch_size, L, h, w), generator, torch.float16, self.device, "cpu")
         return ops.vae_posterior_noise(moments, eps, noise, L, venc.config.scaling_factor, sigma)
+
+    def prepare_handoff_latents(self, latents: torch.Tensor, batch_size: int) -> torch.Tensor:
+        """[3P] StableDiffusionXLImg2ImgPipeline.prepare_latents(add_noise=False) for a latent `image`: the latents as
+        they are (fp16 on the device), tiled to the prompt batch with torch.cat like encoded latents."""
+        n_img = latents.shape[0]
+        if batch_size % n_img:
+            raise ValueError(f"cannot duplicate a latent batch of {n_img} to a prompt batch of {batch_size}")
+        lat = latents.to(self.device, torch.float16)
+        return lat.repeat(batch_size // n_img, 1, 1, 1) if batch_size > n_img else lat
 
     def _posterior_eps(self, n: int, h: int, w: int, generator) -> torch.Tensor:
         """The posterior draw of [3P] diffusers' `_encode_vae_image(images, generator)` for n images with latents of
@@ -463,22 +534,39 @@ class StableDiffusionXLImg2ImgPipeline(StableDiffusionXLCustomPipeline):
                  target_size: Optional[Tuple[int, int]] = None, negative_original_size=None,
                  negative_crops_coords_top_left=(0, 0), negative_target_size=None, aesthetic_score: float = 6.0,
                  negative_aesthetic_score: float = 2.5, control_guidance_start: float = 0.0,
-                 control_guidance_end: float = 1.0, **kwargs):
+                 control_guidance_end: float = 1.0, denoising_start: Optional[float] = None, **kwargs):
         """The text-to-image parameter list without height / width, plus `image` (PIL image(s) or a [B, 3, H, W]
-        tensor in [-1, 1]) and `strength`.  Unknown keywords are ignored as in the text-to-image pipeline, except the
-        diffusers arguments in UNSUPPORTED, which raise IHError."""
+        tensor in [-1, 1], or [B, 4, h, w] latents with `denoising_start`), `strength` and `denoising_start`.  Unknown
+        keywords are ignored as in the text-to-image pipeline, except the diffusers arguments in UNSUPPORTED, which
+        raise IHError."""
         self._require_euler()
         self._require_latent_unet()
         self._refuse_unsupported(kwargs)
-        t_start = self._begin_index(num_inference_steps, strength)
+        start = denoising_start if _fraction(denoising_start) else None
+        if start is not None and _fraction(denoising_end) and start >= denoising_end:
+            raise ValueError(f"`denoising_start`: {start} cannot be larger than or equal to `denoising_end`: "
+                             f"{denoising_end} when using type float.")
+        handoff = isinstance(image, torch.Tensor) and image.dim() == 4 and image.shape[1] == self.unet.config.out_channels
+        if handoff != (start is not None):
+            raise IHError("a latent `image` [B, 4, h, w] needs `denoising_start` as a float in (0, 1)" if handoff else
+                          "`denoising_start` continues from latents (`image` [B, 4, h, w], e.g. a base run's "
+                          "output_type='latent' with denoising_end); a pixel image with denoising_start is not implemented")
+        if start is None:
+            t_start = self._begin_index(num_inference_steps, strength)
+        elif not 0.0 <= strength <= 1.0:
+            raise ValueError(f"The value of strength should in [0.0, 1.0] but is {strength}")
         self._check_callback_steps(callback, callback_steps)
         if image is None:
             raise ValueError("`image` input cannot be undefined")
-        if self.vae_encoder is None:
-            raise IHError("this pipeline has no VAE encoder: build it with from_random(vae_cfg=...) or from_pretrained "
-                          "with a vae/ folder")
-        pixels = preprocess_image(image, self.vae_scale_factor)
-        height, width = pixels.shape[2], pixels.shape[3]
+        if handoff:
+            height, width = image.shape[2] * self.vae_scale_factor, image.shape[3] * self.vae_scale_factor
+        else:
+            if self.vae_encoder is None:
+                raise IHError("this pipeline has no VAE encoder: build it with from_random(vae_cfg=...) or "
+                              "from_pretrained with a vae/ folder")
+            pixels = preprocess_image(image, self.vae_scale_factor)
+            height, width = pixels.shape[2], pixels.shape[3]
+        require_latent_size(self.unet.config, height // self.vae_scale_factor, width // self.vae_scale_factor)
         original_size = original_size or (height, width)
         target_size = target_size or (height, width)
         do_classifier_free_guidance = guidance_scale > 1.0
@@ -486,12 +574,18 @@ class StableDiffusionXLImg2ImgPipeline(StableDiffusionXLCustomPipeline):
                                     negative_prompt, negative_prompt_2, prompt_embeds, negative_prompt_embeds,
                                     pooled_prompt_embeds, negative_pooled_prompt_embeds)
         self.scheduler.set_timesteps(num_inference_steps)
-        lat = self.prepare_img2img_latents(pixels, embeds[0].shape[0], generator, self.scheduler.add_noise_sigma(t_start))
+        if handoff:
+            t_start = denoising_start_begin_step(self.scheduler.timesteps, self.scheduler.num_train_timesteps, start)
+            lat = self.prepare_handoff_latents(image, embeds[0].shape[0])
+        else:
+            lat = self.prepare_img2img_latents(pixels, embeds[0].shape[0], generator,
+                                               self.scheduler.add_noise_sigma(t_start))
         sizes = (original_size, crops_coords_top_left, target_size, negative_original_size,
                  negative_crops_coords_top_left, negative_target_size)
+        aesthetic = (aesthetic_score, negative_aesthetic_score) if self.unet.config.num_time_ids == 5 else None
         out = self._denoise_from(lat, t_start, num_inference_steps, denoising_end, embeds, sizes, guidance_scale,
                                  guidance_rescale, control_guidance_start, control_guidance_end, callback, callback_steps,
-                                 generator=generator)
+                                 generator=generator, aesthetic=aesthetic)
         return self._output(out, output_type, return_dict)
 
     def _require_euler(self) -> None:
@@ -556,7 +650,9 @@ class StableDiffusionXLInpaintPipeline(StableDiffusionXLImg2ImgPipeline):
     (DenoiseEngine.run(unet_cond=...)).  At strength 1 the image itself is not encoded (SURVEY C.32).
     `padding_mask_crop` is not implemented and raises IHError, as does a UNet with any other channel count."""
 
-    UNSUPPORTED = StableDiffusionXLImg2ImgPipeline.UNSUPPORTED + ("masked_image_latents", "padding_mask_crop")
+    UNSUPPORTED = StableDiffusionXLImg2ImgPipeline.UNSUPPORTED + ("denoising_start", "masked_image_latents",
+                                                                  "padding_mask_crop")
+    TIME_IDS = (6,)
 
     def prepare_inpaint_latents(self, image: torch.Tensor, batch_size: int, generator, t_start: int,
                                 is_strength_max: bool) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
@@ -779,8 +875,8 @@ class StableDiffusionXLControlNetPipeline(StableDiffusionXLCustomPipeline):
         SDXL folder `path` of StableDiffusionXLCustomPipeline.from_pretrained."""
         if controlnet is None:
             raise ValueError("StableDiffusionXLControlNetPipeline.from_pretrained needs controlnet=")
-        unet, enc, vae, _, _ = cls._load_pretrained(path, torch_dtype, device, cfg, vae_cfg)
-        return cls(unet, controlnet, prompt_encoder=enc, vae=vae)
+        unet, enc, vae, _, _, index = cls._load_pretrained(path, torch_dtype, device, cfg, vae_cfg)
+        return cls(unet, controlnet, prompt_encoder=enc, vae=vae)._configure(index)
 
     def _align_multi(self, image, scale, start, end):
         """[3P] diffusers 0.30 for a MultiControlNetModel: scalar guidance start / end become lists (the length of the

@@ -7,7 +7,9 @@ generic causal attention kernel, LayerNorm); `transformers` is used for what is 
 BPE tokenizers, the PIL image preprocessing and reading a checkpoint folder.  Semantics restated from diffusers==0.30.0:
   * each prompt is tokenised by both tokenizers with padding="max_length" (77) and truncation;
   * prompt_embeds = concat(hidden_states[-2] of encoder 1 [.., 768], hidden_states[-2] of encoder 2 [.., 1280]) -> 2048;
-  * pooled_prompt_embeds = `text_embeds` of encoder 2 (the projected pooled output) -> 1280.
+  * pooled_prompt_embeds = `text_embeds` of encoder 2 (the projected pooled output) -> 1280;
+  * a model that ships only tokenizer_2 / text_encoder_2 (the SDXL refiner) encodes with tower 2 alone:
+    prompt_embeds = its hidden_states[-2] [.., 1280] (encode_prompt with text_encoder = None).
 No weights or tokenizer vocabularies exist offline; tests build random CLIP models and a toy vocabulary."""
 from __future__ import annotations
 
@@ -22,25 +24,37 @@ from imagharmony_b200.clip import ClipTextTower, ClipVisionTower
 class ClipPromptEncoder:
     def __init__(self, tokenizer, tokenizer_2, text_encoder, text_encoder_2, device="cuda", dtype=torch.float16):
         """`text_encoder*`: transformers CLIPTextModel / CLIPTextModelWithProjection instances (their weights are copied
-        into native towers and the HF modules are dropped) or ready `ClipTextTower`s."""
-        self.tokenizers = [tokenizer, tokenizer_2]
+        into native towers and the HF modules are dropped) or ready `ClipTextTower`s.  `tokenizer` and `text_encoder`
+        may both be None: the single-tower (refiner) mode."""
+        if (tokenizer is None) != (text_encoder is None) or tokenizer_2 is None or text_encoder_2 is None:
+            raise ValueError("ClipPromptEncoder needs tokenizer_2 and text_encoder_2, and tokenizer with text_encoder "
+                             "(both or neither)")
+        pairs = [(tokenizer, text_encoder), (tokenizer_2, text_encoder_2)]
+        if text_encoder is None:
+            pairs = pairs[1:]
+        self.tokenizers = [t for t, _ in pairs]
         self.text_encoders = [e if isinstance(e, ClipTextTower) else ClipTextTower.from_hf(e, device=device)
-                              for e in (text_encoder, text_encoder_2)]
+                              for _, e in pairs]
         self.device, self.dtype = device, dtype
 
     @classmethod
     def from_pretrained(cls, path: str, device="cuda", dtype=torch.float16) -> "ClipPromptEncoder":
-        """`path` = an SDXL snapshot folder with tokenizer/, tokenizer_2/, text_encoder/, text_encoder_2/."""
+        """`path` = an SDXL snapshot folder with tokenizer_2/ and text_encoder_2/, and tokenizer/ and text_encoder/
+        unless it is a single-tower model (the refiner)."""
         from transformers import CLIPTextModel, CLIPTextModelWithProjection, CLIPTokenizer
-        return cls(CLIPTokenizer.from_pretrained(os.path.join(path, "tokenizer")),
+        one = not cls._has(path, ("tokenizer", "text_encoder"))
+        return cls(None if one else CLIPTokenizer.from_pretrained(os.path.join(path, "tokenizer")),
                    CLIPTokenizer.from_pretrained(os.path.join(path, "tokenizer_2")),
-                   CLIPTextModel.from_pretrained(os.path.join(path, "text_encoder")),
+                   None if one else CLIPTextModel.from_pretrained(os.path.join(path, "text_encoder")),
                    CLIPTextModelWithProjection.from_pretrained(os.path.join(path, "text_encoder_2")), device, dtype)
 
     @staticmethod
+    def _has(path: str, dirs) -> bool:
+        return all(os.path.isdir(os.path.join(path, d)) for d in dirs)
+
+    @staticmethod
     def available(path: str) -> bool:
-        return all(os.path.isdir(os.path.join(path, d)) for d in ("tokenizer", "tokenizer_2", "text_encoder",
-                                                                    "text_encoder_2"))
+        return ClipPromptEncoder._has(path, ("tokenizer_2", "text_encoder_2"))
 
     @torch.no_grad()
     def __call__(self, prompts: List[str]) -> Tuple[torch.Tensor, torch.Tensor]:

@@ -70,6 +70,9 @@ def _repeat_for_samples(t: torch.Tensor, num_samples: int) -> torch.Tensor:
 class IPAdapter:
     def __init__(self, sd_pipe, image_encoder_path, ip_ckpt, device, num_tokens=4, target_blocks=None,
                  number_class_crossattention=None):
+        if sd_pipe.unet.config.num_ip_tokens == 0:
+            raise IHError("this UNet has no image-prompt layers (num_ip_tokens = 0, e.g. the SDXL refiner): the "
+                          "IMAGHarmony adapter is trained for the SDXL base UNet")
         self.device, self.num_tokens = device, num_tokens
         self.image_encoder_path, self.ip_ckpt = image_encoder_path, ip_ckpt
         self.pipe = sd_pipe.to(device)
