@@ -105,6 +105,10 @@ class StableDiffusionXLCustomPipeline:
         self.default_sample_size = unet.config.sample_size
         self._engine: Optional[DenoiseEngine] = None
         self.device = unet.conv_in.weight.device
+        self._lora = None                   # imagharmony_b200.lora.LoraWeights once a LoRA is loaded
+        self._lora_active: List[Tuple[str, float]] = []
+        self._lora_enabled = True
+        self._lora_fused: Optional[Dict[str, Dict[str, Tuple[float, float]]]] = None
 
     # ---- construction ------------------------------------------------------------------------------------------
     @classmethod
@@ -209,6 +213,152 @@ class StableDiffusionXLCustomPipeline:
             if isinstance(attn_processor, IPAttnProcessor):
                 attn_processor.scale = scale
 
+    # ---- LoRA ([3P] diffusers 0.30 StableDiffusionXLLoraLoaderMixin with the PEFT backend; SURVEY appendix A.8) --
+    # Adapters are merged into the canonical fp16 weights of the UNet and the text towers (imagharmony_b200.lora); a
+    # pipeline that never loads one runs exactly as without this surface.
+    def load_lora_weights(self, pretrained_model_name_or_path_or_dict, weight_name: Optional[str] = None,
+                          adapter_name: Optional[str] = None, subfolder: Optional[str] = None, **kwargs):
+        """Add a LoRA (a state dict, a .safetensors / .bin file, or a directory -- joined with `subfolder` when given --
+        holding `weight_name`) as adapter `adapter_name` (default `default_{i}`); it becomes the only active adapter,
+        at weight 1.0.  diffusers' other keywords (hub downloads, caching, loading options) are refused: files are read
+        from local paths only."""
+        from imagharmony_b200.lora import LoraWeights, prompt_towers, read_state_dict
+        if kwargs:
+            raise IHError(f"load_lora_weights: keyword arguments {sorted(kwargs)} are not supported (local files, "
+                          "weight_name, adapter_name and subfolder only)")
+        self._lora_require_unfused("load_lora_weights")
+        src = pretrained_model_name_or_path_or_dict
+        if subfolder:
+            if isinstance(src, dict):
+                raise IHError("load_lora_weights: `subfolder` needs a directory, not a state dict")
+            src = os.path.join(str(src), subfolder)
+        if self._lora is None:
+            self._lora = LoraWeights(self.unet, prompt_towers(self.prompt_encoder))
+        name = adapter_name or f"default_{len(self._lora.adapters)}"
+        if name in self._lora.adapters:
+            raise ValueError(f"Adapter name {name} already in use")
+        self._lora.add(name, read_state_dict(src, weight_name))
+        self._lora_active = [(name, 1.0)]
+        self._lora_sync()
+
+    def set_adapters(self, adapter_names, adapter_weights=None):
+        """Activate exactly `adapter_names` with `adapter_weights` (a number or one per adapter; default 1.0)."""
+        self._lora_require_unfused("set_adapters")
+        names = [adapter_names] if isinstance(adapter_names, str) else list(adapter_names)
+        self._lora_require_known(names)
+        weights = adapter_weights if adapter_weights is not None else 1.0
+        weights = list(weights) if isinstance(weights, (list, tuple)) else [weights] * len(names)
+        if len(weights) != len(names):
+            raise ValueError(f"Length of adapter names {len(names)} is not equal to the length of the weights "
+                             f"{len(weights)}")
+        self._lora_active = [(n, float(w)) for n, w in zip(names, weights)]
+        self._lora_sync()
+
+    def disable_lora(self):
+        """Run with the base weights until enable_lora()."""
+        self._lora_require_unfused("disable_lora")
+        self._lora_enabled = False
+        self._lora_sync()
+
+    def enable_lora(self):
+        self._lora_require_unfused("enable_lora")
+        self._lora_enabled = True
+        self._lora_sync()
+
+    def delete_adapters(self, adapter_names):
+        self._lora_require_unfused("delete_adapters")
+        names = [adapter_names] if isinstance(adapter_names, str) else list(adapter_names)
+        self._lora_require_known(names)
+        for n in names:
+            self._lora.remove(n)
+        self._lora_active = [(n, w) for n, w in self._lora_active if n not in names]
+        self._lora_sync()
+        self._lora.release()
+
+    def unload_lora_weights(self):
+        """Remove every adapter (fused ones included): each weight a LoRA touched is its original value again."""
+        if self._lora is None:
+            return
+        for n in list(self._lora.adapters):
+            self._lora.remove(n)
+        self._lora_active, self._lora_enabled, self._lora_fused = [], True, None
+        self._lora_sync()
+        self._lora.release()
+        self._lora = None
+
+    def get_active_adapters(self) -> List[str]:
+        return [n for n, _ in self._lora_active]
+
+    def get_list_adapters(self) -> Dict[str, List[str]]:
+        """{"unet": [...], "text_encoder": [...], "text_encoder_2": [...]}: the adapters each component holds."""
+        out: Dict[str, List[str]] = {}
+        for n in (self._lora.adapters if self._lora is not None else {}):
+            for comp in self._lora.components(n):
+                out.setdefault(comp, []).append(n)
+        return out
+
+    def fuse_lora(self, lora_scale: float = 1.0, fuse_unet: bool = True, fuse_text_encoder: bool = True):
+        """Bake the active adapters x `lora_scale` into the weights: until unfuse_lora(), per-call scales have no
+        effect and set_adapters raises.  Without a loaded adapter it does nothing; while LoRA is disabled it raises
+        (there is no active set to bake: enable_lora() first)."""
+        from imagharmony_b200.lora import TE1, TE2, UNET
+        self._lora_require_unfused("fuse_lora")
+        if self._lora is None or not self._lora.adapters:
+            return
+        if not self._lora_enabled:
+            raise IHError("fuse_lora: LoRA is disabled; call enable_lora() first")
+        comps = ([UNET] if fuse_unet else []) + ([TE1, TE2] if fuse_text_encoder else [])
+        if comps:
+            self._lora_fused = {c: {n: (float(lora_scale), w) for n, w in self._lora_active} for c in comps}
+            self._lora_sync()
+
+    def unfuse_lora(self, unfuse_unet: bool = True, unfuse_text_encoder: bool = True):
+        """Back to the state before fuse_lora() for the chosen components."""
+        from imagharmony_b200.lora import TE1, TE2, UNET
+        if self._lora_fused is None:
+            return
+        for c in ([UNET] if unfuse_unet else []) + ([TE1, TE2] if unfuse_text_encoder else []):
+            self._lora_fused.pop(c, None)
+        if not self._lora_fused:
+            self._lora_fused = None
+        self._lora_sync()
+
+    def _lora_require_unfused(self, what: str) -> None:
+        if self._lora_fused is not None:
+            raise IHError(f"{what}: the LoRA weights are fused; call unfuse_lora() first")
+
+    def _lora_require_known(self, names) -> None:
+        have = self._lora.adapters if self._lora is not None else {}
+        unknown = [n for n in names if n not in have]
+        if unknown:
+            raise ValueError(f"Adapter name(s) {unknown} not in the list of present adapters: {list(have)}")
+
+    def _lora_sync(self, components=None, scale: Optional[float] = None) -> None:
+        """Merge `components` (default: all) for the active set at the per-call `scale` (None = 1.0); fused components
+        keep their baked set."""
+        from imagharmony_b200.lora import COMPONENTS
+        if self._lora is None:
+            return
+        s = 1.0 if scale is None else float(scale)
+        for comp in components or COMPONENTS:
+            if self._lora_fused is not None and comp in self._lora_fused:
+                factors = self._lora_fused[comp]
+            elif not self._lora_enabled:
+                factors = {}
+            else:
+                factors = {n: (s, w) for n, w in self._lora_active}
+            self._lora.sync(comp, factors)
+
+    def _lora_call_scale(self, cross_attention_kwargs: Optional[Dict[str, Any]]) -> Optional[float]:
+        """diffusers' `cross_attention_kwargs={"scale": s}`: merges the UNet for s and returns s for encode_prompt's
+        lora_scale (None without a loaded LoRA or without a scale)."""
+        if self._lora is None:
+            return None
+        s = cross_attention_kwargs.get("scale") if cross_attention_kwargs else None
+        from imagharmony_b200.lora import UNET
+        self._lora_sync([UNET], s)
+        return s
+
     @property
     def engine(self) -> DenoiseEngine:
         if self._engine is None or self._engine.scheduler is not self.scheduler:
@@ -221,10 +371,12 @@ class StableDiffusionXLCustomPipeline:
                       do_classifier_free_guidance: bool = True, negative_prompt=None, negative_prompt_2=None,
                       prompt_embeds=None, negative_prompt_embeds=None, pooled_prompt_embeds=None,
                       negative_pooled_prompt_embeds=None, lora_scale=None, **kwargs):
-        """-> (prompt_embeds [n,77,2048], negative_prompt_embeds, pooled [n,1280], negative_pooled)  ([3P] A.4)."""
+        """-> (prompt_embeds [n,77,2048], negative_prompt_embeds, pooled [n,1280], negative_pooled)  ([3P] A.4).
+        With a loaded LoRA the text towers run with their deltas scaled by `lora_scale` (None = 1.0); they are merged
+        for that scale only when they run (embeddings passed in need no text tower)."""
         if prompt_embeds is None:
             prompts = [prompt] if isinstance(prompt, str) else list(prompt)
-            prompt_embeds, pooled_prompt_embeds = self.prompt_encoder(prompts)
+            prompt_embeds, pooled_prompt_embeds = self._encode_text(prompts, lora_scale)
             prompt_embeds = prompt_embeds.repeat_interleave(num_images_per_prompt, dim=0)
             pooled_prompt_embeds = pooled_prompt_embeds.repeat_interleave(num_images_per_prompt, dim=0)
         if do_classifier_free_guidance and negative_prompt_embeds is None and negative_prompt is None \
@@ -235,10 +387,16 @@ class StableDiffusionXLCustomPipeline:
         elif do_classifier_free_guidance and negative_prompt_embeds is None:
             negs = negative_prompt if negative_prompt is not None else ""
             negs = [negs] * (prompt_embeds.shape[0] // num_images_per_prompt) if isinstance(negs, str) else list(negs)
-            negative_prompt_embeds, negative_pooled_prompt_embeds = self.prompt_encoder(negs)
+            negative_prompt_embeds, negative_pooled_prompt_embeds = self._encode_text(negs, lora_scale)
             negative_prompt_embeds = negative_prompt_embeds.repeat_interleave(num_images_per_prompt, dim=0)
             negative_pooled_prompt_embeds = negative_pooled_prompt_embeds.repeat_interleave(num_images_per_prompt, dim=0)
         return prompt_embeds, negative_prompt_embeds, pooled_prompt_embeds, negative_pooled_prompt_embeds
+
+    def _encode_text(self, prompts, lora_scale):
+        if self._lora is not None:
+            from imagharmony_b200.lora import TE1, TE2
+            self._lora_sync([TE1, TE2], lora_scale)
+        return self.prompt_encoder(prompts)
 
     def prepare_latents(self, batch_size, num_channels_latents, height, width, dtype, device, generator, latents=None):
         """[3P] diffusers prepare_latents: randn * init_noise_sigma; a list of generators draws one sample each."""
@@ -278,7 +436,8 @@ class StableDiffusionXLCustomPipeline:
         do_classifier_free_guidance = guidance_scale > 1.0                            # :223
         embeds = self.encode_prompt(prompt, prompt_2, None, num_images_per_prompt, do_classifier_free_guidance,
                                     negative_prompt, negative_prompt_2, prompt_embeds, negative_prompt_embeds,
-                                    pooled_prompt_embeds, negative_pooled_prompt_embeds)  # :229-247
+                                    pooled_prompt_embeds, negative_pooled_prompt_embeds,
+                                    lora_scale=self._lora_call_scale(cross_attention_kwargs))  # :229-247
         self.scheduler.set_timesteps(num_inference_steps)                             # :250
         lat = self.prepare_latents(embeds[0].shape[0], self.unet.config.in_channels, height, width, torch.float16,
                                    self.device, generator, latents)                  # :255-265
@@ -572,7 +731,8 @@ class StableDiffusionXLImg2ImgPipeline(StableDiffusionXLCustomPipeline):
         do_classifier_free_guidance = guidance_scale > 1.0
         embeds = self.encode_prompt(prompt, prompt_2, None, num_images_per_prompt, do_classifier_free_guidance,
                                     negative_prompt, negative_prompt_2, prompt_embeds, negative_prompt_embeds,
-                                    pooled_prompt_embeds, negative_pooled_prompt_embeds)
+                                    pooled_prompt_embeds, negative_pooled_prompt_embeds,
+                                    lora_scale=self._lora_call_scale(cross_attention_kwargs))
         self.scheduler.set_timesteps(num_inference_steps)
         if handoff:
             t_start = denoising_start_begin_step(self.scheduler.timesteps, self.scheduler.num_train_timesteps, start)
@@ -721,7 +881,8 @@ class StableDiffusionXLInpaintPipeline(StableDiffusionXLImg2ImgPipeline):
         do_classifier_free_guidance = guidance_scale > 1.0
         embeds = self.encode_prompt(prompt, prompt_2, None, num_images_per_prompt, do_classifier_free_guidance,
                                     negative_prompt, negative_prompt_2, prompt_embeds, negative_prompt_embeds,
-                                    pooled_prompt_embeds, negative_pooled_prompt_embeds)
+                                    pooled_prompt_embeds, negative_pooled_prompt_embeds,
+                                    lora_scale=self._lora_call_scale(cross_attention_kwargs))
         batch = embeds[0].shape[0]
         self.scheduler.set_timesteps(num_inference_steps)
         sizes = (original_size or (height, width), crops_coords_top_left, target_size or (height, width),
@@ -961,7 +1122,8 @@ class StableDiffusionXLControlNetPipeline(StableDiffusionXLCustomPipeline):
         do_classifier_free_guidance = guidance_scale > 1.0
         embeds = self.encode_prompt(prompt, prompt_2, None, num_images_per_prompt, do_classifier_free_guidance,
                                     negative_prompt, negative_prompt_2, prompt_embeds, negative_prompt_embeds,
-                                    pooled_prompt_embeds, negative_pooled_prompt_embeds)
+                                    pooled_prompt_embeds, negative_pooled_prompt_embeds,
+                                    lora_scale=self._lora_call_scale(cross_attention_kwargs))
         batch = embeds[0].shape[0]
         # [3P] prepare_image, per net: repeat_interleave by the batch (one image) or by num_images_per_prompt; the CFG
         # copy is the engine's (the embedding is computed once and duplicated)
