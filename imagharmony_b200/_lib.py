@@ -84,7 +84,7 @@ SIGNATURES = {
     "ih_gemm_scaled_f16": (c_int, [c_void_p, c_longlong, c_void_p, c_void_p, c_void_p, c_longlong, c_void_p, c_longlong,
                                    c_int, c_int, c_int, c_int, c_float, c_void_p]),
     "ih_conv2d_scaled_f16": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int,
-                                     c_int, c_float, c_void_p]),
+                                     c_int, c_float, c_void_p, c_int]),
     "ih_conv2d_shortcut_f16": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_longlong, c_void_p, c_int, c_void_p, c_int,
                                        c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p]),
     "ih_conv2d_down_f16": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int,

@@ -256,3 +256,17 @@ SDXL_VAE = VAEConfig()
 # miniature with the same block structure (mid attention, a channel-changing shortcut); channels stay multiples of 64
 # because the implicit-GEMM conv kernel needs Cin % 64 == 0
 TINY_VAE = VAEConfig(block_out_channels=(64, 64, 128, 128), layers_per_block=1, norm_num_groups=8, sample_size=64)
+
+
+@dataclass(frozen=True)
+class TinyVAEConfig:
+    """[3P] diffusers AutoencoderTiny (decoder half) with the defaults of the published TAESD-XL config.json
+    (madebyollin/taesdxl): ReLU, nearest 2x upsampling, 64 channels throughout, blocks (3, 3, 3, 1)."""
+    latent_channels: int = 4
+    out_channels: int = 3
+    decoder_block_out_channels: Tuple[int, ...] = (64, 64, 64, 64)
+    num_decoder_blocks: Tuple[int, ...] = (3, 3, 3, 1)
+    scaling_factor: float = 1.0
+
+
+TAESDXL = TinyVAEConfig()

@@ -59,6 +59,7 @@ struct GemmParams {
   __half* out;
   long long ldo;
   int act;  // 0 none, 1 SiLU, 2 GELU(erf), 3 quick-GELU (applied after bias, before residual)
+  int relu;  // IH_EPI_RELU: max(x, 0) AFTER the residual add (TAESD's fuse(conv(x) + skip(x)))
   unsigned long long* trace;  // optional: %globaltimer stamps of CTA 0 (ih_gemm_set_trace), nullptr in production
   // L2 prefetch of the NEXT kernel's weights (ih_gemm_prefetch_next): inside a denoise step every GEMM streams its weights
   // from HBM (5.2 GB per step >> L2), and a short launch cannot hide the first HBM round trips.  An otherwise idle
@@ -407,6 +408,10 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_f16_kernel(const __grid_
                 x0v += f.x;
                 x1v += f.y;
               }
+              if (p.relu) {
+                x0v = fmaxf(x0v, 0.f);
+                x1v = fmaxf(x1v, 0.f);
+              }
               *slot = pack_half2(x0v, x1v);
             }
           }
@@ -659,6 +664,8 @@ static int gemm_impl(const void* a, long long lda, const void* w, const void* bi
   const bool geglu = (epilogue & IH_EPI_GEGLU) != 0;
   IH_CHECK(!geglu || (N % 16 == 0), IH_ERR_SHAPE, "ih_gemm_f16: GEGLU needs even split of N");
   IH_CHECK(!(residual) || ldr % 8 == 0, IH_ERR_ALIGN, "ih_gemm_f16: ldr must be a multiple of 8");
+  IH_CHECK(!(epilogue & IH_EPI_RELU) || epilogue == IH_EPI_RELU, IH_ERR_ARG,
+           "ih_gemm_f16: IH_EPI_RELU cannot be combined with other epilogue flags");
   IH_CHECK(!rowbias || (rows_per_group > 0 && ld_rowbias % 8 == 0), IH_ERR_ARG,
            "ih_gemm_f16: rowbias needs rows_per_group > 0 and ld_rowbias %% 8 == 0");
 
@@ -685,6 +692,7 @@ static int gemm_impl(const void* a, long long lda, const void* w, const void* bi
   p.out = (__half*)out;
   p.ldo = ldo;
   p.act = (epilogue & IH_EPI_SILU) ? 1 : ((epilogue & IH_EPI_GELU) ? 2 : ((epilogue & IH_EPI_QUICK_GELU) ? 3 : 0));
+  p.relu = epilogue == IH_EPI_RELU;
   p.trace = g_trace;
   p.pf_ptr = hint.ptr;
   p.pf_bytes = hint.bytes;
@@ -705,7 +713,8 @@ static int gemm_impl(const void* a, long long lda, const void* w, const void* bi
 static int conv_impl(const void* x, const void* w, const void* bias, const void* rowbias, long long ld_rowbias,
                      const void* residual, void* out, int B, int Hin, int Win, int Cin, int Cout, int ksize, int stride,
                      int tile_n, float alpha, void* stream, const void* sc0 = nullptr, int Csc0 = 0,
-                     const void* sc1 = nullptr, int Csc1 = 0, bool pad_bottom_right = false);
+                     const void* sc1 = nullptr, int Csc1 = 0, bool pad_bottom_right = false,
+                     int epilogue = IH_EPI_NONE);
 
 extern "C" int ih_conv2d_f16(const void* x, const void* w, const void* bias, const void* rowbias,
                              long long ld_rowbias, const void* residual, void* out, int B, int Hin, int Win, int Cin,
@@ -715,8 +724,10 @@ extern "C" int ih_conv2d_f16(const void* x, const void* w, const void* bias, con
 }
 
 extern "C" int ih_conv2d_scaled_f16(const void* x, const void* w, const void* bias, const void* residual, void* out,
-                                    int B, int Hin, int Win, int Cin, int Cout, int stride, float alpha, void* stream) {
-  return conv_impl(x, w, bias, nullptr, 0, residual, out, B, Hin, Win, Cin, Cout, 3, stride, 0, alpha, stream);
+                                    int B, int Hin, int Win, int Cin, int Cout, int stride, float alpha, void* stream,
+                                    int epilogue) {
+  return conv_impl(x, w, bias, nullptr, 0, residual, out, B, Hin, Win, Cin, Cout, 3, stride, 0, alpha, stream, nullptr, 0,
+                   nullptr, 0, false, epilogue);
 }
 
 extern "C" int ih_conv2d_shortcut_f16(const void* x, const void* w, const void* bias, const void* rowbias,
@@ -737,9 +748,11 @@ extern "C" int ih_conv2d_down_f16(const void* x, const void* w, const void* bias
 static int conv_impl(const void* x, const void* w, const void* bias, const void* rowbias, long long ld_rowbias,
                      const void* residual, void* out, int B, int Hin, int Win, int Cin, int Cout, int ksize, int stride,
                      int tile_n, float alpha, void* stream, const void* sc0, int Csc0, const void* sc1, int Csc1,
-                     bool pad_bottom_right) {
+                     bool pad_bottom_right, int epilogue) {
   const PrefetchHint hint = take_prefetch_hint();
   IH_CHECK(x && w && out, IH_ERR_ARG, "ih_conv2d_f16: null pointer");
+  IH_CHECK(epilogue == IH_EPI_NONE || epilogue == IH_EPI_RELU, IH_ERR_ARG,
+           "ih_conv2d_scaled_f16: epilogue must be IH_EPI_NONE or IH_EPI_RELU (got %d)", epilogue);
   IH_CHECK(ksize == 3, IH_ERR_ARG, "ih_conv2d_f16: ksize must be 3 (1x1 convs are ih_gemm_f16)");
   IH_CHECK(stride == 1 || stride == 2, IH_ERR_ARG, "ih_conv2d_f16: stride must be 1 or 2");
   IH_CHECK(Cin % 8 == 0 && Cout % 8 == 0, IH_ERR_ALIGN, "ih_conv2d_f16: channels must be multiples of 8");
@@ -792,6 +805,7 @@ static int conv_impl(const void* x, const void* w, const void* bias, const void*
   p.pf_ptr = hint.ptr;
   p.pf_bytes = hint.bytes;
   p.alpha = alpha;
+  p.relu = epilogue == IH_EPI_RELU;
 
   TmapSet4 amaps;
   const uint32_t abox[4] = {(uint32_t)BK, (uint32_t)p.bw, (uint32_t)p.bh, 1u};

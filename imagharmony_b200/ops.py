@@ -13,7 +13,7 @@ import torch
 from . import _lib
 from ._lib import IHError, check
 
-EPI_NONE, EPI_GEGLU, EPI_SILU, EPI_GELU, EPI_QUICK_GELU = 0, 1, 2, 4, 8
+EPI_NONE, EPI_GEGLU, EPI_SILU, EPI_GELU, EPI_QUICK_GELU, EPI_RELU = 0, 1, 2, 4, 8, 16
 
 
 def _stream() -> int:
@@ -51,8 +51,11 @@ def linear(x: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor] = None
            residual: Optional[torch.Tensor] = None, rowbias: Optional[torch.Tensor] = None,
            rows_per_group: int = 0, geglu: bool = False, silu: bool = False, gelu: bool = False,
            out: Optional[torch.Tensor] = None, tile_n: int = 0, ln=None,
-           stats_out: Optional[torch.Tensor] = None, quick_gelu: bool = False, alpha: float = 1.0) -> torch.Tensor:
+           stats_out: Optional[torch.Tensor] = None, quick_gelu: bool = False, alpha: float = 1.0,
+           relu: bool = False) -> torch.Tensor:
     """out = epi(x @ w.T + bias + rowbias[row // rows_per_group]) + residual ; x [M,K], w [N,K] (nn.Linear layout).
+    `relu=True`: out = relu(alpha * x @ w.T + bias + residual), the ReLU after the residual (IH_EPI_RELU); it takes no
+    other activation, rowbias, ln, stats_out or tile_n.
 
     LayerNorm folding: `stats_out` (float32 [ceil(N/64), M, 2]) receives per-row (sum, sumsq) of the stored values as
     partial sums whose total over slots is the row's; `ln=(stats, eps)` makes this GEMM consume RAW rows `x` with the gamma-scaled, row-centred weight and
@@ -70,10 +73,15 @@ def linear(x: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor] = None
     ldrb = _rows(rowbias, "rowbias") if rowbias is not None else 0
     epi = ((EPI_GEGLU if geglu else 0) | (EPI_SILU if silu else 0) | (EPI_GELU if gelu else 0)
            | (EPI_QUICK_GELU if quick_gelu else 0))
-    if alpha != 1.0:
-        # out = epi(alpha * x w^T + bias) + residual (ih_gemm_scaled_f16: the VAE decoder's scaled residual stream)
+    if relu:
+        if epi:
+            raise IHError("linear: relu cannot be combined with geglu / silu / gelu / quick_gelu")
+        epi = EPI_RELU
+    if alpha != 1.0 or relu:
+        # out = epi(alpha * x w^T + bias) + residual (ih_gemm_scaled_f16: the VAE decoder's scaled residual stream), or
+        # relu(alpha * x w^T + bias + residual)
         if ln is not None or stats_out is not None or rowbias is not None or tile_n:
-            raise IHError("linear: alpha != 1 cannot be combined with ln / stats_out / rowbias / tile_n")
+            raise IHError("linear: alpha != 1 / relu cannot be combined with ln / stats_out / rowbias / tile_n")
         rc = lib.ih_gemm_scaled_f16(x.data_ptr(), _rows(x, "x"), w.data_ptr(), _p(bias), _p(residual), ldr, out.data_ptr(),
                                     _rows(out, "out"), M, N, K, epi, float(alpha), _stream())
         check(rc, "ih_gemm_scaled_f16")
@@ -157,8 +165,10 @@ def fold_layernorm(w: torch.Tensor, bias: Optional[torch.Tensor], gamma: torch.T
 
 def conv3x3(x: torch.Tensor, w_packed: torch.Tensor, bias: Optional[torch.Tensor] = None, *,
             rowbias: Optional[torch.Tensor] = None, residual: Optional[torch.Tensor] = None, stride: int = 1,
-            out: Optional[torch.Tensor] = None, tile_n: int = 0, alpha: float = 1.0, shortcut=None) -> torch.Tensor:
+            out: Optional[torch.Tensor] = None, tile_n: int = 0, alpha: float = 1.0, shortcut=None,
+            relu: bool = False) -> torch.Tensor:
     """3x3 conv, pad 1. x NHWC [B,H,W,Cin]; w_packed [Cout, 9*Cin] (see pack_conv3x3_weight); rowbias [B, >=Cout].
+    `relu=True`: out = relu(alpha * conv(x) + bias + residual), the ReLU after the residual (IH_EPI_RELU).
     `shortcut=(s0, s1 | None)`: fused 1x1 shortcut conv over the channel concat of the NHWC tensors s0 [, s1]; then
     w_packed is [Cout, 9*Cin + C(s0) + C(s1)] (3x3 taps followed by the shortcut weight), see ih_conv2d_shortcut_f16."""
     lib = _lib.load()
@@ -171,11 +181,12 @@ def conv3x3(x: torch.Tensor, w_packed: torch.Tensor, bias: Optional[torch.Tensor
         _req(s0, "shortcut[0]")
         if s1 is not None:
             _req(s1, "shortcut[1]")
-        if (stride != 1 or residual is not None or alpha != 1.0 or tile_n or not x.is_contiguous() or not s0.is_contiguous()
+        if (stride != 1 or residual is not None or alpha != 1.0 or relu or tile_n or not x.is_contiguous()
+                or not s0.is_contiguous()
                 or (s1 is not None and not s1.is_contiguous()) or tuple(s0.shape[:3]) != (B, H, W)
                 or (s1 is not None and tuple(s1.shape[:3]) != (B, H, W)) or not w_packed.is_contiguous()
                 or w_packed.shape[1] != 9 * Cin + c0 + c1):
-            raise IHError("conv3x3(shortcut=): stride 1, no residual / alpha / tile_n, contiguous NHWC sources of the same "
+            raise IHError("conv3x3(shortcut=): stride 1, no residual / alpha / relu / tile_n, contiguous NHWC sources of the same "
                           "spatial size and w_packed [Cout, 9*Cin + C0 + C1] required")
         if out is None:
             out = torch.empty((B, H, W, Cout), dtype=torch.float16, device=x.device)
@@ -192,11 +203,11 @@ def conv3x3(x: torch.Tensor, w_packed: torch.Tensor, bias: Optional[torch.Tensor
     ldrb = _rows(rowbias, "rowbias") if rowbias is not None else 0
     if residual is not None and (not residual.is_contiguous() or residual.shape != out.shape):
         raise IHError("conv3x3: residual must be contiguous and shaped like the output")
-    if alpha != 1.0:
+    if alpha != 1.0 or relu:
         if rowbias is not None or tile_n:
-            raise IHError("conv3x3: alpha != 1 cannot be combined with rowbias / tile_n")
+            raise IHError("conv3x3: alpha != 1 / relu cannot be combined with rowbias / tile_n")
         rc = lib.ih_conv2d_scaled_f16(x.data_ptr(), w_packed.data_ptr(), _p(bias), _p(residual), out.data_ptr(), B, H, W,
-                                      Cin, Cout, stride, float(alpha), _stream())
+                                      Cin, Cout, stride, float(alpha), _stream(), EPI_RELU if relu else EPI_NONE)
         check(rc, "ih_conv2d_scaled_f16")
         return out
     rc = lib.ih_conv2d_f16(x.data_ptr(), w_packed.data_ptr(), _p(bias), _p(rowbias), ldrb, _p(residual),

@@ -26,6 +26,10 @@ extern "C" {
 #define IH_EPI_SILU 2  /* out = silu(acc + bias) */
 #define IH_EPI_GELU 4  /* out = gelu_erf(acc + bias) */
 #define IH_EPI_QUICK_GELU 8 /* out = x * sigmoid(1.702 x), x = acc + bias  (CLIP-L text tower MLP, scope row f2) */
+/* out = relu(alpha * acc + bias + residual).  Unlike SILU / GELU / QUICK_GELU, which act on acc + bias BEFORE the
+ * residual is added, ReLU acts AFTER it: the tiny autoencoder's block output relu(conv(x) + x) is one launch.  Not
+ * combinable with the other flags; ih_conv2d_scaled_f16 accepts it too. */
+#define IH_EPI_RELU 16
 
 const char* ih_last_error(void);
 int ih_version(void);
@@ -88,9 +92,10 @@ int ih_conv2d_f16(const void* x, const void* w, const void* bias, const void* ro
 int ih_conv2d_shortcut_f16(const void* x, const void* w, const void* bias, const void* rowbias, long long ld_rowbias,
                            const void* sc0, int Csc0, const void* sc1, int Csc1, void* out, int B, int H, int W, int Cin,
                            int Cout, void* stream);
-/* out = alpha * conv(x) + bias + residual (3x3, pad 1): the VAE decoder's scaled residual stream, see ih_gemm_scaled_f16. */
+/* out = alpha * conv(x) + bias + residual (3x3, pad 1): the VAE decoder's scaled residual stream, see ih_gemm_scaled_f16.
+ * epilogue: IH_EPI_NONE, or IH_EPI_RELU for relu(alpha * conv(x) + bias + residual) (the tiny autoencoder's convs). */
 int ih_conv2d_scaled_f16(const void* x, const void* w, const void* bias, const void* residual, void* out, int B, int Hin,
-                         int Win, int Cin, int Cout, int stride, float alpha, void* stream);
+                         int Win, int Cin, int Cout, int stride, float alpha, void* stream, int epilogue);
 
 /* out = alpha * conv(x) + bias: 3x3 conv, stride 2, padded by one zero row / column at the BOTTOM and RIGHT only
  * (Ho = Hin / 2, Wo = Win / 2; Hin, Win even).  Replaces [3P] diffusers Downsample2D(padding=0) of the VAE encoder

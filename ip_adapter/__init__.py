@@ -2,7 +2,7 @@
 (IPAdapter.generate, IPAdapterPlus, IPAdapterFull) are outside the SDXL hot path and are not provided."""
 from .custom_pipelines import (StableDiffusionXLCustomPipeline, StableDiffusionXLImg2ImgPipeline,
                                StableDiffusionXLInpaintPipeline)
-from .ip_adapter import IPAdapter, IPAdapterPlusXL, IPAdapterXL, MultiControlNetModel
+from .ip_adapter import AutoencoderTiny, IPAdapter, IPAdapterPlusXL, IPAdapterXL, MultiControlNetModel
 
-__all__ = ["IPAdapter", "IPAdapterPlusXL", "IPAdapterXL", "MultiControlNetModel", "StableDiffusionXLCustomPipeline",
+__all__ = ["AutoencoderTiny", "IPAdapter", "IPAdapterPlusXL", "IPAdapterXL", "MultiControlNetModel", "StableDiffusionXLCustomPipeline",
            "StableDiffusionXLImg2ImgPipeline", "StableDiffusionXLInpaintPipeline"]

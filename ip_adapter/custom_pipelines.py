@@ -13,7 +13,8 @@ inpainting run Euler Ancestral (`EulerAncestralDiscreteScheduler.from_config(pip
 noise comes from the call's `generator` in diffusers' order.
 VAE decode / PIL post-processing (:365-386, scope row f1) runs on the native decoder `imagharmony_b200.vae` when the
 pipeline owns one (`from_random`, or `from_pretrained` with a `vae/` folder); a `vae_decode` callable overrides it and
-`output_type="latent"` skips it.
+`output_type="latent"` skips it.  `pipe.vae = AutoencoderTiny.from_pretrained(dir)` swaps in the native tiny decoder
+(imagharmony_b200.taesd, TAESD-XL); image-to-image and inpainting then refuse to encode a pixel image.
 """
 from __future__ import annotations
 
@@ -98,7 +99,7 @@ class StableDiffusionXLCustomPipeline:
                           f"micro-conditioning ids; this one has {unet.config.num_time_ids} (a UNet that requires an "
                           "aesthetics score, the SDXL refiner, runs in StableDiffusionXLImg2ImgPipeline)")
         self.unet = unet
-        self.vae = vae                      # imagharmony_b200.vae.AutoencoderKLDecoder or None
+        self.vae = vae                      # imagharmony_b200.vae.AutoencoderKLDecoder, taesd.AutoencoderTiny or None
         self.scheduler = scheduler or EulerDiscreteScheduler()
         self.prompt_encoder = prompt_encoder or SyntheticPromptEncoder(unet.config)
         self.vae_decode = vae_decode
@@ -720,6 +721,7 @@ class StableDiffusionXLImg2ImgPipeline(StableDiffusionXLCustomPipeline):
         if handoff:
             height, width = image.shape[2] * self.vae_scale_factor, image.shape[3] * self.vae_scale_factor
         else:
+            self._refuse_tiny_vae_encode()
             if self.vae_encoder is None:
                 raise IHError("this pipeline has no VAE encoder: build it with from_random(vae_cfg=...) or "
                               "from_pretrained with a vae/ folder")
@@ -747,6 +749,16 @@ class StableDiffusionXLImg2ImgPipeline(StableDiffusionXLCustomPipeline):
                                  guidance_rescale, control_guidance_start, control_guidance_end, callback, callback_steps,
                                  generator=generator, aesthetic=aesthetic)
         return self._output(out, output_type, return_dict)
+
+    def _refuse_tiny_vae_encode(self) -> None:
+        """With a tiny autoencoder as `pipe.vae` diffusers encodes a pixel image with the tiny encoder, which is not built
+        here; encoding with the KL encoder instead would silently give other latents.  Latent hand-overs
+        (`denoising_start`) encode nothing and run."""
+        from imagharmony_b200.taesd import AutoencoderTinyDecoder
+        if isinstance(self.vae, AutoencoderTinyDecoder):
+            raise IHError(f"{type(self).__name__}: encoding a pixel image with a tiny autoencoder (AutoencoderTiny) as "
+                          "pipe.vae is not implemented; keep the KL VAE for this call, or pass latents with "
+                          "denoising_start")
 
     def _require_euler(self) -> None:
         """Image-to-image and inpainting noise the image latents with Euler's add_noise (x + sigma * noise) inside the
@@ -873,6 +885,7 @@ class StableDiffusionXLInpaintPipeline(StableDiffusionXLImg2ImgPipeline):
         self._check_callback_steps(callback, callback_steps)
         if image is None or mask_image is None:
             raise ValueError("`image` and `mask_image` inputs cannot be undefined")
+        self._refuse_tiny_vae_encode()
         if self.vae_encoder is None:
             raise IHError("this pipeline has no VAE encoder: build it with from_random(vae_cfg=...) or from_pretrained "
                           "with a vae/ folder")

@@ -21,6 +21,7 @@ from PIL import Image
 from imagharmony_b200._lib import IHError
 from imagharmony_b200.adapter import HarmonyAttention, ImageProjModel, Resampler  # noqa: F401
 from imagharmony_b200.controlnet import MultiControlNetModel
+from imagharmony_b200.taesd import AutoencoderTiny  # noqa: F401  (re-exported: pipe.vae = AutoencoderTiny.from_pretrained)
 
 from .utils import get_generator, is_torch2_available
 
