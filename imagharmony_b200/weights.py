@@ -3,7 +3,8 @@
 `random_state_dict` fills a {key: shape} description with fp16 values drawn from one seeded generator in key order:
 matrices/convs ~ U(-1/sqrt(fan_in), 1/sqrt(fan_in)) (PyTorch's default Linear/Conv bound), biases likewise, norm
 weights 1 + 0.1 N(0,1), norm biases 0.1 N(0,1) so the affine paths are exercised.  The oracle loads the same dict
-cast to fp32, so both sides see bit-identical (fp16-representable) parameters.
+cast to fp32, so both sides see bit-identical (fp16-representable) parameters.  `random_module` builds a native model
+from such a dict.
 
 `split_ip_adapter_checkpoint` / `join_ip_adapter_checkpoint` mirror the 3-key layout written by the reference's
 convert_bin.py:21-40 ({"image_proj", "ip_adapter", "composed_adapter"}) that ip_adapter.py:149-154 loads.
@@ -49,6 +50,15 @@ def random_state_dict(shapes: Mapping[str, Iterable[int]], seed: int = 0, device
             t = (torch.rand(shape, generator=g, device=device, dtype=torch.float32) * 2.0 - 1.0) * bound
         out[key] = t.to(dtype)
     return out
+
+
+def random_module(cls, cfg, seed: int, device="cuda"):
+    """`cls.from_state_dict(cfg, ...)` with random_state_dict(seed) weights for the shapes of `cls(cfg)` (built on the
+    meta device), drawn on `device` when it is a CUDA device and on the CPU otherwise."""
+    with torch.device("meta"):
+        shapes = shapes_of(cls(cfg))
+    gen_dev = device if str(device).startswith("cuda") else "cpu"
+    return cls.from_state_dict(cfg, random_state_dict(shapes, seed, device=gen_dev), device=device)
 
 
 def split_ip_adapter_checkpoint(full: Mapping[str, torch.Tensor]) -> Dict[str, Dict[str, torch.Tensor]]:

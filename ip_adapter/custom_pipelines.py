@@ -18,6 +18,7 @@ pipeline owns one (`from_random`, or `from_pretrained` with a `vae/` folder); a 
 """
 from __future__ import annotations
 
+import dataclasses
 import hashlib
 import json
 import os
@@ -33,6 +34,7 @@ from imagharmony_b200.denoise import DenoiseEngine
 from imagharmony_b200.scheduler import (DPMSolverMultistepScheduler, EulerAncestralDiscreteScheduler,
                                         EulerDiscreteScheduler, randn_tensor)
 from imagharmony_b200.unet import UNet2DConditionModel, require_latent_size
+from imagharmony_b200.weights import random_module
 
 from .utils import is_torch2_available
 
@@ -69,12 +71,17 @@ def _fraction(value) -> bool:
     return isinstance(value, float) and 0 < value < 1
 
 
+def _denoising_cutoff(num_train_timesteps: int, fraction: float) -> int:
+    """[3P] The timestep that a valid denoising_start / denoising_end splits the schedule at."""
+    return int(round(num_train_timesteps - fraction * num_train_timesteps))
+
+
 def denoising_start_begin_step(timesteps, num_train_timesteps: int, denoising_start: float) -> int:
     """[3P] StableDiffusionXLImg2ImgPipeline.get_timesteps with a valid `denoising_start` (first-order schedulers): the
-    loop runs the n timesteps below int(round(N - denoising_start * N)), the last n of the schedule, so it begins at
+    loop runs the n timesteps below the cutoff (_denoising_cutoff), the last n of the schedule, so it begins at
     index len(timesteps) - n.  A base run with denoising_end = denoising_start keeps the timesteps at or above the same
     cutoff, so it ends at that same index: the handoff repeats and skips no step."""
-    cutoff = int(round(num_train_timesteps - denoising_start * num_train_timesteps))
+    cutoff = _denoising_cutoff(num_train_timesteps, denoising_start)
     return len(timesteps) - int(sum(1 for t in timesteps if t < cutoff))
 
 
@@ -84,6 +91,57 @@ def _read_json(path: str, *parts: str) -> dict:
         return {}
     with open(f) as fh:
         return json.load(fh)
+
+
+@dataclass
+class _Pretrained:
+    """The parts of an SDXL folder that from_pretrained builds a pipeline from."""
+    unet: UNet2DConditionModel
+    prompt_encoder: Optional[Callable]      # ClipPromptEncoder, None without text encoders on disk
+    vae: Any                                # AutoencoderKLDecoder, None without a vae/ folder
+    vae_state: Optional[Dict[str, torch.Tensor]]
+    vae_config: Any
+    index: dict                             # model_index.json, {} without one
+
+
+def _pil_list(image) -> Optional[list]:
+    """A PIL image or a non-empty list / tuple of them as a list; None for anything else."""
+    from PIL import Image
+    if isinstance(image, Image.Image):
+        return [image]
+    if isinstance(image, (list, tuple)) and image and isinstance(image[0], Image.Image):
+        return list(image)
+    return None
+
+
+def _load_images(image, size: Callable[[int, int], Tuple[int, int]], what: str, vae_scale_factor: int) -> torch.Tensor:
+    """PIL image(s) -> RGB, Lanczos resize, / 255; a [B, 3, H, W] / [3, H, W] tensor -> float, nearest resize; both to
+    the (height, width) that `size` gives for the first image's (H, W).  -> float32 [B, 3, height, width], PIL images
+    in [0, 1], a tensor in its own range.  `what` names the image in the error messages."""
+    import numpy as np
+    from PIL import Image
+    images = _pil_list(image)
+    if images is not None:
+        w0, h0 = images[0].size
+        h, w = size(h0, w0)
+        if h <= 0 or w <= 0:
+            raise ValueError(f"{what} of size {images[0].size} is smaller than {vae_scale_factor} pixels")
+        images = [im.convert("RGB") if im.mode != "RGB" else im for im in images]
+        images = [im if im.size == (w, h) else im.resize((w, h), resample=Image.LANCZOS) for im in images]
+        arr = np.stack([np.array(im).astype(np.float32) / 255.0 for im in images])
+        return torch.from_numpy(arr).permute(0, 3, 1, 2).contiguous()
+    if isinstance(image, torch.Tensor):
+        x = image.unsqueeze(0) if image.dim() == 3 else image
+        if x.dim() != 4 or x.shape[1] != 3:
+            raise ValueError(f"{what} tensor must be [B, 3, H, W] or [3, H, W], got {tuple(image.shape)}")
+        x = x.float()
+        h, w = size(x.shape[2], x.shape[3])
+        if h <= 0 or w <= 0:
+            raise ValueError(f"{what} of size {tuple(x.shape[2:])} is smaller than {vae_scale_factor} pixels")
+        if (h, w) != tuple(x.shape[2:]):
+            x = torch.nn.functional.interpolate(x, size=(h, w))
+        return x.contiguous()
+    raise ValueError(f"`image` must be a PIL image, a list of them or a tensor, got {type(image).__name__}")
 
 
 class StableDiffusionXLCustomPipeline:
@@ -115,18 +173,9 @@ class StableDiffusionXLCustomPipeline:
     @classmethod
     def from_random(cls, cfg: UNetConfig = SDXL_BASE, seed: int = 0, device="cuda", vae_cfg=None):
         """Random-init weights of the given architecture (the benchmark / test configuration)."""
-        from imagharmony_b200.weights import random_state_dict, shapes_of
-        with torch.device("meta"):
-            shapes = shapes_of(UNet2DConditionModel(cfg))
-        gen_dev = device if str(device).startswith("cuda") else "cpu"
-        unet = UNet2DConditionModel.from_state_dict(cfg, random_state_dict(shapes, seed, device=gen_dev), device=device)
-        vae = None
-        if vae_cfg is not None:
-            from imagharmony_b200.vae import AutoencoderKLDecoder
-            with torch.device("meta"):
-                vshapes = shapes_of(AutoencoderKLDecoder(vae_cfg))
-            vae = AutoencoderKLDecoder.from_state_dict(vae_cfg, random_state_dict(vshapes, seed + 17, device=gen_dev),
-                                                       device=device)
+        from imagharmony_b200.vae import AutoencoderKLDecoder
+        unet = random_module(UNet2DConditionModel, cfg, seed, device)
+        vae = None if vae_cfg is None else random_module(AutoencoderKLDecoder, vae_cfg, seed + 17, device)
         return cls(unet, vae=vae)
 
     @classmethod
@@ -135,9 +184,15 @@ class StableDiffusionXLCustomPipeline:
         """test.py:68-72.  Loads `<path>/unet/diffusion_pytorch_model.safetensors` (diffusers key names are the native
         UNet's key names, so no key map is needed).  Without `cfg` the UNet's architecture comes from
         `<path>/unet/config.json` when there is one (see _load_pretrained), else it is SDXL-base with the input channel
-        count of the checkpoint's conv_in (4, or 9 for the inpainting UNet)."""
-        unet, enc, vae, _, _, index = cls._load_pretrained(path, torch_dtype, device, cfg, vae_cfg)
-        return cls(unet, prompt_encoder=enc, vae=vae)._configure(index)
+        count of the checkpoint's conv_in (4, or 9 for the inpainting UNet).  Keywords a subclass needs (the ControlNet
+        pipeline's `controlnet`) reach its _from_parts; others are ignored."""
+        parts = cls._load_pretrained(path, torch_dtype, device, cfg, vae_cfg)
+        return cls._from_parts(parts, device, **kwargs)._configure(parts.index)
+
+    @classmethod
+    def _from_parts(cls, parts: _Pretrained, device, **kwargs):
+        """The pipeline of this class over the loaded parts."""
+        return cls(parts.unet, prompt_encoder=parts.prompt_encoder, vae=parts.vae)
 
     def _configure(self, index: dict):
         """Per-checkpoint pipeline settings from model_index.json: force_zeros_for_empty_prompt (true for the base,
@@ -147,12 +202,14 @@ class StableDiffusionXLCustomPipeline:
         return self
 
     @staticmethod
-    def _load_pretrained(path: str, torch_dtype, device, cfg: Optional[UNetConfig], vae_cfg):
-        """-> (unet, prompt encoder or None, VAE decoder or None, VAE state dict or None, VAE config or None,
-        model_index.json as a dict, {} without one).  Without `cfg` the UNet's architecture comes from unet/config.json
-        (with model_index.json's requires_aesthetics_score: 5 time ids when true) or, without that file, is SDXL-base
-        with the input channel count of the checkpoint's conv_in."""
+    def _load_pretrained(path: str, torch_dtype, device, cfg: Optional[UNetConfig], vae_cfg) -> _Pretrained:
+        """Without `cfg` the UNet's architecture comes from unet/config.json (with model_index.json's
+        requires_aesthetics_score: 5 time ids when true) or, without that file, is SDXL-base with the input channel
+        count of the checkpoint's conv_in."""
         from safetensors.torch import load_file
+        from imagharmony_b200.config import SDXL_VAE
+        from imagharmony_b200.vae import AutoencoderKLDecoder
+        from .encoders import ClipPromptEncoder
         f = os.path.join(path, "unet", "diffusion_pytorch_model.safetensors")
         if not os.path.exists(f):
             f = os.path.join(path, "unet", "diffusion_pytorch_model.fp16.safetensors")
@@ -166,33 +223,26 @@ class StableDiffusionXLCustomPipeline:
         if cfg is None:
             cfg = SDXL_BASE
             if "conv_in.weight" in usd and usd["conv_in.weight"].shape[1] != cfg.in_channels:
-                import dataclasses
                 cfg = dataclasses.replace(cfg, in_channels=int(usd["conv_in.weight"].shape[1]))
         unet = UNet2DConditionModel.from_state_dict(cfg, usd, device=device)
         vae = vsd = vcfg = None
         for name in ("diffusion_pytorch_model.fp16.safetensors", "diffusion_pytorch_model.safetensors"):
             vf = os.path.join(path, "vae", name)
             if os.path.exists(vf):
-                import dataclasses
-                import json
-                from imagharmony_b200.config import SDXL_VAE
-                from imagharmony_b200.vae import AutoencoderKLDecoder
                 vcfg = vae_cfg or SDXL_VAE
-                cj = os.path.join(path, "vae", "config.json")
-                if vae_cfg is None and os.path.exists(cj):
+                vmeta = _read_json(path, "vae", "config.json")
+                if vae_cfg is None and vmeta:
                     # `force_upcast` decides between the scaled residual stream (the reference's fp32 upcast,
                     # custom_pipelines.py:366-371) and plain fp16 (fp16-fix checkpoints set it to false)
-                    meta = json.load(open(cj))
-                    vcfg = dataclasses.replace(vcfg, force_upcast=bool(meta.get("force_upcast", True)),
-                                               scaling_factor=float(meta.get("scaling_factor", vcfg.scaling_factor)))
+                    vcfg = dataclasses.replace(vcfg, force_upcast=bool(vmeta.get("force_upcast", True)),
+                                               scaling_factor=float(vmeta.get("scaling_factor", vcfg.scaling_factor)))
                 vsd = load_file(vf)
                 vae = AutoencoderKLDecoder.from_state_dict(vcfg, vsd, device=device)  # decoder keys only
                 break
         enc = None
-        from .encoders import ClipPromptEncoder
         if ClipPromptEncoder.available(path):
             enc = ClipPromptEncoder.from_pretrained(path, device=device, dtype=torch_dtype)
-        return unet, enc, vae, vsd, vcfg, index
+        return _Pretrained(unet, enc, vae, vsd, vcfg, index)
 
     def to(self, device=None, *args, **kwargs):
         """Weights live on the device the UNet was built on (from_random / from_pretrained take `device=`); moving 5 GB
@@ -403,8 +453,7 @@ class StableDiffusionXLCustomPipeline:
         """[3P] diffusers prepare_latents: randn * init_noise_sigma; a list of generators draws one sample each."""
         shape = (batch_size, num_channels_latents, height // self.vae_scale_factor, width // self.vae_scale_factor)
         if latents is None:
-            if isinstance(generator, list) and len(generator) != batch_size:
-                raise ValueError(f"got {len(generator)} generators for a batch of {batch_size}")
+            self._check_batches(batch_size, generator)
             latents = randn_tensor(shape, generator, torch.float32, "cpu")
         latents = latents.to(torch.float32) * self.scheduler.init_noise_sigma
         return latents.to(dtype)
@@ -427,39 +476,53 @@ class StableDiffusionXLCustomPipeline:
         """Parameter list of custom_pipelines.py:23-56.  Unknown keyword arguments are accepted and ignored, because
         IPAdapterXL.generate forwards a stray `number_class_crossattention=` into this call (test.py:38, demo.py:124)."""
         self._require_latent_unet()
-        height = height or self.default_sample_size * self.vae_scale_factor           # :189-190
-        width = width or self.default_sample_size * self.vae_scale_factor
-        original_size = original_size or (height, width)                              # :192-193
-        target_size = target_size or (height, width)
-        if height % 8 or width % 8:
-            raise ValueError(f"`height` and `width` have to be divisible by 8 but are {height} and {width}.")
+        height, width = self._checked_size(height, width)                             # :189-190
         self._check_callback_steps(callback, callback_steps)
-        do_classifier_free_guidance = guidance_scale > 1.0                            # :223
-        embeds = self.encode_prompt(prompt, prompt_2, None, num_images_per_prompt, do_classifier_free_guidance,
-                                    negative_prompt, negative_prompt_2, prompt_embeds, negative_prompt_embeds,
-                                    pooled_prompt_embeds, negative_pooled_prompt_embeds,
-                                    lora_scale=self._lora_call_scale(cross_attention_kwargs))  # :229-247
+        embeds, sizes = self._embeds_and_sizes(locals(), height, width)               # :192-193, :223, :229-247
         self.scheduler.set_timesteps(num_inference_steps)                             # :250
         lat = self.prepare_latents(embeds[0].shape[0], self.unet.config.in_channels, height, width, torch.float16,
                                    self.device, generator, latents)                  # :255-265
-        sizes = (original_size, crops_coords_top_left, target_size, negative_original_size,
-                 negative_crops_coords_top_left, negative_target_size)
-        out = self._denoise_from(lat, 0, num_inference_steps, denoising_end, embeds, sizes, guidance_scale,
-                                 guidance_rescale, control_guidance_start, control_guidance_end, callback, callback_steps,
-                                 generator=generator)
+        out = self._denoise_from(lat, num_inference_steps=num_inference_steps, embeds=embeds, sizes=sizes,
+                                 guidance_scale=guidance_scale, guidance_rescale=guidance_rescale,
+                                 denoising_end=denoising_end, control_guidance_start=control_guidance_start,
+                                 control_guidance_end=control_guidance_end, callback=callback,
+                                 callback_steps=callback_steps, generator=generator)
         return self._output(out, output_type, return_dict)
 
-    def _denoise_from(self, lat, t_start: int, num_inference_steps: int, denoising_end, embeds, sizes, guidance_scale,
-                      guidance_rescale, control_guidance_start, control_guidance_end, callback, callback_steps,
-                      inpaint=None, generator=None, unet_cond=None, controlnet=None, aesthetic=None) -> torch.Tensor:
+    def _checked_size(self, height: Optional[int], width: Optional[int]) -> Tuple[int, int]:
+        """The call's height and width (default: the UNet's sample size x 8), refused unless multiples of 8."""
+        height = height or self.default_sample_size * self.vae_scale_factor
+        width = width or self.default_sample_size * self.vae_scale_factor
+        if height % 8 or width % 8:
+            raise ValueError(f"`height` and `width` have to be divisible by 8 but are {height} and {width}.")
+        return height, width
+
+    def _embeds_and_sizes(self, call: Dict[str, Any], height: int, width: int):
+        """-> (encode_prompt's 4 embeddings, `sizes` for _add_time_ids) from the arguments of a pipeline call (its
+        locals(): every __call__ takes diffusers' prompt, embedding, LoRA-scale and size parameters under the same
+        names).  With a loaded LoRA the UNet is merged for the call's scale first; original_size and target_size
+        default to height x width."""
+        embeds = self.encode_prompt(call["prompt"], call["prompt_2"], None, call["num_images_per_prompt"],
+                                    call["guidance_scale"] > 1.0, call["negative_prompt"], call["negative_prompt_2"],
+                                    call["prompt_embeds"], call["negative_prompt_embeds"], call["pooled_prompt_embeds"],
+                                    call["negative_pooled_prompt_embeds"],
+                                    lora_scale=self._lora_call_scale(call["cross_attention_kwargs"]))
+        sizes = (call["original_size"] or (height, width), call["crops_coords_top_left"],
+                 call["target_size"] or (height, width), call["negative_original_size"],
+                 call["negative_crops_coords_top_left"], call["negative_target_size"])
+        return embeds, sizes
+
+    def _denoise_from(self, lat, *, num_inference_steps: int, embeds, sizes, guidance_scale, guidance_rescale,
+                      generator, callback, callback_steps, t_start: int = 0, denoising_end=None,
+                      control_guidance_start=0.0, control_guidance_end=1.0, inpaint=None, unet_cond=None,
+                      controlnet=None, aesthetic=None) -> torch.Tensor:
         """The loop over timesteps[t_start:], truncated by denoising_end (:307-316), from the noised start latents `lat`
         with the IP scale of the processors (:319-322); the micro-conditioning time ids are formed from `sizes`, and
         from `aesthetic` = (aesthetic_score, negative_aesthetic_score) for a 5-id UNet. -> final latents."""
         add_time_ids, negative_add_time_ids = self._add_time_ids(embeds[0].shape[0], sizes, aesthetic)
         loop_end = num_inference_steps
-        if denoising_end is not None and isinstance(denoising_end, float) and 0 < denoising_end < 1:
-            n_train = self.scheduler.num_train_timesteps
-            cutoff = int(round(n_train - denoising_end * n_train))
+        if _fraction(denoising_end):
+            cutoff = _denoising_cutoff(self.scheduler.num_train_timesteps, denoising_end)
             loop_end = t_start + int(sum(1 for t in self.scheduler.timesteps[t_start:] if t >= cutoff))
         conditioning_scale = self._ip_scale()
         if loop_end > t_start:
@@ -474,6 +537,16 @@ class StableDiffusionXLCustomPipeline:
             out = lat.to(self.device)
         self.set_scale(conditioning_scale)
         return out
+
+    @staticmethod
+    def _check_batches(batch_size: int, generator, *batches: Tuple[str, int]) -> None:
+        """Refuses, before anything is encoded or drawn, an input batch ((description, size) in `batches`) that does
+        not divide the prompt batch, then a list of generators that is not one per prompt-batch entry."""
+        for what, n in batches:
+            if batch_size % n:
+                raise ValueError(f"cannot duplicate {what} batch of {n} to a prompt batch of {batch_size}")
+        if isinstance(generator, list) and len(generator) != batch_size:
+            raise ValueError(f"got {len(generator)} generators for a batch of {batch_size}")
 
     @staticmethod
     def _check_callback_steps(callback, callback_steps) -> None:
@@ -545,35 +618,12 @@ def preprocess_image(image, vae_scale_factor: int = 8, height: Optional[int] = N
     one's size), or the requested `height` x `width` when both are given.  A [B, 3, H, W] / [3, H, W] tensor is taken
     as it is, resized (nearest) when its size is not a multiple of the factor or not the requested one; as in diffusers
     it is expected in [-1, 1], and one without negative values is taken as [0, 1] and normalised."""
-    import numpy as np
-    from PIL import Image
-    if isinstance(image, Image.Image) or (isinstance(image, (list, tuple)) and image and isinstance(image[0], Image.Image)):
-        images = [image] if isinstance(image, Image.Image) else list(image)
-        w, h = (x - x % vae_scale_factor for x in images[0].size)
+    def size(h, w):
         if height is not None and width is not None:
-            h, w = height, width
-        if w <= 0 or h <= 0:
-            raise ValueError(f"image of size {images[0].size} is smaller than {vae_scale_factor} pixels")
-        images = [im.convert("RGB") if im.mode != "RGB" else im for im in images]
-        images = [im if im.size == (w, h) else im.resize((w, h), resample=Image.LANCZOS) for im in images]
-        arr = np.stack([np.array(im).astype(np.float32) / 255.0 for im in images])
-        return torch.from_numpy(arr).permute(0, 3, 1, 2).contiguous() * 2.0 - 1.0
-    if isinstance(image, torch.Tensor):
-        x = image.unsqueeze(0) if image.dim() == 3 else image
-        if x.dim() != 4 or x.shape[1] != 3:
-            raise ValueError(f"image tensor must be [B, 3, H, W] or [3, H, W], got {tuple(image.shape)}")
-        x = x.float()
-        h, w = (v - v % vae_scale_factor for v in x.shape[2:])
-        if height is not None and width is not None:
-            h, w = height, width
-        if h <= 0 or w <= 0:
-            raise ValueError(f"image of size {tuple(x.shape[2:])} is smaller than {vae_scale_factor} pixels")
-        if (h, w) != tuple(x.shape[2:]):
-            x = torch.nn.functional.interpolate(x, size=(h, w))
-        if x.min() >= 0:
-            x = x * 2.0 - 1.0
-        return x.contiguous()
-    raise ValueError(f"`image` must be a PIL image, a list of them or a tensor, got {type(image).__name__}")
+            return height, width
+        return h - h % vae_scale_factor, w - w % vae_scale_factor
+    x = _load_images(image, size, "image", vae_scale_factor)
+    return x * 2.0 - 1.0 if x.min() >= 0 else x           # PIL images are in [0, 1]: always normalised
 
 
 class StableDiffusionXLImg2ImgPipeline(StableDiffusionXLCustomPipeline):
@@ -619,25 +669,17 @@ class StableDiffusionXLImg2ImgPipeline(StableDiffusionXLCustomPipeline):
         pipe = super().from_random(cfg, seed=seed, device=device, vae_cfg=vae_cfg)
         if vae_cfg is not None:
             from imagharmony_b200.vae import AutoencoderKLEncoder
-            from imagharmony_b200.weights import random_state_dict, shapes_of
-            with torch.device("meta"):
-                shapes = shapes_of(AutoencoderKLEncoder(vae_cfg))
-            gen_dev = device if str(device).startswith("cuda") else "cpu"
-            pipe.vae_encoder = AutoencoderKLEncoder.from_state_dict(vae_cfg, random_state_dict(shapes, seed + 19,
-                                                                                               device=gen_dev),
-                                                                    device=device)
+            pipe.vae_encoder = random_module(AutoencoderKLEncoder, vae_cfg, seed + 19, device)
         return pipe
 
     @classmethod
-    def from_pretrained(cls, path: str, torch_dtype=torch.float16, add_watermarker: bool = False, device="cuda",
-                        cfg: Optional[UNetConfig] = None, vae_cfg=None, **kwargs):
-        """As StableDiffusionXLCustomPipeline.from_pretrained; the VAE checkpoint also provides the encoder."""
-        unet, enc, vae, vsd, vcfg, index = cls._load_pretrained(path, torch_dtype, device, cfg, vae_cfg)
-        vae_encoder = None
-        if vsd is not None:
+    def _from_parts(cls, parts: _Pretrained, device, **kwargs):
+        """The VAE checkpoint also provides the encoder."""
+        pipe = super()._from_parts(parts, device)
+        if parts.vae_state is not None:
             from imagharmony_b200.vae import AutoencoderKLEncoder
-            vae_encoder = AutoencoderKLEncoder.from_state_dict(vcfg, vsd, device=device)
-        return cls(unet, prompt_encoder=enc, vae=vae, vae_encoder=vae_encoder)._configure(index)
+            pipe.vae_encoder = AutoencoderKLEncoder.from_state_dict(parts.vae_config, parts.vae_state, device=device)
+        return pipe
 
     def enable_vae_tiling(self):
         super().enable_vae_tiling()
@@ -648,27 +690,35 @@ class StableDiffusionXLImg2ImgPipeline(StableDiffusionXLCustomPipeline):
         """[3P] StableDiffusionXLImg2ImgPipeline.prepare_latents (fp16 latents): encode, sample the posterior, scale,
         add_noise(sigma).  eps (fp32 when the VAE config asks for the upcast, else fp16) and the fp16 noise are drawn
         here from the caller's generator(s) in diffusers' order; the arithmetic is one kernel."""
-        venc = self.vae_encoder
         n_img = image.shape[0]
-        if batch_size % n_img:
-            raise ValueError(f"cannot duplicate an image batch of {n_img} to a prompt batch of {batch_size}")
-        moments = venc.encode_moments_nhwc(image.to(self.device, torch.float16))      # [n_img, h, w, 16]
-        if isinstance(generator, list) and len(generator) != batch_size:
-            raise ValueError(f"got {len(generator)} generators for a batch of {batch_size}")
+        self._check_batches(batch_size, generator, ("an image", n_img))
         # with a list, every generator samples the posterior of the image of its batch slot
-        L, h, w = venc.config.latent_channels, moments.shape[1], moments.shape[2]
-        eps = self._posterior_eps(batch_size if isinstance(generator, list) else n_img, h, w, generator)
-        noise = randn_tensor((batch_size, L, h, w), generator, torch.float16, self.device, "cpu")
-        return ops.vae_posterior_noise(moments, eps, noise, L, venc.config.scaling_factor, sigma)
+        sample, noise = self._encode_posterior(image, batch_size if isinstance(generator, list) else n_img, generator,
+                                               batch_size)
+        return sample(noise, sigma)
 
     def prepare_handoff_latents(self, latents: torch.Tensor, batch_size: int) -> torch.Tensor:
         """[3P] StableDiffusionXLImg2ImgPipeline.prepare_latents(add_noise=False) for a latent `image`: the latents as
         they are (fp16 on the device), tiled to the prompt batch with torch.cat like encoded latents."""
         n_img = latents.shape[0]
-        if batch_size % n_img:
-            raise ValueError(f"cannot duplicate a latent batch of {n_img} to a prompt batch of {batch_size}")
+        self._check_batches(batch_size, None, ("a latent", n_img))
         lat = latents.to(self.device, torch.float16)
         return lat.repeat(batch_size // n_img, 1, 1, 1) if batch_size > n_img else lat
+
+    def _encode_posterior(self, image: torch.Tensor, n_eps: int, generator, noise_batch: Optional[int] = None):
+        """Encodes `image` and draws the posterior eps of n_eps images (_posterior_eps), then, given noise_batch, the
+        fp16 noise [noise_batch, 4, h, w]: both from `generator` in diffusers' order.  -> (sample, noise or None), where
+        sample(x, sigma) is the scaled posterior sample + x * sigma for a [B, 4, h, w] x, fp16 on the device, in one
+        kernel (ops.vae_posterior_noise; slot b samples image b % n_eps).  Zero x and sigma 0 give the clean latents
+        exactly (fp16(zs + 0) = zs)."""
+        venc = self.vae_encoder
+        moments = venc.encode_moments_nhwc(image.to(self.device, torch.float16))      # [n_img, h, w, 16]
+        L, sf, h, w = venc.config.latent_channels, venc.config.scaling_factor, moments.shape[1], moments.shape[2]
+        eps = self._posterior_eps(n_eps, h, w, generator)
+        noise = None
+        if noise_batch is not None:
+            noise = randn_tensor((noise_batch, L, h, w), generator, torch.float16, self.device, "cpu")
+        return (lambda x, sigma: ops.vae_posterior_noise(moments, eps, x, L, sf, sigma)), noise
 
     def _posterior_eps(self, n: int, h: int, w: int, generator) -> torch.Tensor:
         """The posterior draw of [3P] diffusers' `_encode_vae_image(images, generator)` for n images with latents of
@@ -721,20 +771,11 @@ class StableDiffusionXLImg2ImgPipeline(StableDiffusionXLCustomPipeline):
         if handoff:
             height, width = image.shape[2] * self.vae_scale_factor, image.shape[3] * self.vae_scale_factor
         else:
-            self._refuse_tiny_vae_encode()
-            if self.vae_encoder is None:
-                raise IHError("this pipeline has no VAE encoder: build it with from_random(vae_cfg=...) or "
-                              "from_pretrained with a vae/ folder")
+            self._require_vae_encoder()
             pixels = preprocess_image(image, self.vae_scale_factor)
             height, width = pixels.shape[2], pixels.shape[3]
         require_latent_size(self.unet.config, height // self.vae_scale_factor, width // self.vae_scale_factor)
-        original_size = original_size or (height, width)
-        target_size = target_size or (height, width)
-        do_classifier_free_guidance = guidance_scale > 1.0
-        embeds = self.encode_prompt(prompt, prompt_2, None, num_images_per_prompt, do_classifier_free_guidance,
-                                    negative_prompt, negative_prompt_2, prompt_embeds, negative_prompt_embeds,
-                                    pooled_prompt_embeds, negative_pooled_prompt_embeds,
-                                    lora_scale=self._lora_call_scale(cross_attention_kwargs))
+        embeds, sizes = self._embeds_and_sizes(locals(), height, width)
         self.scheduler.set_timesteps(num_inference_steps)
         if handoff:
             t_start = denoising_start_begin_step(self.scheduler.timesteps, self.scheduler.num_train_timesteps, start)
@@ -742,23 +783,26 @@ class StableDiffusionXLImg2ImgPipeline(StableDiffusionXLCustomPipeline):
         else:
             lat = self.prepare_img2img_latents(pixels, embeds[0].shape[0], generator,
                                                self.scheduler.add_noise_sigma(t_start))
-        sizes = (original_size, crops_coords_top_left, target_size, negative_original_size,
-                 negative_crops_coords_top_left, negative_target_size)
         aesthetic = (aesthetic_score, negative_aesthetic_score) if self.unet.config.num_time_ids == 5 else None
-        out = self._denoise_from(lat, t_start, num_inference_steps, denoising_end, embeds, sizes, guidance_scale,
-                                 guidance_rescale, control_guidance_start, control_guidance_end, callback, callback_steps,
-                                 generator=generator, aesthetic=aesthetic)
+        out = self._denoise_from(lat, t_start=t_start, num_inference_steps=num_inference_steps, embeds=embeds,
+                                 sizes=sizes, guidance_scale=guidance_scale, guidance_rescale=guidance_rescale,
+                                 denoising_end=denoising_end, control_guidance_start=control_guidance_start,
+                                 control_guidance_end=control_guidance_end, callback=callback,
+                                 callback_steps=callback_steps, generator=generator, aesthetic=aesthetic)
         return self._output(out, output_type, return_dict)
 
-    def _refuse_tiny_vae_encode(self) -> None:
-        """With a tiny autoencoder as `pipe.vae` diffusers encodes a pixel image with the tiny encoder, which is not built
-        here; encoding with the KL encoder instead would silently give other latents.  Latent hand-overs
-        (`denoising_start`) encode nothing and run."""
+    def _require_vae_encoder(self) -> None:
+        """Encoding a pixel image needs the KL VAE encoder.  With a tiny autoencoder as `pipe.vae` diffusers encodes
+        with the tiny encoder, which is not built here; encoding with the KL encoder instead would silently give other
+        latents.  Latent hand-overs (`denoising_start`) encode nothing and run."""
         from imagharmony_b200.taesd import AutoencoderTinyDecoder
         if isinstance(self.vae, AutoencoderTinyDecoder):
             raise IHError(f"{type(self).__name__}: encoding a pixel image with a tiny autoencoder (AutoencoderTiny) as "
                           "pipe.vae is not implemented; keep the KL VAE for this call, or pass latents with "
                           "denoising_start")
+        if self.vae_encoder is None:
+            raise IHError("this pipeline has no VAE encoder: build it with from_random(vae_cfg=...) or from_pretrained "
+                          "with a vae/ folder")
 
     def _require_euler(self) -> None:
         """Image-to-image and inpainting noise the image latents with Euler's add_noise (x + sigma * noise) inside the
@@ -786,8 +830,8 @@ def preprocess_mask(mask, height: int, width: int) -> torch.Tensor:
     -> float32 [B, 1, height, width]."""
     import numpy as np
     from PIL import Image
-    if isinstance(mask, Image.Image) or (isinstance(mask, (list, tuple)) and mask and isinstance(mask[0], Image.Image)):
-        masks = [mask] if isinstance(mask, Image.Image) else list(mask)
+    masks = _pil_list(mask)
+    if masks is not None:
         masks = [m.convert("L").resize((width, height), resample=Image.LANCZOS) for m in masks]
         x = torch.from_numpy(np.stack([np.array(m).astype(np.float32) / 255.0 for m in masks]))[:, None]
     elif isinstance(mask, torch.Tensor):
@@ -830,25 +874,17 @@ class StableDiffusionXLInpaintPipeline(StableDiffusionXLImg2ImgPipeline):
                                 is_strength_max: bool) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
         """[3P] StableDiffusionXLInpaintPipeline.prepare_latents (return_image_latents, fp16 latents) ->
         (start latents, clean image latents, noise), each [batch_size, 4, h, w] fp16 on the device.  The posterior
-        kernel runs twice: with sigma 0 and zero noise it returns the clean latents exactly (fp16(zs + 0) = zs), with the
-        noise and sigma[t_start] the start latents (add_noise); at strength 1 the start is noise * init_noise_sigma."""
-        venc = self.vae_encoder
+        kernel gives the clean latents (_encode_posterior) and, with the noise and sigma[t_start], the start latents
+        (add_noise); at strength 1 the start is noise * init_noise_sigma."""
         n_img = image.shape[0]
-        if batch_size % n_img:
-            raise ValueError(f"cannot duplicate an image batch of {n_img} to a prompt batch of {batch_size}")
-        moments = venc.encode_moments_nhwc(image.to(self.device, torch.float16))      # [n_img, h, w, 16]
-        if isinstance(generator, list) and len(generator) != batch_size:
-            raise ValueError(f"got {len(generator)} generators for a batch of {batch_size}")
-        L, h, w = venc.config.latent_channels, moments.shape[1], moments.shape[2]
+        self._check_batches(batch_size, generator, ("an image", n_img))
         # _encode_vae_image samples the n_img images with generator[i] before the batch is tiled
-        eps = self._posterior_eps(n_img, h, w, generator)
-        noise = randn_tensor((batch_size, L, h, w), generator, torch.float16, self.device, "cpu")
-        sf = venc.config.scaling_factor
-        image_latents = ops.vae_posterior_noise(moments, eps, torch.zeros_like(noise), L, sf, 0.0)
+        sample, noise = self._encode_posterior(image, n_img, generator, batch_size)
+        image_latents = sample(torch.zeros_like(noise), 0.0)
         if is_strength_max:
             latents = (noise.float() * self.scheduler.init_noise_sigma).half()
         else:
-            latents = ops.vae_posterior_noise(moments, eps, noise, L, sf, self.scheduler.add_noise_sigma(t_start))
+            latents = sample(noise, self.scheduler.add_noise_sigma(t_start))
         return latents, image_latents, noise
 
     @torch.no_grad()
@@ -878,49 +914,39 @@ class StableDiffusionXLInpaintPipeline(StableDiffusionXLImg2ImgPipeline):
                           f"UNet (this one has config.in_channels = {self.unet.config.in_channels} and a conv_in of "
                           f"{self.unet.conv_in.weight.shape[1]} input channels)")
         t_start = self._begin_index(num_inference_steps, strength)
-        height = height or self.default_sample_size * self.vae_scale_factor
-        width = width or self.default_sample_size * self.vae_scale_factor
-        if height % 8 != 0 or width % 8 != 0:
-            raise ValueError(f"`height` and `width` have to be divisible by 8 but are {height} and {width}.")
+        height, width = self._checked_size(height, width)
         self._check_callback_steps(callback, callback_steps)
         if image is None or mask_image is None:
             raise ValueError("`image` and `mask_image` inputs cannot be undefined")
-        self._refuse_tiny_vae_encode()
-        if self.vae_encoder is None:
-            raise IHError("this pipeline has no VAE encoder: build it with from_random(vae_cfg=...) or from_pretrained "
-                          "with a vae/ folder")
+        self._require_vae_encoder()
         pixels = preprocess_image(image, self.vae_scale_factor, height, width)
         mask = preprocess_mask(mask_image, height, width)
-        do_classifier_free_guidance = guidance_scale > 1.0
-        embeds = self.encode_prompt(prompt, prompt_2, None, num_images_per_prompt, do_classifier_free_guidance,
-                                    negative_prompt, negative_prompt_2, prompt_embeds, negative_prompt_embeds,
-                                    pooled_prompt_embeds, negative_pooled_prompt_embeds,
-                                    lora_scale=self._lora_call_scale(cross_attention_kwargs))
+        embeds, sizes = self._embeds_and_sizes(locals(), height, width)
         batch = embeds[0].shape[0]
         self.scheduler.set_timesteps(num_inference_steps)
-        sizes = (original_size or (height, width), crops_coords_top_left, target_size or (height, width),
-                 negative_original_size, negative_crops_coords_top_left, negative_target_size)
         if unet9:
             lat, mask_lat, masked_lat = self.prepare_inpaint9_inputs(pixels, mask, batch, generator, t_start,
                                                                      strength == 1.0)
-            out = self._denoise_from(lat, t_start, num_inference_steps, denoising_end, embeds, sizes, guidance_scale,
-                                     guidance_rescale, control_guidance_start, control_guidance_end, callback,
-                                     callback_steps, generator=generator, unet_cond=(mask_lat, masked_lat))
-            return self._output(out, output_type, return_dict)
-        lat, image_latents, noise = self.prepare_inpaint_latents(pixels, batch, generator, t_start, strength == 1.0)
-        # the masked image's latents only feed a 9-channel UNet: with 4 channels diffusers encodes them unused.  That
-        # encode is skipped; its posterior draw comes after the noise, so it changes only what is drawn later: the step
-        # noise of Euler Ancestral, for which the draw is made and dropped (SURVEY C.31)
-        h, w = height // self.vae_scale_factor, width // self.vae_scale_factor
-        if isinstance(self.scheduler, EulerAncestralDiscreteScheduler):
-            self._posterior_eps(max(pixels.shape[0], mask.shape[0]), h, w, generator)
-        mask_lat = torch.nn.functional.interpolate(mask, size=(h, w)).half()
-        if batch % mask_lat.shape[0]:
-            raise ValueError(f"cannot duplicate a mask batch of {mask_lat.shape[0]} to a prompt batch of {batch}")
-        mask_lat = mask_lat.repeat(batch // mask_lat.shape[0], 1, 1, 1).to(self.device)
-        out = self._denoise_from(lat, t_start, num_inference_steps, denoising_end, embeds, sizes, guidance_scale,
-                                 guidance_rescale, control_guidance_start, control_guidance_end, callback, callback_steps,
-                                 inpaint=(image_latents, noise, mask_lat), generator=generator)
+            cond = dict(unet_cond=(mask_lat, masked_lat))
+        else:
+            # the mask's batch is refused before the encode, after the image's and the generators' checks
+            self._check_batches(batch, generator, ("an image", pixels.shape[0]))
+            self._check_batches(batch, None, ("a mask", mask.shape[0]))
+            lat, image_latents, noise = self.prepare_inpaint_latents(pixels, batch, generator, t_start, strength == 1.0)
+            # the masked image's latents only feed a 9-channel UNet: with 4 channels diffusers encodes them unused.
+            # That encode is skipped; its posterior draw comes after the noise, so it changes only what is drawn later:
+            # the step noise of Euler Ancestral, for which the draw is made and dropped (SURVEY C.31)
+            h, w = height // self.vae_scale_factor, width // self.vae_scale_factor
+            if isinstance(self.scheduler, EulerAncestralDiscreteScheduler):
+                self._posterior_eps(max(pixels.shape[0], mask.shape[0]), h, w, generator)
+            mask_lat = torch.nn.functional.interpolate(mask, size=(h, w)).half()
+            mask_lat = mask_lat.repeat(batch // mask_lat.shape[0], 1, 1, 1).to(self.device)
+            cond = dict(inpaint=(image_latents, noise, mask_lat))
+        out = self._denoise_from(lat, t_start=t_start, num_inference_steps=num_inference_steps, embeds=embeds,
+                                 sizes=sizes, guidance_scale=guidance_scale, guidance_rescale=guidance_rescale,
+                                 denoising_end=denoising_end, control_guidance_start=control_guidance_start,
+                                 control_guidance_end=control_guidance_end, callback=callback,
+                                 callback_steps=callback_steps, generator=generator, **cond)
         return self._output(out, output_type, return_dict)
 
     def prepare_inpaint9_inputs(self, image: torch.Tensor, mask: torch.Tensor, batch_size: int, generator, t_start: int,
@@ -929,33 +955,23 @@ class StableDiffusionXLInpaintPipeline(StableDiffusionXLImg2ImgPipeline):
         for the 9-channel UNet -> (start latents [batch_size, 4, h, w], mask [batch_size, 1, h, w], masked-image latents
         [batch_size, 4, h, w]), fp16 on the device, CFG halves not yet formed.  Per generator the draws come in
         diffusers' order: the image's posterior eps (strength < 1 only: at strength 1 the image is not encoded), the
-        noise, then the masked images' posterior eps (SURVEY C.32).  Both encodes use the posterior kernel; with sigma 0
-        and zero noise it returns the scaled posterior sample exactly."""
-        venc = self.vae_encoder
+        noise, then the masked images' posterior eps (SURVEY C.32).  Both encodes use the posterior kernel
+        (_encode_posterior)."""
         n_img, n_mask = image.shape[0], mask.shape[0]
         if n_img != n_mask and 1 not in (n_img, n_mask):
             raise ValueError(f"an image batch of {n_img} and a mask batch of {n_mask} do not broadcast")
         n_masked = max(n_img, n_mask)
-        for what, k in (("image", n_img), ("mask", n_mask), ("masked image", n_masked)):
-            if batch_size % k:
-                raise ValueError(f"cannot duplicate a {what} batch of {k} to a prompt batch of {batch_size}")
-        if isinstance(generator, list) and len(generator) != batch_size:
-            raise ValueError(f"got {len(generator)} generators for a batch of {batch_size}")
-        L, sf = venc.config.latent_channels, venc.config.scaling_factor
-        shape = (batch_size, L, image.shape[2] // self.vae_scale_factor, image.shape[3] // self.vae_scale_factor)
+        self._check_batches(batch_size, generator, ("a image", n_img), ("a mask", n_mask), ("a masked image", n_masked))
+        shape = (batch_size, self.vae_encoder.config.latent_channels, image.shape[2] // self.vae_scale_factor,
+                 image.shape[3] // self.vae_scale_factor)
         if is_strength_max:
             noise = randn_tensor(shape, generator, torch.float16, self.device, "cpu")
             latents = (noise.float() * self.scheduler.init_noise_sigma).half()
         else:
-            moments = venc.encode_moments_nhwc(image.to(self.device, torch.float16))
-            eps = self._posterior_eps(n_img, *shape[2:], generator)
-            noise = randn_tensor(shape, generator, torch.float16, self.device, "cpu")
-            latents = ops.vae_posterior_noise(moments, eps, noise, L, sf, self.scheduler.add_noise_sigma(t_start))
-        masked = image * (mask < 0.5)
-        moments = venc.encode_moments_nhwc(masked.to(self.device, torch.float16))
-        eps = self._posterior_eps(n_masked, *shape[2:], generator)
-        zeros = torch.zeros(shape, dtype=torch.float16, device=self.device)
-        masked_latents = ops.vae_posterior_noise(moments, eps, zeros, L, sf, 0.0)
+            sample, noise = self._encode_posterior(image, n_img, generator, batch_size)
+            latents = sample(noise, self.scheduler.add_noise_sigma(t_start))
+        sample, _ = self._encode_posterior(image * (mask < 0.5), n_masked, generator)
+        masked_latents = sample(torch.zeros_like(noise), 0.0)
         mask_lat = torch.nn.functional.interpolate(mask, size=shape[2:]).half()
         return latents, mask_lat.repeat(batch_size // n_mask, 1, 1, 1).to(self.device), masked_latents
 
@@ -966,32 +982,10 @@ def preprocess_control_image(image, height: Optional[int] = None, width: Optiona
     control-image processor: PIL image(s) -> RGB, Lanczos resize to width x height, / 255; a [B, 3, H, W] / [3, H, W]
     tensor in [0, 1] is resized with nearest interpolation.  Without height / width the first image's size floored to
     multiples of `vae_scale_factor` is used.  -> float32 [B, 3, height, width] in [0, 1]."""
-    import numpy as np
-    from PIL import Image
-    if isinstance(image, Image.Image) or (isinstance(image, (list, tuple)) and image and isinstance(image[0], Image.Image)):
-        images = [image] if isinstance(image, Image.Image) else list(image)
-        w0, h0 = images[0].size
-        h = height if height is not None else h0 - h0 % vae_scale_factor
-        w = width if width is not None else w0 - w0 % vae_scale_factor
-        if h <= 0 or w <= 0:
-            raise ValueError(f"control image of size {images[0].size} is smaller than {vae_scale_factor} pixels")
-        images = [im.convert("RGB") if im.mode != "RGB" else im for im in images]
-        images = [im if im.size == (w, h) else im.resize((w, h), resample=Image.LANCZOS) for im in images]
-        arr = np.stack([np.array(im).astype(np.float32) / 255.0 for im in images])
-        return torch.from_numpy(arr).permute(0, 3, 1, 2).contiguous()
-    if isinstance(image, torch.Tensor):
-        x = image.unsqueeze(0) if image.dim() == 3 else image
-        if x.dim() != 4 or x.shape[1] != 3:
-            raise ValueError(f"control image tensor must be [B, 3, H, W] or [3, H, W], got {tuple(image.shape)}")
-        x = x.float()
-        h = height if height is not None else x.shape[2] - x.shape[2] % vae_scale_factor
-        w = width if width is not None else x.shape[3] - x.shape[3] % vae_scale_factor
-        if h <= 0 or w <= 0:
-            raise ValueError(f"control image of size {tuple(x.shape[2:])} is smaller than {vae_scale_factor} pixels")
-        if (h, w) != tuple(x.shape[2:]):
-            x = torch.nn.functional.interpolate(x, size=(h, w))
-        return x.contiguous()
-    raise ValueError(f"`image` must be a PIL image, a list of them or a tensor, got {type(image).__name__}")
+    def size(h, w):
+        return (height if height is not None else h - h % vae_scale_factor,
+                width if width is not None else w - w % vae_scale_factor)
+    return _load_images(image, size, "control image", vae_scale_factor)
 
 
 class StableDiffusionXLControlNetPipeline(StableDiffusionXLCustomPipeline):
@@ -1031,26 +1025,24 @@ class StableDiffusionXLControlNetPipeline(StableDiffusionXLCustomPipeline):
         """Random-init UNet and ControlNet weights (every weight random, zero convs included).  A list of ControlNet
         configs gives a Multi-ControlNet pipeline, net j seeded with seed + 23 + 7j."""
         from imagharmony_b200.controlnet import ControlNetModel
-        from imagharmony_b200.weights import random_state_dict, shapes_of
         base = StableDiffusionXLCustomPipeline.from_random(cfg, seed=seed, device=device, vae_cfg=vae_cfg)
-        gen_dev = device if str(device).startswith("cuda") else "cpu"
-        nets = []
-        for j, c in enumerate(controlnet_cfg if isinstance(controlnet_cfg, (list, tuple)) else [controlnet_cfg]):
-            with torch.device("meta"):
-                shapes = shapes_of(ControlNetModel(c))
-            nets.append(ControlNetModel.from_state_dict(c, random_state_dict(shapes, seed + 23 + 7 * j, device=gen_dev),
-                                                        device=device))
+        cfgs = controlnet_cfg if isinstance(controlnet_cfg, (list, tuple)) else [controlnet_cfg]
+        nets = [random_module(ControlNetModel, c, seed + 23 + 7 * j, device) for j, c in enumerate(cfgs)]
         return cls(base.unet, nets if isinstance(controlnet_cfg, (list, tuple)) else nets[0], vae=base.vae)
 
     @classmethod
     def from_pretrained(cls, path: str, controlnet=None, torch_dtype=torch.float16, add_watermarker: bool = False,
                         device="cuda", cfg: Optional[UNetConfig] = None, vae_cfg=None, **kwargs):
         """`controlnet=ControlNetModel.from_pretrained(dir)` (or a list of them, or a MultiControlNetModel) with the
-        SDXL folder `path` of StableDiffusionXLCustomPipeline.from_pretrained."""
+        SDXL folder `path` of StableDiffusionXLCustomPipeline.from_pretrained; refused before anything is read
+        without it."""
         if controlnet is None:
             raise ValueError("StableDiffusionXLControlNetPipeline.from_pretrained needs controlnet=")
-        unet, enc, vae, _, _, index = cls._load_pretrained(path, torch_dtype, device, cfg, vae_cfg)
-        return cls(unet, controlnet, prompt_encoder=enc, vae=vae)._configure(index)
+        return super().from_pretrained(path, torch_dtype, add_watermarker, device, cfg, vae_cfg, controlnet=controlnet)
+
+    @classmethod
+    def _from_parts(cls, parts: _Pretrained, device, controlnet=None, **kwargs):
+        return cls(parts.unet, controlnet, prompt_encoder=parts.prompt_encoder, vae=parts.vae)
 
     def _align_multi(self, image, scale, start, end):
         """[3P] diffusers 0.30 for a MultiControlNetModel: scalar guidance start / end become lists (the length of the
@@ -1130,13 +1122,8 @@ class StableDiffusionXLControlNetPipeline(StableDiffusionXLCustomPipeline):
         if any(tuple(c.shape[2:]) != (height, width) for c in controls):
             raise ValueError(f"the control images come out at different sizes {[tuple(c.shape[2:]) for c in controls]}; "
                              "pass images of one size, or height and width")
-        if height % 8 or width % 8:
-            raise ValueError(f"`height` and `width` have to be divisible by 8 but are {height} and {width}.")
-        do_classifier_free_guidance = guidance_scale > 1.0
-        embeds = self.encode_prompt(prompt, prompt_2, None, num_images_per_prompt, do_classifier_free_guidance,
-                                    negative_prompt, negative_prompt_2, prompt_embeds, negative_prompt_embeds,
-                                    pooled_prompt_embeds, negative_pooled_prompt_embeds,
-                                    lora_scale=self._lora_call_scale(cross_attention_kwargs))
+        height, width = self._checked_size(height, width)
+        embeds, sizes = self._embeds_and_sizes(locals(), height, width)
         batch = embeds[0].shape[0]
         # [3P] prepare_image, per net: repeat_interleave by the batch (one image) or by num_images_per_prompt; the CFG
         # copy is the engine's (the embedding is computed once and duplicated)
@@ -1148,13 +1135,11 @@ class StableDiffusionXLControlNetPipeline(StableDiffusionXLCustomPipeline):
         self.scheduler.set_timesteps(num_inference_steps)
         lat = self.prepare_latents(batch, self.unet.config.in_channels, height, width, torch.float16, self.device,
                                    generator, latents)
-        sizes = (original_size or (height, width), crops_coords_top_left, target_size or (height, width),
-                 negative_original_size, negative_crops_coords_top_left, negative_target_size)
         models = list(self.controlnet.nets) if multi else [self.controlnet]
         cn = [ControlNetCall(m, c.half(), s, bool(guess_mode), controlnet_keep(num_inference_steps, start, end))
               for m, c, s, start, end in zip(models, controls, scales, starts, ends)]
         # the IP scale is not gated: its window stays [0, 1]
-        out = self._denoise_from(lat, 0, num_inference_steps, None, embeds, sizes, guidance_scale, guidance_rescale,
-                                 0.0, 1.0, callback, callback_steps, generator=generator,
-                                 controlnet=cn if multi else cn[0])
+        out = self._denoise_from(lat, num_inference_steps=num_inference_steps, embeds=embeds, sizes=sizes,
+                                 guidance_scale=guidance_scale, guidance_rescale=guidance_rescale, callback=callback,
+                                 callback_steps=callback_steps, generator=generator, controlnet=cn if multi else cn[0])
         return self._output(out, output_type, return_dict)
