@@ -59,7 +59,7 @@ struct GemmParams {
   __half* out;
   long long ldo;
   int act;  // 0 none, 1 SiLU, 2 GELU(erf), 3 quick-GELU (applied after bias, before residual)
-  int relu;  // IH_EPI_RELU: max(x, 0) AFTER the residual add (TAESD's fuse(conv(x) + skip(x)))
+  int relu;  // IH_EPI_RELU: relu_nan_f AFTER the residual add (TAESD's fuse(conv(x) + skip(x)))
   unsigned long long* trace;  // optional: %globaltimer stamps of CTA 0 (ih_gemm_set_trace), nullptr in production
   // L2 prefetch of the NEXT kernel's weights (ih_gemm_prefetch_next): inside a denoise step every GEMM streams its weights
   // from HBM (5.2 GB per step >> L2), and a short launch cannot hide the first HBM round trips.  An otherwise idle
@@ -409,8 +409,8 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_f16_kernel(const __grid_
                 x1v += f.y;
               }
               if (p.relu) {
-                x0v = fmaxf(x0v, 0.f);
-                x1v = fmaxf(x1v, 0.f);
+                x0v = relu_nan_f(x0v);
+                x1v = relu_nan_f(x1v);
               }
               *slot = pack_half2(x0v, x1v);
             }

@@ -250,6 +250,13 @@ __device__ __forceinline__ float erf_as(float x) {
   return copysignf(r, x);
 }
 __device__ __forceinline__ float gelu_erf_f(float x) { return 0.5f * x * (1.f + erf_as(x * 0.70710678118654752f)); }
+// ReLU that keeps NaN as torch.relu does (fmaxf(x, 0) returns 0 for a NaN x): max.NaN.f32 returns NaN when an operand
+// is NaN, and is one FMNMX like fmaxf, where a compare + select would be two instructions per element.
+__device__ __forceinline__ float relu_nan_f(float x) {
+  float r;
+  asm("max.NaN.f32 %0, %1, 0f00000000;" : "=f"(r) : "f"(x));
+  return r;
+}
 
 }  // namespace ih
 

@@ -28,7 +28,8 @@ extern "C" {
 #define IH_EPI_QUICK_GELU 8 /* out = x * sigmoid(1.702 x), x = acc + bias  (CLIP-L text tower MLP, scope row f2) */
 /* out = relu(alpha * acc + bias + residual).  Unlike SILU / GELU / QUICK_GELU, which act on acc + bias BEFORE the
  * residual is added, ReLU acts AFTER it: the tiny autoencoder's block output relu(conv(x) + x) is one launch.  Not
- * combinable with the other flags; ih_conv2d_scaled_f16 accepts it too. */
+ * combinable with the other flags; ih_conv2d_scaled_f16 accepts it too.  NaN propagates as in torch.relu (NaN and +inf
+ * pass through, negatives and -inf become 0; the sign of a zero is unspecified). */
 #define IH_EPI_RELU 16
 
 const char* ih_last_error(void);

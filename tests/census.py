@@ -21,6 +21,9 @@ plus the magnitudes the bars need.  Bars (max err / bar <= 1 passes):
   - the epilogue in fp32 (fma with the bias, activation, residual add): EPI = 2^-21 of the values it forms, a few
     fp32 roundings and the fp32 erf / exp approximations;
   - both carried through the steepest slope of the activation (1.13 for GELU; SiLU and quick-GELU peak at 1.10);
+  - `relu` (IH_EPI_RELU, applied after the residual): the reference is relu of the fp64 sum and the slack stays that
+    of the sum, because ReLU is 1-Lipschitz (|relu(a) - relu(b)| <= |a - b|); the half ulp is of the stored value;
+  the fp64 references of convs with more than 2^28 output elements are computed a slice of images at a time;
 * the folded-LayerNorm consumer, against both the slot statistics the kernel reads and the true fp64 statistics of
   its raw rows: plus the error of var = E[x^2] - mean^2 from fp32 sums of K terms (the producer's slots and their
   total; each sum off by at most K 2^-24 of its magnitude, the fp16 squares exact in fp32), 3 K 2^-24 E[x^2] /
@@ -74,6 +77,10 @@ plus the magnitudes the bars need.  Bars (max err / bar <= 1 passes):
 
 The scheduler step kernels and the model-input scaling are not model ops: STEP_KERNELS names the bit-exact test that
 checks each at SDXL bucket latent sizes.
+
+A reference that ignores one of its op's arguments would pass a kernel that ignores it too.  So each reference reads
+its arguments through a dict that records the keys read, and `Census.unread()` lists every (op, argument) of the
+calls checked that the reference never read and that UNREAD does not excuse.
 """
 import inspect
 import math
@@ -175,7 +182,7 @@ def _act_slack(p, pre, s):
 
 
 def ref_linear(res, p):
-    x, w, bias, ln = p["x"].double(), p["w"].double(), p["bias"], p["ln"]
+    x, w, bias, ln, relu = p["x"].double(), p["w"].double(), p["bias"], p["ln"], p["relu"]
     K = x.shape[1]
     kw = dict(rowbias=p["rowbias"], rows_per_group=p["rows_per_group"], geglu=p["geglu"], silu=p["silu"],
               gelu=p["gelu"], quick_gelu=p["quick_gelu"], alpha=p["alpha"])
@@ -194,8 +201,8 @@ def ref_linear(res, p):
     s = _act_slack(p, pre, s)
 
     def ratio(act):          # act: the epilogue's value before the residual, unrounded fp64
-        ref = act + resid
-        return ulp_ratio(res, ref, 0.5, s + EPI * (ref.abs() + act.abs()))
+        tot = act + resid
+        return ulp_ratio(res, torch.relu(tot) if relu else tot, 0.5, s + EPI * (tot.abs() + act.abs()))
     worst = ratio(fake_ops.linear(x, w, bias, ln=ln, **kw))
     if ln is not None:
         # the same GEMM with the true fp64 statistics of the raw rows: rstd * x through the plain path
@@ -217,14 +224,24 @@ def stats_ratio(stats, out):
 
 
 def ref_conv3x3(res, p):
-    sc = p["shortcut"]
-    x, w = p["x"].double(), p["w_packed"].double()
-    sc64 = None if sc is None else (sc[0].double(), None if sc[1] is None else sc[1].double())
-    pre = fake_ops.conv3x3(x, w, p["bias"], rowbias=p["rowbias"], shortcut=sc64, stride=p["stride"], alpha=p["alpha"])
-    ref = pre + (0.0 if p["residual"] is None else p["residual"].double())
-    sc_abs = None if sc64 is None else tuple(None if t is None else t.abs() for t in sc64)
-    mag = fake_ops.conv3x3(x.abs(), w.abs(), stride=p["stride"], alpha=abs(p["alpha"]), shortcut=sc_abs)
-    return ulp_ratio(res, ref, 0.5, acc_allowance(w.shape[1]) * mag + EPI * (pre.abs() + ref.abs()))
+    sc, rowbias, residual, stride, alpha, relu = (p[n] for n in ("shortcut", "rowbias", "residual", "stride", "alpha",
+                                                                "relu"))
+    w = p["w_packed"].double()
+    B = p["x"].shape[0]
+    per = max(1, (1 << 28) // res[0].numel())        # images per slice: <= 2 GiB per fp64 output-sized tensor
+    worst = 0.0
+    for b0 in range(0, B, per):
+        i = slice(b0, min(B, b0 + per))
+        x = p["x"][i].double()
+        sc64 = None if sc is None else (sc[0][i].double(), None if sc[1] is None else sc[1][i].double())
+        pre = fake_ops.conv3x3(x, w, p["bias"], rowbias=None if rowbias is None else rowbias[i], shortcut=sc64,
+                               stride=stride, alpha=alpha)
+        tot = pre + (0.0 if residual is None else residual[i].double())
+        sc_abs = None if sc64 is None else tuple(None if t is None else t.abs() for t in sc64)
+        mag = fake_ops.conv3x3(x.abs(), w.abs(), stride=stride, alpha=abs(alpha), shortcut=sc_abs)
+        worst = max(worst, ulp_ratio(res[i], torch.relu(tot) if relu else tot, 0.5,
+                                     acc_allowance(w.shape[1]) * mag + EPI * (pre.abs() + tot.abs())))
+    return worst
 
 
 def ref_attention(res, p):
@@ -437,6 +454,30 @@ REFERENCES = {
 IN_PLACE = {"softmax_rows_masked_": "x", "controlnet_add_residuals": "skips", "controlnet_add_residuals_multi": "skips"}
 OUTPUTS = {"out", "stats_out"}                  # written by the op: compared after the call, never snapshotted
 NOT_KEYED = {"ws"}                            # persistent scratch: its size does not change what the op computes
+UNREAD = {             # arguments a reference may leave unread, and why; any other unread argument fails the census
+    "out": "the destination: the reference compares what the op wrote there (or returned)",
+    "tile_n": "GEMM / conv tile width: every output still sums its own K products in one fp32 accumulator, so the bar "
+              "holds for every width; the census key records it",
+    "kv_split": "attention work split: the bar of the unsplit softmax covers the split-and-merge (test_kernels_gpu.py"
+                "::test_attention_kv_split checks the two plans against each other)",
+    "ws": "GroupNorm's persistent scratch, not an input",
+}
+
+
+class _Reads(dict):
+    """Bound arguments that record which keys a reference reads."""
+
+    def __init__(self, p):
+        super().__init__(p)
+        self.read = set()
+
+    def __getitem__(self, k):
+        self.read.add(k)
+        return super().__getitem__(k)
+
+    def get(self, k, default=None):
+        self.read.add(k)
+        return super().get(k, default)
 
 
 # ---------------------------------------------------------------------------------------------------------------------
@@ -463,12 +504,13 @@ def _label(name, p):
     def dims(t):
         return "x".join(str(d) for d in t.shape)
     if name == "linear":
-        flags = [f for f in ("geglu", "silu", "gelu", "quick_gelu") if p[f]]
+        flags = [f for f in ("geglu", "silu", "gelu", "quick_gelu", "relu") if p[f]]
         flags += [f for f in ("residual", "rowbias", "ln", "stats_out") if p[f] is not None]
         flags += [] if p["alpha"] == 1.0 else [f"alpha={p['alpha']:g}"]
         return f"{p['x'].shape[0]}x{p['w'].shape[0]}x{p['x'].shape[1]} tile_n={p['tile_n']} {' '.join(flags)}"
     if name == "conv3x3":
         flags = [f for f in ("rowbias", "residual", "shortcut") if p[f] is not None]
+        flags += ["relu"] if p["relu"] else []
         flags += [] if p["alpha"] == 1.0 else [f"alpha={p['alpha']:g}"]
         return f"{dims(p['x'])}->{p['w_packed'].shape[0]} s{p['stride']} {' '.join(flags)}"
     if name == "attention":
@@ -502,6 +544,7 @@ class Census:
     def __init__(self, ops, check_all=True, plan=None, references=REFERENCES):
         self.ops, self.check_all, self.plan, self.references = ops, check_all, plan, references
         self.rows = {}          # key -> {"op", "shape", "plan", "calls", "checked", "worst"}
+        self.args = {}          # op -> (arguments of its checked calls, the ones its reference read)
 
     def install(self, monkeypatch):
         for name in op_names(self.ops):
@@ -535,13 +578,21 @@ class Census:
             res = orig(*a, **k)
             row["checked"] += 1
             got = p[IN_PLACE[name]] if res is None and name in IN_PLACE else res
-            row["worst"] = max(row["worst"], ref(got, snap))
+            reads = _Reads(snap)
+            row["worst"] = max(row["worst"], ref(got, reads))
+            have, read = self.args.setdefault(name, (set(), set()))
+            have.update(p)
+            read.update(reads.read)
             return res
         wrapped.__wrapped_op__ = orig
         return wrapped
 
     def failures(self):
         return [r for r in self.rows.values() if r["checked"] and not r["worst"] <= 1.0]
+
+    def unread(self):
+        """"op(argument)" for every argument of a checked call that the op's reference never read, except UNREAD."""
+        return sorted(f"{op}({a})" for op, (have, read) in self.args.items() for a in have - read - set(UNREAD))
 
     def report(self, title):
         lines = [f"== census: {title}: {len(self.rows)} keys, {sum(r['calls'] for r in self.rows.values())} calls, "

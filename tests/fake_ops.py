@@ -33,7 +33,7 @@ def _up(t):
 
 
 def linear(x, w, bias=None, *, residual=None, rowbias=None, rows_per_group=0, geglu=False, silu=False, gelu=False,
-           out=None, tile_n=0, ln=None, stats_out=None, quick_gelu=False, alpha=1.0):
+           out=None, tile_n=0, ln=None, stats_out=None, quick_gelu=False, alpha=1.0, relu=False):
     _count[0] += 1
     y = (_up(x) @ _up(w).t()) * alpha
     if ln is not None:
@@ -58,6 +58,8 @@ def linear(x, w, bias=None, *, residual=None, rowbias=None, rows_per_group=0, ge
         y = y * torch.sigmoid(1.702 * y)
     if residual is not None:
         y = y + residual.float()
+    if relu:                                # IH_EPI_RELU: after the residual
+        y = torch.relu(y)
     y = y.to(x.dtype)
     if stats_out is not None:
         yf = y.float()
@@ -103,7 +105,8 @@ def pack_conv3x3_weight(w):
     return w.permute(0, 2, 3, 1).reshape(Cout, 9 * Cin).contiguous()
 
 
-def conv3x3(x, w_packed, bias=None, *, rowbias=None, residual=None, stride=1, out=None, tile_n=0, alpha=1.0, shortcut=None):
+def conv3x3(x, w_packed, bias=None, *, rowbias=None, residual=None, stride=1, out=None, tile_n=0, alpha=1.0, shortcut=None,
+            relu=False):
     _count[0] += 1
     B, H, W, Cin = x.shape
     Cout = w_packed.shape[0]
@@ -122,6 +125,8 @@ def conv3x3(x, w_packed, bias=None, *, rowbias=None, residual=None, stride=1, ou
         y = y + residual.float()
     if sc_term is not None:
         y = y + sc_term
+    if relu:                                # IH_EPI_RELU: after the residual
+        y = torch.relu(y)
     return y.to(x.dtype).contiguous()
 
 

@@ -22,12 +22,14 @@ EXEMPT = {
 
 REGISTRY = {
     "ih_gemm_f16": ["test_kernels_gpu::test_gemm_plain", "test_kernel_edges_gpu::test_gemm_epilogue_matrix"],
-    "ih_gemm_ln_f16": ["test_kernels_gpu::test_gemm_layernorm_fold",
+    "ih_gemm_ln_f16": ["test_kernels_gpu::test_gemm_layernorm_fold", "test_kernel_edges_gpu::test_gemm_epilogue_matrix",
                        "test_kernel_edges_gpu::test_layernorm_fold_accuracy_envelope"],
-    "ih_gemm_scaled_f16": ["test_kernel_edges_gpu::test_gemm_alpha_with_residual_and_gelu"],
+    "ih_gemm_scaled_f16": ["test_kernel_edges_gpu::test_gemm_alpha_with_residual_and_gelu",
+                           "test_kernel_edges_gpu::test_relu_epilogue_propagates_nan_and_inf"],
     "ih_conv2d_f16": ["test_kernels_gpu::test_conv3x3", "test_kernel_edges_gpu::test_conv3x3_rowbias_every_tile"],
     "ih_conv2d_shortcut_f16": ["test_kernels_gpu::test_conv3x3_fused_shortcut"],
-    "ih_conv2d_scaled_f16": ["test_kernel_edges_gpu::test_conv2d_scaled_stride2_residual"],
+    "ih_conv2d_scaled_f16": ["test_kernel_edges_gpu::test_conv2d_scaled_stride2_residual",
+                             "test_kernel_edges_gpu::test_relu_epilogue_propagates_nan_and_inf"],
     "ih_conv2d_down_f16": ["test_img2img_gpu::test_conv_down_kernel"],
     "ih_attention_workspace_bytes": ["test_kernels_gpu::test_attention_kv_split"],
     "ih_attention_ws_f16": ["test_kernels_gpu::test_attention", "test_kernels_gpu::test_attention_kv_split",

@@ -15,6 +15,7 @@ import pytest
 import torch
 import torch.nn.functional as F
 
+from census import stats_ratio
 from fp16_ulps import close_ulps, ulp16
 from imagharmony_b200 import _lib
 from imagharmony_b200._lib import IHError
@@ -240,7 +241,10 @@ TILES = [64, 128, 160, 192, 256]
 @pytest.mark.parametrize("tile_n", TILES)
 def test_gemm_epilogue_matrix(ops, tile_n, M):
     """bias + rowbias (groups not dividing M) + residual + each activation, N clipped in the last tile, strided output
-    and residual views."""
+    and residual views.  ReLU acts after the residual and goes through ih_gemm_f16 itself (ops.linear takes no tile_n
+    or rowbias with it); on the 64- and 160-column tiles also with `stats_out`, whose slots must sum the stored ReLU'd
+    values."""
+    lib = _lib.load()
     K, N = 320, 2 * tile_n + 40
     rpg = 100 if M == 333 else 300
     x, w, b = rnd(M, K, seed=1), rnd(N, K, scale=K ** -0.5, seed=2), rnd(N, seed=3)
@@ -255,6 +259,28 @@ def test_gemm_epilogue_matrix(ops, tile_n, M):
                          silu=act == "silu", gelu=act == "gelu", quick_gelu=act == "quick_gelu")
         assert (ob[:, :8] == 0).all() and (ob[:, 8 + N:] == 0).all(), "wrote outside the output view"
         check(out, fn(base) + res.double(), f"gemm bn{tile_n} M{M} N{N} {act}")
+    ob = torch.zeros(M, N + 16, dtype=torch.float16, device="cuda")
+    rc = lib.ih_gemm_f16(x.data_ptr(), K, w.data_ptr(), b.data_ptr(), rb.data_ptr(), rpg, rb.stride(0), res.data_ptr(),
+                         res.stride(0), ob[:, 8:].data_ptr(), ob.stride(0), M, N, K, ops.EPI_RELU, tile_n, stream())
+    _lib.check(rc, "ih_gemm_f16 relu")
+    assert (ob[:, :8] == 0).all() and (ob[:, 8 + N:] == 0).all(), "wrote outside the output view"
+    relu = torch.relu(base + res.double())
+    assert bool((relu == 0).float().mean() > 0.2), "the ReLU must clip a good share of the outputs"
+    check(ob[:, 8:8 + N], relu, f"gemm bn{tile_n} M{M} N{N} relu")
+    if tile_n in (64, 160):
+        Ns = 640                                              # stats_out: N % 64 == 0, and N % 320 == 0 at 160 columns
+        ws, bs, rs = rnd(Ns, K, scale=K ** -0.5, seed=6), rnd(Ns, seed=7), rnd(M, Ns, seed=8)
+        rbs = rnd(-(-M // rpg), Ns + 8, seed=9)[:, 8:]
+        stats = torch.full((Ns // 64, M, 2), float("nan"), dtype=torch.float32, device="cuda")
+        out = torch.empty(M, Ns, dtype=torch.float16, device="cuda")
+        rc = lib.ih_gemm_ln_f16(x.data_ptr(), K, ws.data_ptr(), bs.data_ptr(), rbs.data_ptr(), rpg, rbs.stride(0),
+                                rs.data_ptr(), Ns, out.data_ptr(), Ns, M, Ns, K, ops.EPI_RELU, tile_n, None, 0, 0.0,
+                                stats.data_ptr(), stream())
+        _lib.check(rc, "ih_gemm_ln_f16 relu stats_out")
+        want = (x.double() @ ws.double().t() + bs.double() + rbs.double()[torch.arange(M, device="cuda") // rpg]
+                + rs.double())
+        check(out, torch.relu(want), f"gemm bn{tile_n} M{M} N{Ns} relu stats_out")
+        assert stats_ratio(stats, out) <= 1.0, f"bn{tile_n} M{M}: slot sums are not those of the stored ReLU'd values"
 
 
 def test_gemm_alpha_with_residual_and_gelu(ops):
@@ -279,13 +305,68 @@ def test_conv3x3_rowbias_every_tile(ops, tile_n, H, W):
 
 
 def test_conv2d_scaled_stride2_residual(ops):
-    B, H, W, Cin, Cout = 2, 30, 46, 128, 192
+    """alpha * conv(x) + bias + residual at stride 2 and four output widths, and with IH_EPI_RELU relu of that sum."""
+    B, H, W, Cin = 2, 30, 46, 128
     x = rnd(B, H, W, Cin, seed=1)
-    w = rnd(Cout, Cin, 3, 3, scale=(9 * Cin) ** -0.5, seed=2)
-    b, res = rnd(Cout, seed=3), rnd(B, H // 2, W // 2, Cout, seed=4)
-    out = ops.conv3x3(x, ops.pack_conv3x3_weight(w), b, stride=2, residual=res, alpha=0.125)
-    conv = F.conv2d(x.double().permute(0, 3, 1, 2), w.double(), None, stride=2, padding=1).permute(0, 2, 3, 1)
-    check(out, 0.125 * conv + b.double() + res.double(), "conv2d_scaled s2 + residual")
+    for Cout in (192, 128, 320, 360):
+        w = rnd(Cout, Cin, 3, 3, scale=(9 * Cin) ** -0.5, seed=2)
+        b, res = rnd(Cout, seed=3), rnd(B, H // 2, W // 2, Cout, seed=4)
+        conv = F.conv2d(x.double().permute(0, 3, 1, 2), w.double(), None, stride=2, padding=1).permute(0, 2, 3, 1)
+        want = 0.125 * conv + b.double() + res.double()
+        assert bool((want < 0).double().mean() > 0.2), "the ReLU must clip a good share of the outputs"
+        for relu in (False, True):
+            out = ops.conv3x3(x, ops.pack_conv3x3_weight(w), b, stride=2, residual=res, alpha=0.125, relu=relu)
+            check(out, torch.relu(want) if relu else want,
+                  f"conv2d_scaled s2 + residual Cout {Cout}{' relu' if relu else ''}")
+
+
+def _nonfinite_like_relu(out, ref, what):
+    """ref: the fp64 reference before the ReLU.  out's NaN, +inf and -inf elements are exactly those of torch.relu(ref)
+    (NaN and +inf pass, -inf becomes 0), and its other elements are within check's bar."""
+    want = torch.relu(ref)
+    for kind in (torch.isnan, torch.isposinf, torch.isneginf):
+        assert torch.equal(kind(out), kind(want)), f"{what}: {kind.__name__} elements differ"
+    fin = torch.isfinite(want)
+    assert bool((~fin).any()) and bool(fin.any())
+    check(out[fin], want[fin], what)
+
+
+def test_relu_epilogue_propagates_nan_and_inf(ops):
+    """IH_EPI_RELU keeps NaN as torch.relu does: NaN rows of the GEMM's A, a NaN input pixel of the conv at a
+    spatial-tile corner, an image border and the batch boundary (its NaN footprint is exactly the 3x3 neighbourhood
+    F.conv2d gives), and NaN / +inf / -inf in the residual."""
+    from test_unet_census_gpu import conv_tile
+    nan, inf = float("nan"), float("inf")
+    # GEMM: NaN rows at both sides of the 128-row tile boundary and in the last row; non-finite residual elements
+    M, N, K = 300, 360, 320
+    x, w, b, res = rnd(M, K, seed=1), rnd(N, K, scale=K ** -0.5, seed=2), rnd(N, seed=3), rnd(M, N, seed=4)
+    x[[0, 127, 128, 299]] = nan
+    x[5, 17] = nan
+    res[40, 7], res[200, 100], res[250, 359], res[251, 0] = nan, inf, -inf, -inf
+    for alpha in (1.0, 0.5):
+        out = ops.linear(x, w, b, residual=res, alpha=alpha, relu=True)
+        ref = alpha * (x.double() @ w.double().t()) + b.double() + res.double()
+        _nonfinite_like_relu(out, ref, f"gemm relu alpha {alpha}")
+    # conv: 24 x 40 outputs run on 16 x 8 spatial tiles; (7, 15) is the bottom-right corner of the first tile
+    B, H, W, C = 2, 24, 40, 64
+    assert conv_tile(H, W) == (16, 8)
+    xc = rnd(B, H, W, C, seed=5)
+    # a tile corner, the top border, image 0's last pixel (next to image 1's first in memory), image 1's left border
+    px = [(0, 7, 15), (0, 0, 20), (0, H - 1, W - 1), (1, 12, 0)]
+    for i, y, xx in px:
+        xc[i, y, xx, (7 * y + xx) % C] = nan
+    wc = rnd(C, C, 3, 3, scale=(9 * C) ** -0.5, seed=6)
+    bc, rc = rnd(C, seed=7), rnd(B, H, W, C, seed=8)
+    rc[1, 3, 30, 5], rc[1, 20, 2, 60], rc[0, 15, 33, 0] = nan, inf, -inf
+    for stride in (1, 2):
+        r = rc if stride == 1 else rnd(B, H // 2, W // 2, C, seed=9)
+        out = ops.conv3x3(xc, ops.pack_conv3x3_weight(wc), bc, residual=r, stride=stride, relu=True)
+        # in fp64 on the host: every output reads exactly its 3 x 3 window there
+        xn = xc.double().cpu().permute(0, 3, 1, 2)
+        conv = F.conv2d(xn, wc.double().cpu(), bc.double().cpu(), stride=stride, padding=1).permute(0, 2, 3, 1)
+        window = F.max_pool2d(torch.isnan(xn).any(1, keepdim=True).double(), 3, stride, 1).bool().permute(0, 2, 3, 1)
+        assert torch.equal(torch.isnan(conv), window.expand_as(conv)), "fp64 reference: NaN beyond the 3x3 windows"
+        _nonfinite_like_relu(out, (conv + r.double().cpu()).cuda(), f"conv relu s{stride}")
 
 
 # ------------------------------------------------------------------------------------------------------------

@@ -1,8 +1,11 @@
 """The census plumbing of test_model_census_gpu.py without a GPU: every public op is classified (a census reference, a
 host helper, or a scheduler step kernel with its own bit-exact test); each model the product runs besides the UNet and
 the untiled VAE decoder runs on its TINY configuration at a non-square size under the recorder, with the stand-in ops
-of tests/fake_ops*.py, every op it calls has a reference and none is beyond its bar; and the new comparators reject an
-output one element of which is 2 fp16 ulps off (1 ulp for the bit-exact ones)."""
+of tests/fake_ops*.py, every op it calls has a reference that reads every argument of the op and none is beyond its
+bar (a reference blind to `relu` fails both ways); the new comparators reject an output one element of which is 2 fp16
+ulps off (1 ulp for the bit-exact ones), and the ReLU-aware ones an output without the ReLU or with it before the
+residual."""
+import inspect
 import math
 import os
 
@@ -187,24 +190,50 @@ def _adapters():
     return run, {"attention_small", "add_bcast", "mean_tokens", "attention", "linear_small", "layernorm"}
 
 
+def _taesd():
+    from test_taesd_cpu import SMALL, _cfg, _pair
+    native, _ = _pair(_cfg(**SMALL), seed=3)
+    z = torch.randn(1, 4, 6, 9, generator=torch.Generator().manual_seed(8)) * 4
+    return lambda: native.decode(z), {"im2col3x3_nchw", "linear", "conv3x3", "upsample2x", "nhwc_to_nchw"}
+
+
 MODELS = {"vae-tiled-decode": _vae_tiled_decode, "vae-tiled-encode": _vae_tiled_encode,
           "controlnet": _controlnet(1), "multi-controlnet": _controlnet(2), "unet9": _unet9,
-          "clip-text": _clip_text, "clip-vision": _clip_vision, "adapters": _adapters}
+          "clip-text": _clip_text, "clip-vision": _clip_vision, "adapters": _adapters, "taesd": _taesd}
+
+
+def _run_model(model, monkeypatch, references=census.REFERENCES):
+    from imagharmony_b200 import ops
+    run, want = MODELS[model]()
+    c = census.Census(ops, references=references).install(monkeypatch)
+    with torch.no_grad():
+        run()
+    return c, want
 
 
 @pytest.mark.parametrize("model", list(MODELS))
 def test_every_op_of_the_model_has_a_reference(stand_ins, monkeypatch, model):
-    from imagharmony_b200 import ops
-    run, want = MODELS[model]()
-    c = census.Census(ops).install(monkeypatch)
-    with torch.no_grad():
-        run()
+    c, want = _run_model(model, monkeypatch)
     print(c.report(model))
     called = {r["op"] for r in c.rows.values()}
     assert want <= called, f"{model}: {sorted(want - called)} ran unchecked"
     assert called <= set(census.REFERENCES)
+    assert not c.unread(), f"{model}: arguments no reference reads: {c.unread()}"
     assert not c.failures(), c.report(model)
     assert all(r["checked"] == r["calls"] for r in c.rows.values())
+    if model == "taesd":              # the ReLU epilogue on the GEMM (conv_in) and on the convs, and the scaled conv_out
+        shapes = {(r["op"], f) for r in c.rows.values() for f in r["shape"].split()}
+        assert {("linear", "relu"), ("conv3x3", "relu"), ("conv3x3", "alpha=2")} <= shapes
+
+
+def test_a_reference_that_ignores_an_argument_fails_the_census(stand_ins, monkeypatch):
+    """ref_linear handed a copy of its arguments with `relu` forced off: the guard names linear(relu), and the ReLU
+    rows of the tiny decoder are beyond their bar."""
+    def blind(res, p):
+        return census.ref_linear(res, {**{k: p[k] for k in p if k != "relu"}, "relu": False})
+    c, _ = _run_model("taesd", monkeypatch, references=dict(census.REFERENCES, linear=blind))
+    assert c.unread() == ["linear(relu)"]
+    assert [r["op"] for r in c.failures()] == ["linear"]
 
 
 # ---------------------------------------------------------------------------------------------------------------------
@@ -263,6 +292,35 @@ def test_new_comparators_reject_two_ulps():
     eps, noise = torch.randn(1, 4, 13, 11, generator=g), torch.randn(4, 4, 13, 11, generator=g).half()
     p = dict(moments=mom, eps=eps, noise=noise, channels=4, scaling_factor=0.13025, sigma=3.0742, out=None)
     _rejects(census.ref_vae_posterior_noise, posterior_noise_ref(mom, eps, noise, 4, 0.13025, 3.0742).contiguous(), p)
+
+
+def _bound(fn, *a, **k):
+    b = inspect.signature(fn).bind(*a, **k)
+    b.apply_defaults()
+    return dict(b.arguments)
+
+
+def test_relu_comparators_reject_a_missing_or_misplaced_relu():
+    """ref_linear / ref_conv3x3 with relu=True (IH_EPI_RELU: relu(alpha * acc + bias + residual)) reject the output
+    without the ReLU, the output with the ReLU before the residual, and one element 2 fp16 ulps off."""
+    g = torch.Generator().manual_seed(20)
+    # linear: conv_in's GEMM form (im2col rows of 64) with a residual and alpha
+    x, w, b, r = _rnd(96, 64, seed=21), _rnd(64, 64, scale=0.125, seed=22), _rnd(64, scale=0.5, seed=23), _rnd(96, 64, seed=24)
+    cases = [(census.ref_linear, fake_ops.linear, (x, w, b), dict(residual=r, alpha=0.5))]
+    # conv3x3: a TinyBlock's third conv (residual) and a stride-2 conv with a residual and alpha
+    for B, H, W, C, stride, alpha in ((2, 6, 10, 64, 1, 1.0), (1, 8, 12, 128, 2, 2.0)):
+        xc = (torch.randn(B, H, W, C, generator=g)).half()
+        wc = (torch.randn(C, 9 * C, generator=g) * (9 * C) ** -0.5).half()
+        bc, rc = (torch.randn(C, generator=g) * 0.5).half(), torch.randn(B, H // stride, W // stride, C, generator=g).half()
+        cases.append((census.ref_conv3x3, fake_ops.conv3x3, (xc, wc, bc), dict(residual=rc, stride=stride, alpha=alpha)))
+    for ref, fn, args, kw in cases:
+        p = _bound(fn, *args, **kw, relu=True)
+        good = fn(*args, **kw, relu=True)
+        assert ref(good, p) <= 1.0
+        assert ref(fn(*args, **kw), p) > 1.0, "no ReLU"
+        pre = fn(*(a.float() for a in args), **dict(kw, residual=None))              # fp32: alpha * acc + bias
+        assert ref((torch.relu(pre) + kw["residual"].float()).half(), p) > 1.0, "ReLU before the residual"
+        assert ref(_nudge(good, 2), p) > 1.0, "2 ulps"
 
 
 def test_bit_exact_comparators_reject_one_ulp():

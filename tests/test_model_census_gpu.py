@@ -12,12 +12,16 @@ decoder (those are test_unet_census_gpu.py), at the sizes they are used at:
 * the 9-channel inpainting UNet at every bucket;
 * both SDXL CLIP text towers at batch 1, 2 and 8, the ViT-bigG vision tower at batch 1 and 4, and the PNS judge's
   resize of decoded candidates to 224^2;
+* the tiny autoencoder decoder (TAESD-XL) at every bucket, batch 1, and at 1024^2 and 832 x 1216 with 4 and 8 images:
+  its ReLU epilogue on conv_in's GEMM and on every block conv, and conv_out at alpha = 2 with Cout padded to 16;
 * ImageProjModel, HarmonyAttention and the IP-Adapter Plus Resampler (also with its position-embedding and mean-pooled
   latent options) at batch 1, 2 and 4, and the SDXL UNet with the 16-token processors of IPAdapterPlusXL.
 
-Random weights, eager forwards; the first call of each distinct key is checked.  `-s` prints one row per key and, at
-the end, how many keys each op got next to the coverage summary of the UNet census."""
+Random weights, eager forwards; the first call of each distinct key is checked (every call of the tiny decoder at
+1024^2, one image).  `-s` prints one row per key and, at the end, how many keys each op got next to the coverage
+summary of the UNet census."""
 import dataclasses
+import time
 import types
 import zlib
 
@@ -144,6 +148,45 @@ def test_vae_tiled_census(ops, sdxl_vae_decoder, sdxl_vae_encoder, monkeypatch, 
         assert min(min(t) for t in dec_tiles) == 8 and min(min(t) for t in enc_tiles) == 64
     print(f"\n[tiles {height}x{width}] decode {sorted(dec_tiles)} encode {sorted(enc_tiles)}")
     _done(c, f"tiled VAE {height}x{width}")
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# tiny autoencoder decoder
+# ---------------------------------------------------------------------------------------------------------------------
+@pytest.fixture(scope="module")
+def taesdxl(ops):  # noqa: F811
+    from imagharmony_b200.config import TAESDXL
+    from imagharmony_b200.taesd import AutoencoderTinyDecoder
+    from imagharmony_b200.weights import random_state_dict, shapes_of
+    from taesd_ref import AutoencoderTinyRef
+    with torch.device("meta"):
+        shapes = shapes_of(AutoencoderTinyRef(TAESDXL))
+    return AutoencoderTinyDecoder.from_state_dict(TAESDXL, random_state_dict(shapes, 14, device="cuda"), device="cuda")
+
+
+TAESD_CASES = [(h, w, 1) for h, w in BUCKETS] + [(h, w, n) for h, w in ((1024, 1024), (832, 1216)) for n in (4, 8)]
+
+
+@pytest.mark.parametrize("height,width,n", TAESD_CASES, ids=[f"{h}x{w}-n{n}" for h, w, n in TAESD_CASES])
+def test_taesd_census(ops, taesdxl, monkeypatch, height, width, n):  # noqa: F811
+    g = _gen("taesd", height, width, n)
+    z = (torch.randn(n, 4, height // 8, width // 8, generator=g) * 3).half().cuda()
+    torch.cuda.reset_peak_memory_stats()
+    t0 = time.perf_counter()
+    c = census.Census(ops, check_all=(height, width, n) == (1024, 1024, 1), plan=plan).install(monkeypatch)
+    img = taesdxl.decode(z)
+    monkeypatch.undo()
+    torch.cuda.synchronize()
+    print(f"\n[taesd census {height}x{width} n={n}] {time.perf_counter() - t0:.1f} s, "
+          f"peak {torch.cuda.max_memory_allocated() / 2 ** 30:.1f} GiB allocated")
+    assert img.shape == (n, 3, height, width)
+    flags = {(r["op"], f) for r in c.rows.values() for f in r["shape"].split()}
+    assert {("linear", "relu"), ("conv3x3", "relu")} <= flags, "the ReLU epilogue must run on the GEMM and the conv"
+    assert any(r["op"] == "conv3x3" and r["shape"].split("->")[1].startswith("16 ") and "alpha=2" in r["shape"]
+               for r in c.rows.values()), "conv_out: Cout padded to 16, alpha = 2"
+    del img, z
+    _done(c, f"TAESD-XL decoder {height}x{width} n={n}")
+    torch.cuda.empty_cache()
 
 
 # ---------------------------------------------------------------------------------------------------------------------

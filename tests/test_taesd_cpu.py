@@ -20,13 +20,10 @@ SMALL = dict(num_decoder_blocks=(1, 2, 1, 1))       # four stages, fewer blocks:
 @pytest.fixture()
 def taesd_ops(monkeypatch):
     import fake_ops
-    import fake_ops_taesd
     import imagharmony_b200.ops as real_ops
     for name in dir(fake_ops):
         if not name.startswith("_") and callable(getattr(fake_ops, name)) and hasattr(real_ops, name):
             monkeypatch.setattr(real_ops, name, getattr(fake_ops, name))
-    for name in fake_ops_taesd.NAMES:
-        monkeypatch.setattr(real_ops, name, getattr(fake_ops_taesd, name))
     yield
 
 

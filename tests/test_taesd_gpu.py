@@ -1,7 +1,7 @@
 """GPU tests of the tiny autoencoder decoder (imagharmony_b200.taesd) and the ReLU epilogue it runs on (IH_EPI_RELU):
 the epilogue against torch fp32 within fp16-ulp bounds at every 64-channel resolution the decoder sees, IH_EPI_NONE
 through the widened ih_conv2d_scaled_f16 bit-equal to the plain conv, the decoder against the fp32 oracle
-(tests/taesd_ref.py) at every SDXL bucket, a launch census of one decode, the PNS judge with the tiny decode and one
+(tests/taesd_ref.py) at every SDXL bucket and with a NaN latent, a launch census of one decode, the PNS judge with the tiny decode and one
 IPAdapterXL.generate to PIL images."""
 import pytest
 import torch
@@ -176,6 +176,23 @@ def test_decoder_matches_oracle_at_sdxl_buckets(H, W):
     for B in (1, 8):
         _check(_taesdxl(), _rnd(B, 4, H // 8, W // 8, scale=3.0, seed=B), f"B{B} {H}x{W}")
         torch.cuda.empty_cache()
+
+
+def test_nan_latent_gives_the_nan_footprint_of_the_oracle():
+    """One NaN in a latent: the native decode's NaN elements are exactly those of the fp32 oracle (ReLU keeps NaN as
+    torch.relu does), the other image of the batch stays NaN-free and everything else is finite."""
+    import copy
+    native, ref32, _ = _taesdxl()
+    z = _rnd(2, 4, 48, 64, scale=3.0, seed=6)
+    z[0, 2, 40, 7] = float("nan")          # footprint: 209 x 209 px at image 0's bottom-left
+    o = native.decode(z)
+    with torch.no_grad():       # on the host: every conv output there reads exactly its 3x3 window
+        r = copy.deepcopy(ref32).cpu().decode(z.float().cpu())
+    nan_o, nan_r = torch.isnan(o).cpu(), torch.isnan(r)
+    print(f"[taesd nan] oracle NaN elements {int(nan_r.sum())}, native {int(nan_o.sum())}")
+    assert 0 < nan_r[0].float().mean() < 0.5 and not nan_r[1].any()
+    assert torch.equal(nan_o, nan_r)
+    assert torch.isfinite(o.cpu()[~nan_r]).all()
 
 
 def test_decode_launch_census():

@@ -1,7 +1,7 @@
 """The census plumbing of test_unet_census_gpu.py without a GPU: the TINY UNet at a non-square latent on the stand-in
-ops (tests/fake_ops.py) runs under the recorder, every op it calls has a reference, an op without one fails the run,
-the dedupe key checks each distinct call once, and the comparators reject an output one element of which is 2 fp16
-ulps off."""
+ops (tests/fake_ops.py) runs under the recorder, every op it calls has a reference that reads every argument of the
+op, an op without one fails the run, the dedupe key checks each distinct call once, and the comparators reject an
+output one element of which is 2 fp16 ulps off."""
 import pytest
 import torch
 
@@ -33,6 +33,7 @@ def test_every_op_of_the_forward_has_a_reference(patched, monkeypatch, check_all
     called = {r["op"] for r in c.rows.values()}
     assert {"linear", "conv3x3", "attention", "groupnorm", "linear_small", "sinusoid", "upsample2x", "im2col3x3_nchw",
             "nhwc_to_nchw"} <= called <= set(census.REFERENCES)
+    assert not c.unread(), f"arguments no reference reads: {c.unread()}"
     assert not c.failures(), c.report("TINY 16x24")
     calls, checked = sum(r["calls"] for r in c.rows.values()), sum(r["checked"] for r in c.rows.values())
     assert checked == (calls if check_all else len(c.rows))
@@ -78,14 +79,14 @@ def _rnd(*shape, scale=1.0, seed=0):
 def test_comparators_reject_two_ulps():
     x, w, b = _rnd(40, 128, seed=1), _rnd(72, 128, scale=128 ** -0.5, seed=2), _rnd(72, seed=3)
     p = dict(x=x, w=w, bias=b, residual=None, rowbias=None, rows_per_group=0, geglu=False, silu=False, gelu=False,
-             out=None, tile_n=0, ln=None, stats_out=None, quick_gelu=False, alpha=1.0)
+             out=None, tile_n=0, ln=None, stats_out=None, quick_gelu=False, alpha=1.0, relu=False)
     good = fake_ops.linear(x, w, b)
     assert census.ref_linear(good, p) <= 1.0
     assert census.ref_linear(_nudge(good), p) > 1.0
 
     xc, wc = _rnd(2, 6, 10, 64, seed=4), _rnd(96, 9 * 64, scale=(9 * 64) ** -0.5, seed=5)
     pc = dict(x=xc, w_packed=wc, bias=None, rowbias=None, residual=None, stride=2, out=None, tile_n=0, alpha=1.0,
-              shortcut=None)
+              shortcut=None, relu=False)
     good = fake_ops.conv3x3(xc, wc, stride=2)
     assert census.ref_conv3x3(good, pc) <= 1.0
     assert census.ref_conv3x3(_nudge(good), pc) > 1.0

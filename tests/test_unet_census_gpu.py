@@ -84,6 +84,7 @@ def sdxl_vae(ops):  # noqa: F811
 def _finish(c, title):
     torch.cuda.synchronize()
     print("\n" + c.report(title))
+    assert not c.unread(), f"{title}: arguments no reference reads: {c.unread()}"
     bad = c.failures()
     assert not bad, f"{title}: {len(bad)} keys beyond their bar:\n" + "\n".join(
         f"{r['op']} {r['shape']} {r['plan']}: err/bar {r['worst']:.3f}" for r in bad)
