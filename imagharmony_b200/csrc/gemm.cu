@@ -232,6 +232,11 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_f16_kernel(const __grid_
     const bool issuer = (ct == 0);
     constexpr int SLABS = S::SLABS;
     constexpr int NBUF = S::STG_SLABS;
+    // Epilogue latency cuts for every tile but the 256-row ones: the LayerNorm statistics of both rows in flight
+    // together, each slab's bias columns loaded ahead of its stores, and the lazy store drain.  The 256-row tiles keep
+    // the plain order: their 128 accumulator registers leave no room for the batched loads, and the GEGLU tile got
+    // slower with the restructured epilogue even where it did not spill (DESIGN section 3).
+    constexpr bool FAST_EPI = BN != 256;
     uint32_t res_par = 0;                             // bit b: parity of res_bar[b]
     int stage = 0;
     uint32_t phase = 0;
@@ -328,7 +333,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_f16_kernel(const __grid_
         }
         // folded LayerNorm: 1 / std of the row from the producer's slabs
         rstd[h] = p.alpha;
-        if (p.ln_stats && orow[h] < p.M) {
+        if (!FAST_EPI && p.ln_stats && orow[h] < p.M) {
           const float2* st = reinterpret_cast<const float2*>(p.ln_stats) + orow[h];   // [slab][row]
           float ssum = 0.f, ssq = 0.f;
           for (int i0 = 0; i0 < p.ln_slabs; i0 += 10) {   // 10 independent loads in flight
@@ -347,10 +352,67 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_f16_kernel(const __grid_
           rstd[h] = p.alpha * rsqrtf(var + p.ln_eps);
         }
       }
+      if constexpr (FAST_EPI) {
+        // the same per-row sums in the same slab order, with the loads of both rows in flight together
+        if (p.ln_stats) {
+          const bool ok[2] = {orow[0] < p.M, orow[1] < p.M};
+          float ssum[2] = {0.f, 0.f}, ssq[2] = {0.f, 0.f};
+          for (int i0 = 0; i0 < p.ln_slabs; i0 += 10) {
+            float2 t[2][10];
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              const float2* st = reinterpret_cast<const float2*>(p.ln_stats) + orow[h];   // [slab][row]
+#pragma unroll
+              for (int i = 0; i < 10; ++i)
+                t[h][i] = (ok[h] && i0 + i < p.ln_slabs) ? __ldg(st + (long long)(i0 + i) * p.M) : make_float2(0.f, 0.f);
+            }
+#pragma unroll
+            for (int h = 0; h < 2; ++h)
+#pragma unroll
+              for (int i = 0; i < 10; ++i) {
+                ssum[h] += t[h][i].x;
+                ssq[h] += t[h][i].y;
+              }
+          }
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            if (ok[h]) {
+              const float ln_mean = ssum[h] * p.ln_inv_c;
+              const float var = fmaxf(ssq[h] * p.ln_inv_c - ln_mean * ln_mean, 0.f);
+              rstd[h] = p.alpha * rsqrtf(var + p.ln_eps);
+            }
+          }
+        }
+        // lazy store drain: without a residual nothing writes staging between the last slab of one tile and the first
+        // slab of the next, so the previous tile's stores are waited for here, after this tile's main loop, rather
+        // than before it; the barrier also keeps the previous tile's statistics readers ahead of the overwrite
+        if (!p.residual && it > 0) {
+          if (issuer) tma_store_wait_read0();
+          named_bar_sync(1, GEMM_MMA_THREADS);
+        }
+      }
 #pragma unroll
       for (int sl = 0; sl < SLABS; ++sl) {
         const int col0 = n0 + sl * 64;
         if (col0 < p.N) {
+          // the slab's bias, gate-bias and row-bias columns, loaded ahead of the waits and stores below: loaded where
+          // they are used, each would wait behind the staging stores before it (one global round trip per 8 columns)
+          __half2 bh[8], gh[8], rh[2][8];
+          if constexpr (FAST_EPI) {
+#pragma unroll
+            for (int j = 0; j < 8; ++j) {
+              const int col = col0 + j * 8 + cq;
+              const bool ok = j < (narrow(sl) ? 4 : 8) && col < p.N;
+              bh[j] = gh[j] = rh[0][j] = rh[1][j] = __float2half2_rn(0.f);
+              if (p.bias && ok) {
+                bh[j] = *reinterpret_cast<const __half2*>(p.bias + col);
+                if (GEGLU) gh[j] = *reinterpret_cast<const __half2*>(p.bias + p.gate_row_off + col);
+              }
+#pragma unroll
+              for (int h = 0; h < 2; ++h)
+                if (rb[h] && ok) rh[h][j] = *reinterpret_cast<const __half2*>(rb[h] + col);
+            }
+          }
           const int buf = sl % NBUF;
           uint8_t* sbuf = stg + buf * S::SLAB_BYTES;
           if (sl >= NBUF) {
@@ -373,7 +435,10 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_f16_kernel(const __grid_
             const int col = n0 + lc;
             const bool col_ok = col < p.N;
             float2 bv = make_float2(0.f, 0.f), bg = make_float2(0.f, 0.f);
-            if (p.bias && col_ok) {
+            if constexpr (FAST_EPI) {
+              bv = __half22float2(bh[j]);   // zero without a bias
+              bg = __half22float2(gh[j]);
+            } else if (p.bias && col_ok) {
               bv = __half22float2(*reinterpret_cast<const __half2*>(p.bias + col));
               if (GEGLU) bg = __half22float2(*reinterpret_cast<const __half2*>(p.bias + p.gate_row_off + col));
             }
@@ -388,7 +453,8 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_f16_kernel(const __grid_
                 x1v *= gelu_erf_f(fmaf(rstd[h], acc[4 * (i + G) + 2 * h + 1], bg.y));
               }
               if (rb[h] && col_ok) {
-                const float2 f = __half22float2(*reinterpret_cast<const __half2*>(rb[h] + col));
+                const float2 f = FAST_EPI ? __half22float2(rh[h][j])
+                                          : __half22float2(*reinterpret_cast<const __half2*>(rb[h] + col));
                 x0v += f.x;
                 x1v += f.y;
               }
@@ -472,9 +538,12 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_f16_kernel(const __grid_
       }
       // the staging buffers may be rewritten (next tile) / must stay valid (kernel end) until the bulk stores have read
       // them; global visibility is given by kernel completion (the next kernel's griddepcontrol.wait / stream order)
-      if (issuer) tma_store_wait_read0();
-      named_bar_sync(1, GEMM_MMA_THREADS);          // statistics readers are done with the staging buffers too
+      if (!FAST_EPI || p.residual) {
+        if (issuer) tma_store_wait_read0();
+        named_bar_sync(1, GEMM_MMA_THREADS);        // statistics readers are done with the staging buffers too
+      }
     }
+    if (FAST_EPI && issuer) tma_store_wait_read0();   // lazy drain: the last tile's stores read out before exit
   }
   __syncthreads();
   if (threadIdx.x == 0) stamp(8);
@@ -570,21 +639,39 @@ static int pick_bn(long long m_tiles, int N, int num_kb, bool allow160) {
 static int dispatch(const TmapSet4& amaps, const OutView& ov, const void* w, int ldw_rows, long long K, GemmParams& p,
                     int m_tiles, int geglu, int force_bn, cudaStream_t stream) {
   // tile_n: 0 = the cost model's choice, 64 / 128 / 160 / 192 / 256 force that tile width; 512 and 384 (the widest
-  // tiles a caller may ask for) are the 256- and 192-column tiles
+  // tiles a caller may ask for) are the 256- and 192-column tiles.  For GEGLU the width counts the B tile's rows
+  // (value and gate halves: 128 / 192 / 256, i.e. 64 / 96 / 128 outputs per tile).
   if (force_bn == 512) force_bn = 256;
   if (force_bn == 384) force_bn = 192;
-  const bool allow160 = !p.stats_out || p.N % 320 == 0;
-  const int bn = geglu ? 256 : (force_bn > 0 ? force_bn : pick_bn(m_tiles, p.N, p.num_kb, allow160));
-  IH_CHECK(bn != 160 || allow160, IH_ERR_SHAPE, "ih_gemm_ln_f16: 160-column tiles with stats_out need N %% 320 == 0");
+  int bn;
+  if (geglu) {
+    // 256 unless asked: it is the fastest GEGLU tile at the UNet's shapes (tools/ab_probe.py geglu, DESIGN section 3)
+    bn = force_bn > 0 ? force_bn : 256;
+    IH_CHECK(bn == 128 || bn == 192 || bn == 256, IH_ERR_ARG, "ih_gemm_f16: GEGLU tile_n must be 128, 192 or 256 (got %d)",
+             bn);
+    // the 96-output tile would split a 64-column statistics slot between two tiles
+    IH_CHECK(bn != 192 || !p.stats_out, IH_ERR_SHAPE, "ih_gemm_ln_f16: the 192-row GEGLU tile cannot write stats_out");
+  } else {
+    const bool allow160 = !p.stats_out || p.N % 320 == 0;
+    bn = force_bn > 0 ? force_bn : pick_bn(m_tiles, p.N, p.num_kb, allow160);
+    IH_CHECK(bn != 160 || allow160, IH_ERR_SHAPE, "ih_gemm_ln_f16: 160-column tiles with stats_out need N %% 320 == 0");
+  }
+  const int bn_out = geglu ? bn / 2 : bn;
   CUtensorMap bmap;
   const uint64_t bdims[2] = {(uint64_t)K, (uint64_t)ldw_rows};
   const uint64_t bstr[1] = {(uint64_t)K * 2};
-  const uint32_t bbox[2] = {(uint32_t)BK, (uint32_t)(geglu ? 128 : bn)};
+  const uint32_t bbox[2] = {(uint32_t)BK, (uint32_t)bn_out};   // GEGLU: the value and the gate half are loaded apart
   int rc = get_tmap_f16(&bmap, w, 2, bdims, bstr, bbox);
   if (rc) return rc;
   OutMaps om;
-  if ((rc = out_maps(ov, !geglu && bn == 160, om))) return rc;
-  if (geglu) return launch_gemm<256, 4, true>(amaps, bmap, om, p, m_tiles, stream);
+  if ((rc = out_maps(ov, bn_out % 64 == 32, om))) return rc;
+  if (geglu) {
+    switch (bn) {
+      case 256: return launch_gemm<256, 4, true>(amaps, bmap, om, p, m_tiles, stream);
+      case 192: return launch_gemm<192, 5, true>(amaps, bmap, om, p, m_tiles, stream);
+      default: return launch_gemm<128, 6, true>(amaps, bmap, om, p, m_tiles, stream);
+    }
+  }
   switch (bn) {
     case 256: return launch_gemm<256, 4, false>(amaps, bmap, om, p, m_tiles, stream);
     case 192: return launch_gemm<192, 4, false>(amaps, bmap, om, p, m_tiles, stream);

@@ -56,6 +56,8 @@ def linear(x: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor] = None
     """out = epi(x @ w.T + bias + rowbias[row // rows_per_group]) + residual ; x [M,K], w [N,K] (nn.Linear layout).
     `relu=True`: out = relu(alpha * x @ w.T + bias + residual), the ReLU after the residual (IH_EPI_RELU); it takes no
     other activation, rowbias, ln, stats_out or tile_n.
+    `tile_n`: 0 lets the library choose; else 64 / 128 / 160 / 192 / 256 output columns per tile, or with `geglu`
+    128 / 192 / 256 weight rows per tile (value and gate halves: 64 / 96 / 128 outputs).
 
     LayerNorm folding: `stats_out` (float32 [ceil(N/64), M, 2]) receives per-row (sum, sumsq) of the stored values as
     partial sums whose total over slots is the row's; `ln=(stats, eps)` makes this GEMM consume RAW rows `x` with the gamma-scaled, row-centred weight and

@@ -41,7 +41,8 @@ void ih_launch_count_reset(void);
  * Replaces nn.Linear: attention_processor.py:292,299-300,320 (AttnProcessor2_0 to_q/to_k/to_v/to_out),
  * :396,410-411,432-433,453 (IPAttnProcessor2_0 incl. to_k_ip/to_v_ip), and the diffusers proj_in/proj_out/FF/1x1
  * conv layers reached through custom_pipelines.py:338-345.  tile_n: 0 = auto, else 64/128/160/192/256 (384 and
- * 512 mean 192 and 256). */
+ * 512 mean 192 and 256).  With IH_EPI_GEGLU tile_n counts the weight rows of a tile, value and gate halves together:
+ * 128/192/256 (64/96/128 outputs per tile); the 192-row GEGLU tile cannot write stats_out. */
 int ih_gemm_f16(const void* a, long long lda, const void* w, const void* bias, const void* rowbias,
                 int rows_per_group, long long ld_rowbias, const void* residual, long long ldr, void* out,
                 long long ldo, int M, int N, int K, int epilogue, int tile_n, void* stream);

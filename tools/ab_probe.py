@@ -1,5 +1,6 @@
 """Small A/B probes (graph-timed, same process => same thermal state).  `python tools/ab_probe.py tile` measures the
-main-loop cost per 64-deep k-block of the 128xBN tiles with every SM busy (calibrates pick_bn in gemm.cu)."""
+main-loop cost per 64-deep k-block of the 128xBN tiles, plain and GEGLU, with every SM busy (calibrates the tile
+costs in gemm.cu)."""
 import os
 import sys
 
@@ -25,6 +26,37 @@ def tile_costs():
               f"fixed {(ts[0] - 20 * per_kb)*1e6:.1f} us", flush=True)
 
 
+def geglu_tile_costs():
+    """The same for GEGLU (value + gate halves in one B tile of `bn` rows, bn / 2 outputs), LayerNorm-folded with bias
+    as in the UNet's feed-forward: one round with (nearly) every SM busy."""
+    M = 2048
+    cols = torch.cuda.get_device_properties(0).multi_processor_count // 16
+    for bn in (128, 192, 256):
+        N = 2 * cols * (bn // 2)
+        ts = []
+        for K in (1280, 5120):
+            x, w, b = r(M, K), r(N, K, scale=K ** -0.5), r(N)
+            st = torch.rand((K // 64, M, 2), device="cuda")
+            st[..., 1] += 64.0
+            ts.append(timeit(lambda: ops.linear(x, w, b, geglu=True, ln=(st, 1e-5), tile_n=bn)))
+        per_kb = (ts[1] - ts[0]) / ((5120 - 1280) / 64)
+        print(f"GEGLU 128x{bn}: K=1280 {ts[0]*1e6:.1f} us, K=5120 {ts[1]*1e6:.1f} us -> {per_kb*1e6:.3f} us per k-block, "
+              f"fixed {(ts[0] - 20 * per_kb)*1e6:.1f} us", flush=True)
+
+
+def geglu_shapes():
+    """The UNet's LayerNorm-folded GEGLU launches at 1024^2, batch 2 (level 2: M 2048, K 1280; level 1: M 8192, K 640)
+    on every GEGLU tile and on the library's choice."""
+    for (M, K) in [(2048, 1280), (8192, 640)]:
+        N = 8 * K
+        x, w, b = r(M, K), r(N, K, scale=K ** -0.5), r(N)
+        st = torch.rand((K // 64, M, 2), device="cuda")
+        st[..., 1] += 64.0
+        for bn in (128, 192, 256, 0):
+            t = timeit(lambda: ops.linear(x, w, b, geglu=True, ln=(st, 1e-5), tile_n=bn))
+            print(f"GEGLU M{M} N{N} K{K} bn{bn}: {t*1e6:.1f} us", flush=True)
+
+
 def shapes():
     for (M, N, K, geglu, tn) in [(2048, 1280, 1280, False, 0), (2048, 3840, 1280, False, 0), (8192, 1920, 640, False, 0),
                                  (2048, 10240, 1280, True, 0), (2048, 1280, 5120, False, 0)]:
@@ -44,5 +76,8 @@ def shapes():
 if __name__ == "__main__":
     if len(sys.argv) > 1 and sys.argv[1] == "tile":
         tile_costs()
+        geglu_tile_costs()
+    elif len(sys.argv) > 1 and sys.argv[1] == "geglu":
+        geglu_shapes()
     else:
         shapes()
