@@ -550,6 +550,260 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_f16_kernel(const __grid_
 }
 
 // ------------------------------------------------------------------------------------------------
+// Ping-pong GEMM for the LayerNorm-folded GEGLU-in and q|k|v launches (plain GEMM mode; bias, LN fold and GEGLU only).
+//
+// In gemm_f16_kernel both MMA warpgroups share every tile, so the tensor cores idle through each epilogue; with the
+// 10-20 k-blocks of a transformer GEMM that is about half of a multi-round launch.  Here each MMA warpgroup owns WHOLE
+// 128 x 128 tiles (two m64n128 blocks, 128 accumulator registers): CTA c walks tiles c, c + grid, ... and hands them to
+// warpgroup 1, 2, 1, 2, ..., so one warpgroup's epilogue runs under the other's main loop.  Each MMA warpgroup has its
+// own stage ring, filled by its own producer warp (warp 0 for warpgroup 1, warp 2 for warpgroup 2): every ring has
+// one producer and one consumer, as in gemm_f16_kernel.  The main loops take turns through two named barriers (as
+// CUTLASS's ping-pong does), so that the two warpgroups' epilogues do not fall together.
+// The epilogue is gemm_f16_kernel's expressions in the same order -- the LayerNorm statistics summed in slab order,
+// fmaf(rstd, acc, bias), gelu_erf_f on the gate, pack_half2 -- so the outputs are bitwise equal to it.  The LayerNorm
+// statistics of the tile's rows and its bias columns are fetched during the main loop.
+// ------------------------------------------------------------------------------------------------
+constexpr int PP_STAGES = 3;      // per MMA warpgroup
+constexpr int PP_BN = 128;        // B-tile rows (GEGLU: 64 value + 64 gate rows, 64 outputs)
+// named barriers (gemm_f16_kernel uses 1 and 2): 3 + wg lets warpgroup wg start its next main loop, 5 + wg is its
+// epilogue barrier
+constexpr int PP_BAR_ORDER = 3;
+constexpr int PP_BAR_EPI = 5;
+
+struct PpOperands {   // one MMA warpgroup's epilogue operands of its current tile
+  float rstd[BM];      // alpha (LayerNorm folded: alpha / std) of every tile row
+  __half2 bias[64];    // bias pairs of the tile's columns (GEGLU: 32 value pairs, then 32 gate pairs)
+};
+
+template <bool GEGLU>
+struct PpSmem {
+  static constexpr int STAGE_BYTES = A_STAGE_BYTES + PP_BN * BK * 2;   // 32 KiB
+  static constexpr int RING_BYTES = PP_STAGES * STAGE_BYTES;
+  static constexpr int TILE_BYTES = 2 * RING_BYTES;
+  static constexpr int BN_OUT = GEGLU ? PP_BN / 2 : PP_BN;
+  static constexpr int SLABS = BN_OUT / 64;
+  static constexpr int SLAB_BYTES = BM * 64 * 2;
+  static constexpr int STG_BYTES = 2 * SLAB_BYTES;   // one staging slab per MMA warpgroup
+  static constexpr int BAR_BYTES = 128;              // full and empty barriers of both rings
+  static constexpr int TOTAL = TILE_BYTES + STG_BYTES + BAR_BYTES + 2 * sizeof(PpOperands) + 1024;   // + alignment slack
+  static_assert(4 * PP_STAGES * 8 <= BAR_BYTES, "ping-pong GEMM barriers");
+  static_assert(TOTAL <= GemmSmem<128, 6, false>::SMEM_LIMIT, "ping-pong GEMM shared-memory budget exceeded");
+};
+
+template <bool GEGLU>
+__global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_pp_f16_kernel(const __grid_constant__ CUtensorMap amap,
+                                                                       const __grid_constant__ CUtensorMap bmap,
+                                                                       const __grid_constant__ CUtensorMap omap,
+                                                                       const GemmParams p) {
+  using S = PpSmem<GEGLU>;
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint8_t* stg = smem + S::TILE_BYTES;
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + S::TILE_BYTES + S::STG_BYTES);   // [ring][stage]
+  uint64_t* empty_bar = full_bar + 2 * PP_STAGES;
+
+  const int warp = threadIdx.x >> 5;
+  const int lane = threadIdx.x & 31;
+  auto stamp = [&](int slot) {
+    if (p.trace && blockIdx.x == 0) {
+      unsigned long long t;
+      asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+      p.trace[slot] = t;
+    }
+  };
+  if (threadIdx.x == 0) stamp(0);
+  constexpr int BN_OUT = S::BN_OUT;
+  const int n_tiles = (p.N + BN_OUT - 1) / BN_OUT;
+  const int num_tiles = n_tiles * p.m_tiles;
+
+  if (threadIdx.x == 0) {
+    tma_prefetch_desc(&amap);
+    tma_prefetch_desc(&bmap);
+    tma_prefetch_desc(&omap);
+    for (int s = 0; s < 2 * PP_STAGES; ++s) {
+      mbar_init(&full_bar[s], 1);
+      mbar_init(&empty_bar[s], 4);   // lane 0 of the four warps of the ring's MMA warpgroup
+    }
+    fence_barrier_init();
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) stamp(1);
+  pdl_launch_dependents();
+  pdl_wait();
+  if (threadIdx.x == 0) stamp(2);
+
+  if (warp < 4) {
+    // ------------------------------ producer warpgroup ------------------------------
+    setmaxnreg_dec<40>();
+    if (warp == 0 || warp == 2) {
+      // the ring of MMA warpgroup `ring`, which takes every other tile of the CTA
+      const int ring = warp >> 1;
+      uint8_t* ring_smem = smem + ring * S::RING_BYTES;
+      uint64_t* ring_full = full_bar + ring * PP_STAGES;
+      uint64_t* ring_empty = empty_bar + ring * PP_STAGES;
+      int stage = 0;
+      uint32_t phase = 0;
+      for (int tile = blockIdx.x + ring * gridDim.x; tile < num_tiles; tile += 2 * gridDim.x) {
+        const int n0 = (tile % n_tiles) * BN_OUT;
+        const int m0 = (tile / n_tiles) * BM;
+        for (int kb = 0; kb < p.num_kb; ++kb) {
+          mbar_wait(&ring_empty[stage], phase ^ 1);
+          uint8_t* sA = ring_smem + stage * S::STAGE_BYTES;
+          uint8_t* sB = sA + A_STAGE_BYTES;
+          if (elect_one()) {
+            mbar_arrive_expect_tx(&ring_full[stage], S::STAGE_BYTES);
+            tma_load_2d(sA, &amap, &ring_full[stage], kb * BK, m0);
+            tma_load_2d(sB, &bmap, &ring_full[stage], kb * BK, n0);
+            if (GEGLU) tma_load_2d(sB + (PP_BN / 2) * BK * 2, &bmap, &ring_full[stage], kb * BK, p.gate_row_off + n0);
+          }
+          __syncwarp();
+          if (++stage == PP_STAGES) {
+            stage = 0;
+            phase ^= 1;
+          }
+        }
+      }
+    } else if (warp == 1 && lane == 0 && p.pf_ptr) {
+      constexpr unsigned long long CH = 16384;
+      const unsigned long long per = ((p.pf_bytes / gridDim.x) + CH - 1) / CH * CH;
+      unsigned long long off = per * blockIdx.x;
+      const unsigned long long end = off + per < p.pf_bytes ? off + per : p.pf_bytes;
+      for (; off < end; off += CH) {
+        const unsigned long long n = end - off < CH ? ((end - off) & ~15ull) : CH;
+        if (n) l2_prefetch_bulk(p.pf_ptr + off, (uint32_t)n);
+      }
+    }
+  } else {
+    // ------------------------------ MMA + epilogue warpgroups, one whole tile each ------------------------------
+    setmaxnreg_inc<232>();
+    const int wg = (threadIdx.x >> 7) - 1;
+    const int rw = ((warp & 3) << 4) + (lane >> 2);   // my accumulator rows: 64 mb + rw + 8 h
+    const int cq = (lane & 3) << 1;                   // my column pair inside every 8-column group
+    const int t = threadIdx.x & 127;
+    const bool issuer = t == 0;
+    uint8_t* my_stg = stg + wg * S::SLAB_BYTES;
+    uint8_t* ring_smem = smem + wg * S::RING_BYTES;
+    uint64_t* ring_full = full_bar + wg * PP_STAGES;
+    uint64_t* ring_empty = empty_bar + wg * PP_STAGES;
+    PpOperands* my_ops = reinterpret_cast<PpOperands*>(smem + S::TILE_BYTES + S::STG_BYTES + S::BAR_BYTES) + wg;
+    const int ln_n = p.ln_stats ? p.ln_slabs : 0;
+    const float2* ln_st = reinterpret_cast<const float2*>(p.ln_stats);   // [slab][row]
+    int stage = 0;
+    uint32_t phase = 0;
+    float acc[2][PP_BN / 2];
+    int j = wg;   // index of the tile among this CTA's tiles
+    for (int tile = blockIdx.x + wg * gridDim.x; tile < num_tiles; tile += 2 * gridDim.x, j += 2) {
+      const int n0 = (tile % n_tiles) * BN_OUT;
+      const int m_tile = tile / n_tiles;
+      // epilogue operands, fetched behind the main loop and handed over in shared memory: the warpgroup's thread t
+      // sums the LayerNorm statistics of tile row t, the load of slab kb + 1 in flight behind k-block kb, and threads
+      // 0..63 fetch one bias pair each (GEGLU: 32 value pairs, then 32 gate pairs)
+      const long long ln_row = (long long)m_tile * BM + t;
+      const bool ln_ok = ln_row < p.M;
+      auto ln_load = [&](int s) {
+        return ln_ok && s < ln_n ? __ldg(ln_st + (long long)s * p.M + ln_row) : make_float2(0.f, 0.f);
+      };
+      float ssum = 0.f, ssq = 0.f;
+      float2 st = ln_load(0);
+      auto ln_step = [&](int s) {   // add slab s (in st) to the row's sums, then fetch slab s + 1
+        ssum += st.x;
+        ssq += st.y;
+        st = ln_load(s + 1);
+      };
+      __half2 bias_pair = __float2half2_rn(0.f);
+      {
+        const int col = n0 + 2 * (GEGLU ? (t & 31) : t);
+        if (t < 64 && p.bias && col < p.N)
+          bias_pair = *reinterpret_cast<const __half2*>(p.bias + ((GEGLU && t >= 32) ? p.gate_row_off : 0) + col);
+      }
+
+      // ---- main loop, after the other warpgroup has issued all of the CTA's previous tile
+      if (j > 0) named_bar_sync(PP_BAR_ORDER + wg, 256);
+      int prev = -1;
+      for (int kb = 0; kb < p.num_kb; ++kb) {
+        mbar_wait(&ring_full[stage], phase);
+        if (issuer && j == 0 && kb == 0) stamp(3);
+        const uint32_t a_addr = smem_u32(ring_smem + stage * S::STAGE_BYTES);
+        const uint64_t a_desc0 = wgmma_desc_sw128(a_addr);
+        const uint64_t a_desc1 = wgmma_desc_sw128(a_addr + 64 * 128);
+        const uint64_t b_desc = wgmma_desc_sw128(a_addr + A_STAGE_BYTES);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < BK / 16; ++k) {
+          wgmma_ss<PP_BN>(acc[0], a_desc0 + 2 * k, b_desc + 2 * k, (kb | k) != 0 ? 1 : 0);
+          wgmma_ss<PP_BN>(acc[1], a_desc1 + 2 * k, b_desc + 2 * k, (kb | k) != 0 ? 1 : 0);
+        }
+        wgmma_commit();
+        if (prev >= 0) {
+          wgmma_wait<1>();
+          if (lane == 0) mbar_arrive(&ring_empty[prev]);
+        }
+        prev = stage;
+        if (++stage == PP_STAGES) {
+          stage = 0;
+          phase ^= 1;
+        }
+        if (kb == 0 && t < 64) my_ops->bias[t] = bias_pair;
+        if (kb < ln_n) ln_step(kb);
+      }
+      // this tile's MMAs are issued: the other warpgroup may start the CTA's next tile
+      if (tile + gridDim.x < num_tiles) named_bar_arrive(PP_BAR_ORDER + (wg ^ 1), 256);
+      wgmma_wait<0>();
+      fence_regs(acc[0]);
+      fence_regs(acc[1]);
+      if (lane == 0) mbar_arrive(&ring_empty[prev]);
+      if (issuer) stamp(4 + (j < 3 ? j : 3));
+
+      // ---- epilogue: the same expressions in the same order as gemm_f16_kernel
+      for (int s = p.num_kb; s < ln_n; ++s) ln_step(s);   // statistics slabs past the k-blocks
+      float rstd = p.alpha;
+      if (ln_n && ln_ok) {
+        const float ln_mean = ssum * p.ln_inv_c;
+        const float var = fmaxf(ssq * p.ln_inv_c - ln_mean * ln_mean, 0.f);
+        rstd = p.alpha * rsqrtf(var + p.ln_eps);
+      }
+      my_ops->rstd[t] = rstd;
+      const uint32_t stg_row = smem_u32(my_stg) + rw * 128 + cq * 2;   // rows 64 mb + rw + 8 h: (row & 7) == lane >> 2
+      const uint32_t ops_bias = smem_u32(my_ops->bias) + (cq >> 1) * 4;
+#pragma unroll
+      for (int sl = 0; sl < S::SLABS; ++sl) {
+        // the staging slab is rewritten: the stores of my previous slab must have read it out; the first barrier of
+        // the tile also publishes the operands above
+        if (issuer) tma_store_wait_read0();
+        named_bar_sync(PP_BAR_EPI + wg, 128);
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+          const int mb = q >> 1, h = q & 1;
+          const float rs = __uint_as_float(ld_shared_u32(smem_u32(my_ops->rstd) + (64 * mb + rw + 8 * h) * 4));
+#pragma unroll
+          for (int c = 0; c < 8; ++c) {
+            const int i = sl * 8 + c;   // accumulator 8-column group; its bias pair is 4 i + cq / 2 (GEGLU gate: + 32)
+            const float2 bv = unpack_half2(ld_shared_u32(ops_bias + 16 * i));
+            float x0v = fmaf(rs, acc[mb][4 * i + 2 * h], bv.x);
+            float x1v = fmaf(rs, acc[mb][4 * i + 2 * h + 1], bv.y);
+            if (GEGLU) {
+              const float2 bg = unpack_half2(ld_shared_u32(ops_bias + 128 + 16 * i));
+              x0v *= gelu_erf_f(fmaf(rs, acc[mb][4 * (i + 8) + 2 * h], bg.x));
+              x1v *= gelu_erf_f(fmaf(rs, acc[mb][4 * (i + 8) + 2 * h + 1], bg.y));
+            }
+            st_shared_u32(stg_row + (64 * mb + 8 * h) * 128 + ((c ^ (lane >> 2)) << 4), pack_half2(x0v, x1v));
+          }
+        }
+        fence_proxy_async_smem();
+        named_bar_sync(PP_BAR_EPI + wg, 128);   // the slab is complete in staging
+        if (issuer) {
+          if (n0 + sl * 64 < p.N) tma_store_2d(&omap, my_stg, n0 + sl * 64, m_tile * BM);
+          tma_store_commit();
+        }
+      }
+    }
+    if (issuer) tma_store_wait_read0();   // staging stays valid until the last stores have read it
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) stamp(8);
+}
+
+// ------------------------------------------------------------------------------------------------
 // host side
 // ------------------------------------------------------------------------------------------------
 // The output (and residual) tensor as the epilogue's TMA stores and loads see it: 64-column slabs with a 128-byte
@@ -602,11 +856,28 @@ static int launch_gemm(const TmapSet4& amaps, const CUtensorMap& bmap, const Out
   return 0;
 }
 
+template <bool GEGLU>
+static int launch_gemm_pp(const TmapSet4& amaps, const CUtensorMap& bmap, const OutMaps& om, GemmParams& p, int m_tiles,
+                          cudaStream_t stream) {
+  using S = PpSmem<GEGLU>;
+  static bool configured = false;
+  auto kern = gemm_pp_f16_kernel<GEGLU>;
+  if (!configured) {
+    IH_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, S::TOTAL));
+    configured = true;
+  }
+  p.m_tiles = m_tiles;
+  const long long tiles = (long long)((p.N + S::BN_OUT - 1) / S::BN_OUT) * m_tiles;
+  const int grid = (int)(tiles < num_sms() ? tiles : num_sms());
+  IH_CUDA(launch_kernel(kern, dim3(grid), dim3(GEMM_THREADS), (size_t)(S::TOTAL), stream, amaps.m[0], bmap, om.o, p));
+  return 0;
+}
+
 // Cost model for the persistent kernel (one CTA per SM): a launch takes `rounds` tiles per SM one after the other,
 // each costing num_kb k-blocks of main loop plus a fixed part (pipeline fill, epilogue, store drain).  Padded columns of
 // a partially filled last N tile cost as much as real ones.  160-column tiles need N % 320 == 0 when the launch writes
-// row statistics (see the epilogue).
-static int pick_bn(long long m_tiles, int N, int num_kb, bool allow160) {
+// row statistics (see the epilogue).  `cost` receives the chosen tile's estimate (not set for the 64-column tile).
+static int pick_bn(long long m_tiles, int N, int num_kb, bool allow160, double* cost = nullptr) {
   if (N <= 64) return 64;
   const int sms = num_sms();
   // 128x64 tiles for launches that cannot fill the SMs with wider ones (e.g. the 1280-channel level of a 512^2 edit,
@@ -633,7 +904,31 @@ static int pick_bn(long long m_tiles, int N, int num_kb, bool allow160) {
       best_bn = bn;
     }
   }
+  if (cost) *cost = best;
   return best_bn;
+}
+
+// Whether the ping-pong kernel beats gemm_f16_kernel's choice.  Both are linear models of the launch time in us, fitted
+// to tools/ab_probe.py pp (the LayerNorm-folded q|k|v and GEGLU launches of the SDXL base and refiner UNets at 512^2 -
+// 1024^2, 1 and 4 images; H100 80GB HBM3 at a 700 W power limit; DESIGN section 3), in the rounds R of tiles per SM:
+//   ping-pong, plain  0.461 R kb + 0.898 R + 3.21     (128 x 128 tiles; within 8 % of the table)
+//   ping-pong, GEGLU  0.650 R kb - 1.03 R + 5.81      (64 outputs per tile; within 13 %)
+//   old, plain        0.627 (pick_bn's cost) + 1.33   (within 17 %)
+//   old, GEGLU        0.969 R kb + 6.95 R - 1.28      (the 256-row tile, 128 outputs; within 7 %)
+// The ping-pong GEGLU tile spends more per k-block (its epilogue is as long as the main loop) and nothing per round, so
+// it wins up to about 20 k-blocks (K = 1280).  The GEGLU per-k-block coefficient is the least-squares one lowered from
+// 0.674 to 0.650, which minimises the time lost to wrong picks over the table (12.6 us in all, at K = 1536).
+static bool pick_pp(long long m_tiles, int N, int num_kb, bool geglu) {
+  const int sms = num_sms();
+  auto rounds = [&](int cols) { return (double)((m_tiles * ((N + cols - 1) / cols) + sms - 1) / sms); };
+  if (geglu) {
+    const double pp = rounds(64) * (0.650 * num_kb - 1.03) + 5.81;
+    const double old = rounds(128) * (0.969 * num_kb + 6.95) - 1.28;
+    return pp < old;
+  }
+  double cost;
+  if (pick_bn(m_tiles, N, num_kb, true, &cost) == 64) return false;   // one round of narrow tiles: not in the table
+  return rounds(128) * (0.461 * num_kb + 0.898) + 3.21 < 0.627 * cost + 1.33;
 }
 
 static int dispatch(const TmapSet4& amaps, const OutView& ov, const void* w, int ldw_rows, long long K, GemmParams& p,
@@ -643,15 +938,21 @@ static int dispatch(const TmapSet4& amaps, const OutView& ov, const void* w, int
   // (value and gate halves: 128 / 192 / 256, i.e. 64 / 96 / 128 outputs per tile).
   if (force_bn == 512) force_bn = 256;
   if (force_bn == 384) force_bn = 192;
-  int bn;
-  if (geglu) {
-    // 256 unless asked: it is the fastest GEGLU tile at the UNet's shapes (tools/ab_probe.py geglu, DESIGN section 3)
+  // the ping-pong kernel: bias, LayerNorm fold and GEGLU only (the q|k|v and GEGLU-in launches of a transformer block)
+  const bool pp_ok = p.mode == 0 && !p.residual && !p.rowbias && !p.stats_out && p.act == 0 && !p.relu && p.alpha == 1.f;
+  IH_CHECK(force_bn != IH_TILE_PINGPONG || pp_ok, IH_ERR_ARG,
+           "ih_gemm_f16: tile_n = IH_TILE_PINGPONG supports bias, LayerNorm folding and GEGLU only");
+  const bool pp = force_bn == IH_TILE_PINGPONG || (force_bn == 0 && pp_ok && pick_pp(m_tiles, p.N, p.num_kb, geglu));
+  int bn = PP_BN;   // the ping-pong tile: 128 B-tile rows
+  if (!pp && geglu) {
+    // 256 unless asked: it is the fastest GEGLU tile of this kernel at the UNet's shapes (tools/ab_probe.py geglu,
+    // DESIGN section 3)
     bn = force_bn > 0 ? force_bn : 256;
     IH_CHECK(bn == 128 || bn == 192 || bn == 256, IH_ERR_ARG, "ih_gemm_f16: GEGLU tile_n must be 128, 192 or 256 (got %d)",
              bn);
     // the 96-output tile would split a 64-column statistics slot between two tiles
     IH_CHECK(bn != 192 || !p.stats_out, IH_ERR_SHAPE, "ih_gemm_ln_f16: the 192-row GEGLU tile cannot write stats_out");
-  } else {
+  } else if (!pp) {
     const bool allow160 = !p.stats_out || p.N % 320 == 0;
     bn = force_bn > 0 ? force_bn : pick_bn(m_tiles, p.N, p.num_kb, allow160);
     IH_CHECK(bn != 160 || allow160, IH_ERR_SHAPE, "ih_gemm_ln_f16: 160-column tiles with stats_out need N %% 320 == 0");
@@ -665,6 +966,8 @@ static int dispatch(const TmapSet4& amaps, const OutView& ov, const void* w, int
   if (rc) return rc;
   OutMaps om;
   if ((rc = out_maps(ov, bn_out % 64 == 32, om))) return rc;
+  if (pp) return geglu ? launch_gemm_pp<true>(amaps, bmap, om, p, m_tiles, stream)
+                       : launch_gemm_pp<false>(amaps, bmap, om, p, m_tiles, stream);
   if (geglu) {
     switch (bn) {
       case 256: return launch_gemm<256, 4, true>(amaps, bmap, om, p, m_tiles, stream);

@@ -14,6 +14,7 @@ from . import _lib
 from ._lib import IHError, check
 
 EPI_NONE, EPI_GEGLU, EPI_SILU, EPI_GELU, EPI_QUICK_GELU, EPI_RELU = 0, 1, 2, 4, 8, 16
+TILE_PINGPONG = 1   # IH_TILE_PINGPONG: linear(tile_n=TILE_PINGPONG) forces the ping-pong GEMM kernel
 
 
 def _stream() -> int:
@@ -57,7 +58,8 @@ def linear(x: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor] = None
     `relu=True`: out = relu(alpha * x @ w.T + bias + residual), the ReLU after the residual (IH_EPI_RELU); it takes no
     other activation, rowbias, ln, stats_out or tile_n.
     `tile_n`: 0 lets the library choose; else 64 / 128 / 160 / 192 / 256 output columns per tile, or with `geglu`
-    128 / 192 / 256 weight rows per tile (value and gate halves: 64 / 96 / 128 outputs).
+    128 / 192 / 256 weight rows per tile (value and gate halves: 64 / 96 / 128 outputs).  `tile_n=TILE_PINGPONG`
+    forces the ping-pong kernel (bias, ln and geglu only), which the library's choice takes where it is faster.
 
     LayerNorm folding: `stats_out` (float32 [ceil(N/64), M, 2]) receives per-row (sum, sumsq) of the stored values as
     partial sums whose total over slots is the row's; `ln=(stats, eps)` makes this GEMM consume RAW rows `x` with the gamma-scaled, row-centred weight and

@@ -42,7 +42,11 @@ void ih_launch_count_reset(void);
  * :396,410-411,432-433,453 (IPAttnProcessor2_0 incl. to_k_ip/to_v_ip), and the diffusers proj_in/proj_out/FF/1x1
  * conv layers reached through custom_pipelines.py:338-345.  tile_n: 0 = auto, else 64/128/160/192/256 (384 and
  * 512 mean 192 and 256).  With IH_EPI_GEGLU tile_n counts the weight rows of a tile, value and gate halves together:
- * 128/192/256 (64/96/128 outputs per tile); the 192-row GEGLU tile cannot write stats_out. */
+ * 128/192/256 (64/96/128 outputs per tile); the 192-row GEGLU tile cannot write stats_out.
+ * tile_n = IH_TILE_PINGPONG forces the ping-pong kernel (128x128 tiles, one per MMA warpgroup; GEGLU: 64 outputs per
+ * tile), which the automatic choice takes where it is faster.  It supports bias, LayerNorm folding and GEGLU only, and
+ * its outputs are bitwise equal to the other tiles'. */
+#define IH_TILE_PINGPONG 1
 int ih_gemm_f16(const void* a, long long lda, const void* w, const void* bias, const void* rowbias,
                 int rows_per_group, long long ld_rowbias, const void* residual, long long ldr, void* out,
                 long long ldo, int M, int N, int K, int epilogue, int tile_n, void* stream);

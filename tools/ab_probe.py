@@ -1,6 +1,7 @@
 """Small A/B probes (graph-timed, same process => same thermal state).  `python tools/ab_probe.py tile` measures the
 main-loop cost per 64-deep k-block of the 128xBN tiles, plain and GEGLU, with every SM busy (calibrates the tile
-costs in gemm.cu)."""
+costs in gemm.cu).  `python tools/ab_probe.py pp` times the ping-pong kernel against gemm_f16_kernel at the
+LayerNorm-folded q|k|v and GEGLU launches of the SDXL base and refiner UNets (calibrates pick_pp in gemm.cu)."""
 import os
 import sys
 
@@ -73,11 +74,44 @@ def shapes():
             print(f"conv B{B} {H}^2 {Cin}->{Cout} bn{tn}: {t*1e6:.1f} us", flush=True)
 
 
+def pp_shapes():
+    """LayerNorm-folded q|k|v (N = 3C) and GEGLU (N = 8C) launches with bias, as in the UNet: M = 2 * images * tokens
+    (CFG), C the block width.  The base UNet's transformer levels have C = 640 at res / 16 and C = 1280 at res / 32,
+    the refiner's C = 768 and 1536 at the same levels.  `old` is gemm_f16_kernel's fastest tile (GEGLU: the 256-row
+    tile, its automatic choice), `auto` the library's choice."""
+    sms = torch.cuda.get_device_properties(0).multi_processor_count
+    print(f"{torch.cuda.get_device_name(0)}, {sms} SMs", flush=True)
+    for net, widths in (("base", (640, 1280)), ("refiner", (768, 1536))):
+        for res in (512, 768, 1024):
+            for images in (1, 4):
+                for lvl, c in enumerate(widths):
+                    m = 2 * images * (res // (16 << lvl)) ** 2
+                    st = torch.rand((c // 64, m, 2), device="cuda")
+                    st[..., 1] += 64.0
+                    x = r(m, c)
+                    for geglu in (False, True):
+                        n = 8 * c if geglu else 3 * c
+                        w, b = r(n, c, scale=c ** -0.5), r(n)
+
+                        def run(tn):
+                            return timeit(lambda: ops.linear(x, w, b, geglu=geglu, ln=(st, 1e-5), tile_n=tn))
+                        old_tiles = (256,) if geglu else (128, 160, 192, 256)
+                        old = min(run(tn) for tn in old_tiles)
+                        pp, auto = run(ops.TILE_PINGPONG), run(0)
+                        kb = (c + 63) // 64
+                        tiles = -(-m // 128) * -(-(n // 2 if geglu else n) // (64 if geglu else 128))
+                        print(f"{net} {res}^2 x{images} C{c} {'GEGLU' if geglu else 'qkv  '} M{m} N{n} K{c}: kb {kb}, "
+                              f"pp tiles/SM {tiles / sms:.2f}: old {old*1e6:.1f} us, pp {pp*1e6:.1f} us "
+                              f"(x{old / pp:.3f}), auto {auto*1e6:.1f} us", flush=True)
+
+
 if __name__ == "__main__":
     if len(sys.argv) > 1 and sys.argv[1] == "tile":
         tile_costs()
         geglu_tile_costs()
     elif len(sys.argv) > 1 and sys.argv[1] == "geglu":
         geglu_shapes()
+    elif len(sys.argv) > 1 and sys.argv[1] == "pp":
+        pp_shapes()
     else:
         shapes()
