@@ -116,6 +116,22 @@ TINY_CONTROLNET = ControlNetConfig(
 )
 
 
+@dataclass(frozen=True)
+class T2IAdapterConfig:
+    """[3P] diffusers 0.30.0 T2IAdapter config (e.g. TencentARC/t2i-adapter-canny-sdxl-1.0 config.json):
+    `full_adapter_xl` with one feature per UNet injection point (imagharmony_b200.t2i_adapter)."""
+    in_channels: int = 3
+    channels: Tuple[int, ...] = (320, 640, 1280, 1280)
+    num_res_blocks: int = 2
+    downscale_factor: int = 16
+    adapter_type: str = "full_adapter_xl"
+
+
+SDXL_T2I_ADAPTER = T2IAdapterConfig()
+# the same architecture at TINY's widths (its three UNet levels and mid block)
+TINY_T2I_ADAPTER = T2IAdapterConfig(channels=(64, 128, 256, 256))
+
+
 # diffusers config.json fields the native UNet / ControlNet build only with these values (absent = the default)
 _REQUIRED = {
     "addition_embed_type": ("text_time",),

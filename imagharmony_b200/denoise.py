@@ -36,11 +36,15 @@ their residuals summed and injected after the mid block in one launch, then the 
 graph.  There is one graph per distinct set of active nets (staggered windows of K nets give at most 2K + 1); steps
 where no net is active (keep[i] = 0 for all) replay the ControlNet-free graph.  The scale vectors are read from device
 memory, so a new controlnet_conditioning_scale does not re-capture.
+
+T2I-Adapter (`run(adapter=...)`): the adapter runs once per call, outside the loop (the pipeline's job); its four
+features are copied into static buffers and its scale into a device value, and the step graph with the features adds
+them inside the UNet's encoder (4 launches).  Steps past the adapter's window (keep[i] = 0) replay the plain graph.
 """
 from __future__ import annotations
 
 from dataclasses import dataclass
-from typing import Callable, Dict, List, Optional, Tuple, Union
+from typing import Callable, Dict, List, NamedTuple, Optional, Tuple, Union
 
 import numpy as np
 import torch
@@ -50,7 +54,8 @@ from ._lib import IH_CN_MAX_NETS, IHError
 from .controlnet import controlnet_scales
 from .scheduler import (DPMSolverMultistepScheduler, EulerAncestralDiscreteScheduler, EulerDiscreteScheduler,
                         randn_tensor)
-from .unet import UNet2DConditionModel, require_latent_size
+from .t2i_adapter import AdapterCall
+from .unet import UNet2DConditionModel, require_adapter_shapes, require_latent_size
 
 # option -> the options it cannot be combined with, and why
 _EXCLUDES = (
@@ -61,7 +66,29 @@ _EXCLUDES = (
     ("controlnet", ("begin_step", "inpaint", "unet_cond", "start_step", "stop_after"), "it runs text-to-image loops"),
     ("inpaint", ("start_step", "stop_after"), "inpainting resumes nothing"),
     ("begin_step", ("start_step", "stop_after"), "image-to-image resumes nothing"),
+    ("adapter", ("begin_step", "inpaint", "unet_cond", "controlnet", "start_step", "stop_after"),
+     "the T2I-Adapter runs text-to-image loops (diffusers has no SDXL pipeline for these combinations)"),
 )
+
+
+class GraphKey(NamedTuple):
+    """The key of one captured step graph (DenoiseEngine._graphs).  Read it by field name.  It is also a plain tuple,
+    and fields added later go before `cond`, so the positions of the older fields stay where they were (the shape in
+    front, `ib` second to last, `controlnet` last)."""
+    n: int
+    h: int
+    w: int
+    L: int
+    T: int
+    use_cfg: bool
+    guidance: float
+    rescale: float
+    scale: float                              # the IP scale of the step
+    kind: str                                 # the scheduler's
+    adapter: bool                             # T2I-Adapter features added
+    cond: bool                                # 9-channel UNet
+    ib: bool                                  # 4-channel inpainting blend
+    controlnet: Optional[tuple]               # ("controlnet", guess mode with CFG, active net indices) or None
 
 
 @dataclass
@@ -81,11 +108,14 @@ class _Loop:
     noise: Optional[torch.Tensor] = None      # Euler Ancestral step noise [T, n, C, h, w]
     ib: Optional[dict] = None                 # 4-channel inpainting: image_latents, noise, mask, blend_end
     cond: Optional[torch.Tensor] = None       # 9-channel UNet: mask | masked-image latents
+    adapter: Optional[tuple] = None           # T2I-Adapter: (static feature buffers, device fp32 scale)
 
-    def graph_key(self, scale: float, cn) -> tuple:
-        """The key of the step graph with IP scale `scale` and active ControlNet step `cn` (see DenoiseEngine._step)."""
-        return (*self.shape, self.use_cfg, self.guidance, self.rescale, scale, self.kind, self.cond is not None,
-                self.ib is not None, None if cn is None else ("controlnet", cn[2] > 0, cn[0]))
+    def graph_key(self, scale: float, cn, adapter: bool = False) -> "GraphKey":
+        """The key of the step graph with IP scale `scale`, active ControlNet step `cn` (see DenoiseEngine._step) and
+        the T2I-Adapter's features added or not."""
+        return GraphKey(*self.shape, self.use_cfg, self.guidance, self.rescale, scale, self.kind, bool(adapter),
+                        self.cond is not None, self.ib is not None,
+                        None if cn is None else ("controlnet", cn[2] > 0, cn[0]))
 
 
 class DenoiseEngine:
@@ -96,7 +126,7 @@ class DenoiseEngine:
         self.device = unet.conv_in.weight.device
         self.scheduler = scheduler or EulerDiscreteScheduler()      # the pipeline's own scheduler object when given
         self.use_cuda_graph = use_cuda_graph and self.device.type == "cuda"
-        self._graphs: Dict[Tuple, Tuple[torch.cuda.CUDAGraph, int]] = {}   # key -> (graph, workspace generation)
+        self._graphs: Dict[GraphKey, Tuple[torch.cuda.CUDAGraph, int]] = {}   # key -> (graph, workspace generation)
         self._pool: Dict[Tuple[str, Tuple], torch.Tensor] = {}         # (buffer name, shape key) -> static buffer
         # (kind, T) -> (timesteps fp32, sigmas fp32, init_noise_sigma, coefficient table or None)
         self._schedules: Dict[Tuple[str, int], tuple] = {}
@@ -186,7 +216,7 @@ class DenoiseEngine:
         loop.st["step"].fill_(step)
         self._first_input(loop)
 
-    def _step(self, loop: _Loop, cn=None):
+    def _step(self, loop: _Loop, cn=None, adapter: bool = False):
         st, residuals = loop.st, None
         if cn is not None:          # (active net indices, [(ControlNet, emb, scale)], first image they run on)
             _, nets, b0 = cn
@@ -195,7 +225,8 @@ class DenoiseEngine:
                     for model, emb, scale in nets]
             residuals = (outs[0] if len(outs) == 1 else outs, b0)
         noise = self.unet(st["model_in"], loop.timesteps, st["ehs"], st["text_embeds"], st["time_ids"], step=st["step"],
-                          cond=loop.cond, controlnet_residuals=residuals)
+                          cond=loop.cond, controlnet_residuals=residuals,
+                          adapter_residuals=loop.adapter if adapter else None)
         ib = loop.ib
         if loop.dpm is not None:
             ops.dpm_solver_step(noise, st["latents"], st["model_in"], loop.dpm["prev_x0"], loop.coeffs, st["step"],
@@ -224,7 +255,8 @@ class DenoiseEngine:
             negative_time_ids: Optional[torch.Tensor] = None, begin_step: int = 0,
             inpaint: Optional[Tuple[torch.Tensor, torch.Tensor, torch.Tensor]] = None,
             generator: Optional[Union[torch.Generator, List[torch.Generator]]] = None,
-            unet_cond: Optional[Tuple[torch.Tensor, torch.Tensor]] = None, controlnet=None) -> torch.Tensor:
+            unet_cond: Optional[Tuple[torch.Tensor, torch.Tensor]] = None, controlnet=None,
+            adapter: Optional[AdapterCall] = None) -> torch.Tensor:
         """latents [n,4,h,w] (already scaled by init_noise_sigma; host or device); embeds host or device tensors.
         Returns the latents after the last executed step as a new device tensor.
 
@@ -276,7 +308,15 @@ class DenoiseEngine:
         `controlnet` = a sequence of ControlNetCalls (up to 8, one per net, sharing guess_mode) is a Multi-ControlNet
         ([3P] MultiControlNetModel): at step i the nets with keep[i] = 1 run in net order and their scaled residuals
         are summed in fp16 and added in one launch.  diffusers runs an inactive net with scale 0; skipping it is exact
-        (fp16(acc + 0) = acc).  A list of one call is the single-net case."""
+        (fp16(acc + 0) = acc).  A list of one call is the single-net case.
+
+        `adapter` = an AdapterCall ([3P] StableDiffusionXLAdapterPipeline, T2I-Adapter): the call's 4 features are
+        copied once into static buffers and its scale into a device fp32 value; at every step i with keep[i] = 1 the
+        UNet adds them inside its encoder (UNet2DConditionModel.forward(adapter_residuals=)) to both CFG halves, at
+        steps with keep[i] = 0 the step is the plain one.  There are at most two graphs per shape, with and without the
+        features, and a new scale or image re-captures neither.  It works with every scheduler and the loop options
+        of text-to-image, not with begin_step, inpaint, unet_cond, controlnet, start_step or stop_after (IHError).  It
+        draws no random numbers."""
         use_cfg = guidance_scale > 1.0                                            # :223
         is_dpm = isinstance(self.scheduler, DPMSolverMultistepScheduler)         # the one scheduler dispatch
         is_ancestral = isinstance(self.scheduler, EulerAncestralDiscreteScheduler)
@@ -288,7 +328,7 @@ class DenoiseEngine:
             raise IHError("classifier-free guidance needs negative_prompt_embeds / negative_pooled")
         given = {"DPMSolverMultistepScheduler": is_dpm, "begin_step": bool(begin_step), "inpaint": inpaint is not None,
                  "unet_cond": unet_cond is not None, "controlnet": controlnet is not None,
-                 "start_step": bool(start_step), "stop_after": stop_after is not None}
+                 "start_step": bool(start_step), "stop_after": stop_after is not None, "adapter": adapter is not None}
         for option, excluded, why in _EXCLUDES:
             clash = [o for o in excluded if given[o]]
             if given[option] and clash:
@@ -333,6 +373,18 @@ class DenoiseEngine:
                 if tuple(call.image.shape) != (n, mcfg.conditioning_channels, 8 * h, 8 * w):
                     raise IHError(f"ControlNet {j}: image: expected {(n, mcfg.conditioning_channels, 8 * h, 8 * w)}, "
                                   f"got {tuple(call.image.shape)}")
+        ad_keep = None
+        if adapter is not None:
+            if ucfg.in_channels != 4:
+                raise IHError(f"adapter: the T2I-Adapter runs with the 4-channel UNet only (this one has "
+                              f"{ucfg.in_channels} input channels)")
+            feats = list(adapter.features)
+            require_adapter_shapes(ucfg, h, w, [tuple(f.shape[1:]) for f in feats])
+            if any(f.shape[0] != n for f in feats):
+                raise IHError(f"adapter: features of {[f.shape[0] for f in feats]} images for a batch of {n}")
+            ad_keep = [1.0] * T if adapter.keep is None else [float(k) for k in adapter.keep]
+            if len(ad_keep) != T:
+                raise IHError(f"adapter: keep has {len(ad_keep)} entries for a {T}-step schedule")
         start_step = begin_step or start_step
         steps = loop_T if stop_after is None else min(stop_after, loop_T)
 
@@ -376,6 +428,13 @@ class DenoiseEngine:
             for half in ((0, n), (n, 2 * n)) if use_cfg else ((0, n),):     # [3P] cat([mask] * 2) under CFG
                 cond[half[0]:half[1], :1].copy_(unet_cond[0], non_blocking=True)
                 cond[half[0]:half[1], 1:].copy_(unet_cond[1], non_blocking=True)
+        if adapter is not None:     # the features of one CFG half; the UNet adds them to each half
+            bufs = [self._buf("adapter_feature", (k, n, h, w), tuple(f.shape)) for k, f in enumerate(adapter.features)]
+            for b, f in zip(bufs, adapter.features):
+                b.copy_(f, non_blocking=True)
+            scale = self._buf("adapter_scale", (n, h, w), (2,), torch.float32, zero=True)
+            scale.fill_(float(adapter.scale))
+            loop.adapter = (bufs, scale)
         self.unet.prepare_conditioning(st["ehs"], st["text_embeds"], st["time_ids"])
         nets = []                               # per ControlNet: (model, conditioning embedding, scale vector)
         b_cn0 = n if (use_cfg and calls and calls[0].guess_mode) else 0      # guess mode + CFG: the conditional half
@@ -404,6 +463,9 @@ class DenoiseEngine:
             active = tuple(j for j, keep in enumerate(keeps) if keep[i] > 0)
             return (active, [nets[j] for j in active], b_cn0) if active else None
 
+        def ad_at(i: int) -> bool:
+            return ad_keep is not None and ad_keep[i] > 0
+
         if self.use_cuda_graph:
             if self._epoch != getattr(self.unet, "graph_epoch", 0):       # weights / processors changed since capture
                 self._graphs.clear()
@@ -411,11 +473,11 @@ class DenoiseEngine:
             for j, (model, _, _) in enumerate(nets):
                 seen = self._cn_epochs.get(j)
                 if seen is None or seen[0] is not model or seen[1] != model.graph_epoch:   # another / a reloaded net
-                    self._graphs = {k: v for k, v in self._graphs.items() if k[-1] is None or j not in k[-1][2]}
+                    self._graphs = {k: v for k, v in self._graphs.items() if k.controlnet is None or j not in k.controlnet[2]}
                     self._cn_epochs[j] = (model, model.graph_epoch)
             needed = {}
             for i in range(start_step, steps):
-                needed.setdefault(loop.graph_key(scale_at(i), cn_at(i)), (scale_at(i), cn_at(i)))
+                needed.setdefault(loop.graph_key(scale_at(i), cn_at(i), ad_at(i)), (scale_at(i), cn_at(i), ad_at(i)))
             captured = False
             for _ in range(4):      # a warm-up may grow a scratch buffer, which invalidates graphs captured before it
                 gen = ops.workspace_generation()
@@ -423,9 +485,9 @@ class DenoiseEngine:
                 if not missing:
                     break
                 for k in missing:
-                    sc, cn_step = needed[k]
+                    sc, cn_step, ad_step = needed[k]
                     self.set_scale(sc)
-                    self._graphs[k] = (self._capture(loop, cn_step), ops.workspace_generation())
+                    self._graphs[k] = (self._capture(loop, cn_step, ad_step), ops.workspace_generation())
                     captured = True
             else:
                 raise IHError("scratch buffers kept growing during graph capture")
@@ -436,30 +498,30 @@ class DenoiseEngine:
         for i in range(start_step, steps):
             sc = scale_at(i)
             if self.use_cuda_graph:
-                self._graphs[loop.graph_key(sc, cn_at(i))][0].replay()
+                self._graphs[loop.graph_key(sc, cn_at(i), ad_at(i))][0].replay()
             else:
                 self.set_scale(sc)
-                self._step(loop, cn_at(i))
+                self._step(loop, cn_at(i), ad_at(i))
             if callback is not None and (i - b0) % callback_steps == 0:           # :359-363 (Euler: order 1, no warm-up)
                 callback(i - b0, timesteps[i], st["latents"])
         self.set_scale(ip_scale)
         return st["latents"].clone()
 
-    def _capture(self, loop: _Loop, cn=None):
+    def _capture(self, loop: _Loop, cn=None, adapter: bool = False):
         # warm-up on a side stream (sets kernel attributes, fills the TMA descriptor cache, sizes the allocator and
         # the library's scratch buffers)
         side = torch.cuda.Stream(device=self.device)
         side.wait_stream(torch.cuda.current_stream())
         with torch.cuda.stream(side):
             loop.st["step"].zero_()
-            self._step(loop, cn)
+            self._step(loop, cn, adapter)
         torch.cuda.current_stream().wait_stream(side)
         torch.cuda.synchronize()
         loop.st["step"].zero_()
         g = torch.cuda.CUDAGraph()
         before = ops.launch_count()
         with torch.cuda.graph(g):
-            self._step(loop, cn)
+            self._step(loop, cn, adapter)
         self.last_launches_per_step = ops.launch_count() - before
         self.graphs_captured += 1
         return g

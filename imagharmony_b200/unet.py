@@ -26,6 +26,36 @@ from ._lib import IHError
 from .config import UNetConfig
 
 
+def adapter_targets(cfg: UNetConfig, h: int, w: int) -> List[tuple]:
+    """(h, w, C) of the points where [3P] diffusers' UNet2DConditionModel adds down_intrablock_additional_residuals
+    (T2I-Adapter features), in the order it takes them: one per down block -- after the block (after its downsampler)
+    for a block without cross-attention, after its last resnet / attention pair for one with -- then, last, the mid
+    block's output, which takes a leftover feature only if the shapes are equal."""
+    out = []
+    for i, co in enumerate(cfg.block_out_channels):
+        down = i < len(cfg.block_out_channels) - 1 and cfg.transformer_layers_per_block[i] == 0
+        s = 2 ** (i + down)
+        out.append((h // s, w // s, co))
+    s = 2 ** (len(cfg.block_out_channels) - 1)
+    out.append((h // s, w // s, cfg.block_out_channels[-1]))
+    return out
+
+
+def require_adapter_shapes(cfg: UNetConfig, h: int, w: int, shapes) -> None:
+    """IHError unless T2I-Adapter features of (h, w, C) `shapes` each land on an injection point of this UNet at an
+    h x w latent (adapter_targets), every one of them used, as diffusers would add them."""
+    targets = adapter_targets(cfg, h, w)
+    shapes = [tuple(int(v) for v in s) for s in shapes]
+    n_down = len(targets) - 1
+    ok = len(shapes) <= n_down + 1 and all(s == t for s, t in zip(shapes, targets[:n_down]))
+    if ok and len(shapes) == n_down + 1:
+        ok = shapes[-1] == targets[-1]
+    if not ok:
+        raise IHError(f"T2I-Adapter features (h, w, C) {shapes} do not match this UNet's injection points {targets} at a "
+                      f"{h}x{w} latent (its down blocks, then the mid block): the adapter's channels must equal the "
+                      f"UNet's block_out_channels {list(cfg.block_out_channels)} plus the mid block's")
+
+
 def require_latent_size(cfg: UNetConfig, h: int, w: int) -> None:
     """IHError unless an h x w latent fits the UNet: each of its len(block_out_channels) - 1 stride-2 downsamplers
     halves the sides exactly, and every up-block upsamples to twice its input, so both sides must be divisible by
@@ -267,11 +297,15 @@ class DownBlock(nn.Module):
         if add_down:
             self.downsamplers = nn.ModuleList([Resample(cout, up=False)])
 
-    def forward(self, x, temb_all, ehs, skips: List[torch.Tensor]):
+    def forward(self, x, temb_all, ehs, skips: List[torch.Tensor], inject=None):
+        """`inject(x)`: an in-place addition to the output of the last resnet / attention pair, before it is appended
+        to the skips and downsampled (diffusers' additional_residuals of CrossAttnDownBlock2D)."""
         for j, res in enumerate(self.resnets):
             x = res(x, temb_all)
             if self.has_attn:
                 x = self.attentions[j](x, ehs)
+            if inject is not None and j == len(self.resnets) - 1:
+                inject(x)
             skips.append(x)
         if self.has_down:
             x = self.downsamplers[0](x)
@@ -545,10 +579,41 @@ class UNet2DConditionModel(SDXLEncoderModel):
         self._b_out = torch.zeros((16,), dtype=w_out.dtype, device=w_out.device)
         self._b_out[: w_out.shape[0]] = self.conv_out.bias.detach()
 
+    def _down_mid_with_adapter(self, x, temb_all, ehs, skips, adapter_residuals):
+        """The down and mid blocks with T2I-Adapter features added at diffusers' points (see forward)."""
+        if self.config.in_channels != 4:
+            raise IHError("adapter_residuals: the T2I-Adapter runs with the 4-channel UNet only (diffusers has no SDXL "
+                          "adapter pipeline for the 9-channel inpainting UNet)")
+        feats, scale = adapter_residuals
+        B, H, W, _ = x.shape
+        require_adapter_shapes(self.config, H, W, [f.shape[1:] for f in feats])
+        m = feats[0].shape[0]
+        if any(f.shape[0] != m for f in feats) or B % m or scale.numel() < B // m:
+            raise IHError(f"adapter_residuals: features of {[f.shape[0] for f in feats]} images and {scale.numel()} "
+                          f"scales for a batch of {B}")
+        pending = list(feats)
+
+        def add(t: torch.Tensor) -> None:
+            f = pending.pop(0)
+            rows = m * f.shape[1] * f.shape[2]
+            ops.controlnet_add_residuals([t] * (B // m), [f] * (B // m), scale, [r * rows for r in range(B // m)])
+
+        for blk in self.down_blocks:
+            if pending and blk.has_attn:
+                x = blk(x, temb_all, ehs, skips, inject=add)
+            else:
+                x = blk(x, temb_all, ehs, skips)
+                if pending:
+                    add(x)                  # in place: the skip this block appended last is x itself
+        x = self.mid_block(x, temb_all, ehs)
+        if pending:                         # require_adapter_shapes: it has the mid block's shape
+            add(x)
+        return x
+
     def forward(self, sample: torch.Tensor, timesteps: torch.Tensor, encoder_hidden_states: torch.Tensor,
                 text_embeds: Optional[torch.Tensor] = None, time_ids: Optional[torch.Tensor] = None,
                 step: Optional[torch.Tensor] = None, cond: Optional[torch.Tensor] = None,
-                controlnet_residuals=None) -> torch.Tensor:
+                controlnet_residuals=None, adapter_residuals=None) -> torch.Tensor:
         """sample NCHW fp16 [B,4,H,W]; timesteps fp32 device tensor ([B] values, or the whole schedule when `step`
         -- a device int32 index -- is given); returns noise prediction NCHW fp16.  The 9-channel inpainting UNet also
         takes `cond` NCHW fp16 [B,5,H,W] (mask | masked-image latents), which conv_in reads after the 4 latent channels;
@@ -559,7 +624,15 @@ class UNet2DConditionModel(SDXLEncoderModel):
         to the mid-block output, into the rows of the images from the offset on (n in guess mode: the ControlNet ran on
         the conditional half only, the unconditional half gets nothing).  With a list of ControlNetOutputs (one per net
         of a Multi-ControlNet, one row offset for all) the nets' scaled residuals are summed in fp16 in list order and
-        the sum is added, in one launch (ops.controlnet_add_residuals_multi)."""
+        the sum is added, in one launch (ops.controlnet_add_residuals_multi).
+
+        `adapter_residuals` = (features, scale): T2I-Adapter features, diffusers' down_intrablock_additional_residuals.
+        features[k] is NHWC fp16 [m, h_k, w_k, C_k] with m dividing the batch (the features of one CFG half); scale is
+        a device fp32 vector with at least batch / m entries, all the same value.  Feature k is added in place, as
+        fp16(x + fp16(feature * scale)), to each group of m images at injection point k (adapter_targets): after a
+        down block without cross-attention (its skip, the same tensor, sees the sum), after the last resnet /
+        attention pair of one with it (before the skip is taken and the block downsamples), and a leftover feature
+        after the mid block.  One launch per point; diffusers' single fp16(v * s) and fp16 add give the same bits."""
         if self._w_temb is None:
             raise IHError("UNet2DConditionModel.finalize() has not been called")
         B = sample.shape[0]
@@ -579,9 +652,12 @@ class UNet2DConditionModel(SDXLEncoderModel):
         x = ops.linear(a, self._w_in, self.conv_in.bias).reshape(Bs, Hs, Ws, -1)
         skips = [x]
         ehs = encoder_hidden_states
-        for blk in self.down_blocks:
-            x = blk(x, temb_all, ehs, skips)
-        x = self.mid_block(x, temb_all, ehs)
+        if adapter_residuals is None:
+            for blk in self.down_blocks:
+                x = blk(x, temb_all, ehs, skips)
+            x = self.mid_block(x, temb_all, ehs)
+        else:
+            x = self._down_mid_with_adapter(x, temb_all, ehs, skips, adapter_residuals)
         if controlnet_residuals is not None:
             # in place, and only here: the mid block has consumed skips[-1] (its input), and no skip is read again
             # before the up blocks pop them, so nothing sees a skip both before and after the addition

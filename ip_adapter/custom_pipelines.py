@@ -515,15 +515,12 @@ class StableDiffusionXLCustomPipeline:
     def _denoise_from(self, lat, *, num_inference_steps: int, embeds, sizes, guidance_scale, guidance_rescale,
                       generator, callback, callback_steps, t_start: int = 0, denoising_end=None,
                       control_guidance_start=0.0, control_guidance_end=1.0, inpaint=None, unet_cond=None,
-                      controlnet=None, aesthetic=None) -> torch.Tensor:
+                      controlnet=None, aesthetic=None, adapter=None) -> torch.Tensor:
         """The loop over timesteps[t_start:], truncated by denoising_end (:307-316), from the noised start latents `lat`
         with the IP scale of the processors (:319-322); the micro-conditioning time ids are formed from `sizes`, and
         from `aesthetic` = (aesthetic_score, negative_aesthetic_score) for a 5-id UNet. -> final latents."""
         add_time_ids, negative_add_time_ids = self._add_time_ids(embeds[0].shape[0], sizes, aesthetic)
-        loop_end = num_inference_steps
-        if _fraction(denoising_end):
-            cutoff = _denoising_cutoff(self.scheduler.num_train_timesteps, denoising_end)
-            loop_end = t_start + int(sum(1 for t in self.scheduler.timesteps[t_start:] if t >= cutoff))
+        loop_end = self._loop_end(num_inference_steps, denoising_end, t_start)
         conditioning_scale = self._ip_scale()
         if loop_end > t_start:
             out = self.engine.run(lat, *embeds, add_time_ids, num_inference_steps,
@@ -532,11 +529,20 @@ class StableDiffusionXLCustomPipeline:
                                   control_guidance_end=control_guidance_end, guidance_rescale=guidance_rescale,
                                   num_loop_steps=loop_end, callback=callback, callback_steps=callback_steps,
                                   negative_time_ids=negative_add_time_ids, begin_step=t_start, inpaint=inpaint,
-                                  generator=generator, unet_cond=unet_cond, controlnet=controlnet)
+                                  generator=generator, unet_cond=unet_cond, controlnet=controlnet, adapter=adapter)
         else:
             out = lat.to(self.device)
         self.set_scale(conditioning_scale)
         return out
+
+    def _loop_end(self, num_inference_steps: int, denoising_end, t_start: int = 0) -> int:
+        """The schedule index the loop over timesteps[t_start:] stops at: num_inference_steps, or with a valid
+        denoising_end (:307-316) t_start + the number of those timesteps at or above its cutoff.  The scheduler's
+        timesteps must be set."""
+        if not _fraction(denoising_end):
+            return num_inference_steps
+        cutoff = _denoising_cutoff(self.scheduler.num_train_timesteps, denoising_end)
+        return t_start + int(sum(1 for t in self.scheduler.timesteps[t_start:] if t >= cutoff))
 
     @staticmethod
     def _check_batches(batch_size: int, generator, *batches: Tuple[str, int]) -> None:
@@ -1142,4 +1148,190 @@ class StableDiffusionXLControlNetPipeline(StableDiffusionXLCustomPipeline):
         out = self._denoise_from(lat, num_inference_steps=num_inference_steps, embeds=embeds, sizes=sizes,
                                  guidance_scale=guidance_scale, guidance_rescale=guidance_rescale, callback=callback,
                                  callback_steps=callback_steps, generator=generator, controlnet=cn if multi else cn[0])
+        return self._output(out, output_type, return_dict)
+
+
+def preprocess_adapter_image(image, height: int, width: int) -> torch.Tensor:
+    """[3P] diffusers' _preprocess_adapter_image (pipeline_stable_diffusion_xl_adapter.py): a tensor is returned as it
+    is; PIL image(s) are resized with Lanczos to width x height and divided by 255, a grayscale image giving one channel
+    ([h, w] -> [1, 1, h, w], [h, w, c] -> [1, c, h, w]); a list of [C, H, W] tensors is stacked and a list of
+    [B, C, H, W] tensors concatenated.  -> float32 [B, C, height, width] (PIL) or the tensor(s) as given."""
+    import numpy as np
+    from PIL import Image
+    if isinstance(image, torch.Tensor):
+        return image
+    if isinstance(image, Image.Image):
+        image = [image]
+    if isinstance(image, (list, tuple)) and image and isinstance(image[0], Image.Image):
+        arrs = [np.array(im.resize((width, height), resample=Image.LANCZOS)) for im in image]
+        arrs = [a[None, ..., None] if a.ndim == 2 else a[None, ...] for a in arrs]
+        arr = np.concatenate(arrs, axis=0).astype(np.float32) / 255.0
+        return torch.from_numpy(arr.transpose(0, 3, 1, 2).copy())
+    if isinstance(image, (list, tuple)) and image and isinstance(image[0], torch.Tensor):
+        if image[0].ndim == 3:
+            return torch.stack(list(image), dim=0)
+        if image[0].ndim == 4:
+            return torch.cat(list(image), dim=0)
+        raise ValueError(f"Invalid image tensor! Expecting image tensor with 3 or 4 dimension, but recive: "
+                         f"{image[0].ndim}")
+    raise ValueError(f"the adapter `image` must be a PIL image, a list of them, a tensor or a list of tensors, got "
+                     f"{type(image).__name__}")
+
+
+class StableDiffusionXLAdapterPipeline(StableDiffusionXLCustomPipeline):
+    """Text-to-image with an SDXL T2I-Adapter, with the call surface of [3P] diffusers 0.30
+    `StableDiffusionXLAdapterPipeline`, so that `IPAdapterXL(adapter_pipe, ...).generate(pil_image=..., image=sketch,
+    adapter_conditioning_scale=s)` combines an image prompt with a layout image.  The adapter runs once per call
+    (imagharmony_b200.t2i_adapter); its features are added inside the UNet's encoder in the replayed step graph
+    (DenoiseEngine.run(adapter=...)) at the steps i < int(num_inference_steps * adapter_conditioning_factor), where
+    num_inference_steps counts the steps left after a denoising_end cut.
+
+    `adapter` may be a list of T2IAdapters, wrapped in a MultiAdapter as diffusers does, or a MultiAdapter.  Then
+    `image` is a list with one image (or batch) per adapter and `adapter_conditioning_scale` a list of weights (a float
+    is taken as the weight of every adapter, an extension: diffusers' MultiAdapter fails on a float); the weighted sum is
+    formed once per call.
+
+    As in diffusers, the features are repeated num_images_per_prompt times as a whole ([a, b] -> [a, b, a, b]) and
+    then for the CFG halves, and must then equal the prompt batch or, without CFG, be one image; any other image batch
+    raises IHError before any work.  One layout image for num_samples > 1 images of IPAdapterXL.generate is therefore
+    passed as a list of num_samples copies.
+
+    `control_guidance_start` / `control_guidance_end` gate the IP-adapter scale, as in the text-to-image pipeline.
+    T2I-Adapter image-to-image / inpainting / refiner, together with ControlNet or PNS resume, and the SD1.5 adapter
+    types are not built (IHError); so are the diffusers arguments in UNSUPPORTED."""
+
+    UNSUPPORTED = ("timesteps", "sigmas", "ip_adapter_image", "ip_adapter_image_embeds", "clip_skip",
+                   "callback_on_step_end", "denoising_start")
+
+    def __init__(self, unet: UNet2DConditionModel, adapter, prompt_encoder: Optional[Callable] = None,
+                 vae_decode: Optional[Callable] = None, scheduler=None, vae=None):
+        from imagharmony_b200.t2i_adapter import MultiAdapter, T2IAdapter
+        if isinstance(adapter, (list, tuple)):              # [3P] diffusers wraps a list the same way
+            adapter = MultiAdapter(adapter)
+        if not isinstance(adapter, (T2IAdapter, MultiAdapter)):
+            raise IHError(f"StableDiffusionXLAdapterPipeline: adapter must be a T2IAdapter, a MultiAdapter or a list of "
+                          f"T2IAdapters, got {type(adapter).__name__}")
+        super().__init__(unet, prompt_encoder=prompt_encoder, vae_decode=vae_decode, scheduler=scheduler, vae=vae)
+        self.adapter = adapter
+
+    @classmethod
+    def from_random(cls, cfg: UNetConfig = SDXL_BASE, adapter_cfg=None, seed: int = 0, device="cuda", vae_cfg=None):
+        """Random-init UNet and adapter weights (SDXL_T2I_ADAPTER by default).  A list of adapter configs gives a
+        MultiAdapter pipeline, adapter j seeded with seed + 31 + 7j."""
+        from imagharmony_b200.config import SDXL_T2I_ADAPTER
+        from imagharmony_b200.t2i_adapter import T2IAdapter
+        adapter_cfg = SDXL_T2I_ADAPTER if adapter_cfg is None else adapter_cfg
+        base = StableDiffusionXLCustomPipeline.from_random(cfg, seed=seed, device=device, vae_cfg=vae_cfg)
+        cfgs = adapter_cfg if isinstance(adapter_cfg, (list, tuple)) else [adapter_cfg]
+        ads = [random_module(T2IAdapter, c, seed + 31 + 7 * j, device) for j, c in enumerate(cfgs)]
+        return cls(base.unet, ads if isinstance(adapter_cfg, (list, tuple)) else ads[0], vae=base.vae)
+
+    @classmethod
+    def from_pretrained(cls, path: str, adapter=None, torch_dtype=torch.float16, add_watermarker: bool = False,
+                        device="cuda", cfg: Optional[UNetConfig] = None, vae_cfg=None, **kwargs):
+        """`adapter=T2IAdapter.from_pretrained(dir)` (or a list of them, or a MultiAdapter) with the SDXL folder `path`
+        of StableDiffusionXLCustomPipeline.from_pretrained; refused before anything is read without it."""
+        if adapter is None:
+            raise ValueError("StableDiffusionXLAdapterPipeline.from_pretrained needs adapter=")
+        return super().from_pretrained(path, torch_dtype, add_watermarker, device, cfg, vae_cfg, adapter=adapter)
+
+    @classmethod
+    def _from_parts(cls, parts: _Pretrained, device, adapter=None, **kwargs):
+        return cls(parts.unet, adapter, prompt_encoder=parts.prompt_encoder, vae=parts.vae)
+
+    def _default_height_width(self, height: Optional[int], width: Optional[int], image) -> Tuple[int, int]:
+        """[3P] diffusers: the first image's size (the first of nested lists), rounded down to a multiple of the
+        adapter's downscale factor (16); sizes given are kept."""
+        from PIL import Image
+        while isinstance(image, list):
+            image = image[0]
+        f = self.adapter.downscale_factor
+        if height is None:
+            height = image.height if isinstance(image, Image.Image) else int(image.shape[-2])
+            height = (height // f) * f
+        if width is None:
+            width = image.width if isinstance(image, Image.Image) else int(image.shape[-1])
+            width = (width // f) * f
+        return height, width
+
+    @torch.no_grad()
+    def __call__(self, prompt: Optional[Union[str, List[str]]] = None, prompt_2=None, image=None,
+                 height: Optional[int] = None, width: Optional[int] = None, num_inference_steps: int = 50,
+                 denoising_end: Optional[float] = None, guidance_scale: float = 5.0, negative_prompt=None,
+                 negative_prompt_2=None, num_images_per_prompt: Optional[int] = 1, eta: float = 0.0, generator=None,
+                 latents: Optional[torch.Tensor] = None, prompt_embeds: Optional[torch.Tensor] = None,
+                 negative_prompt_embeds: Optional[torch.Tensor] = None,
+                 pooled_prompt_embeds: Optional[torch.Tensor] = None,
+                 negative_pooled_prompt_embeds: Optional[torch.Tensor] = None, output_type: Optional[str] = "pil",
+                 return_dict: bool = True, callback=None, callback_steps: int = 1,
+                 cross_attention_kwargs: Optional[Dict[str, Any]] = None, guidance_rescale: float = 0.0,
+                 original_size: Optional[Tuple[int, int]] = None, crops_coords_top_left: Tuple[int, int] = (0, 0),
+                 target_size: Optional[Tuple[int, int]] = None, negative_original_size=None,
+                 negative_crops_coords_top_left=(0, 0), negative_target_size=None,
+                 adapter_conditioning_scale: Union[float, List[float]] = 1.0, adapter_conditioning_factor: float = 1.0,
+                 control_guidance_start: float = 0.0, control_guidance_end: float = 1.0, **kwargs):
+        """diffusers' parameter list: `image` is the adapter image (PIL image(s) or a tensor in [0, 1]; for a
+        MultiAdapter one per adapter); height and width default to its size rounded down to a multiple of 16.  Unknown
+        keywords are ignored as in the text-to-image pipeline, except the arguments in UNSUPPORTED, which raise
+        IHError."""
+        from imagharmony_b200.t2i_adapter import AdapterCall, MultiAdapter, adapter_keep, require_image_size
+        self._require_latent_unet()
+        self._refuse_unsupported(kwargs)
+        if image is None:
+            raise ValueError("`image` (the adapter image) cannot be undefined")
+        multi = isinstance(self.adapter, MultiAdapter)
+        if multi:
+            k = self.adapter.num_adapter
+            if not isinstance(image, list) or len(image) != k:
+                raise ValueError(f"MultiAdapter is enabled: `image` must be a list with one entry per adapter ({k})")
+            scales = adapter_conditioning_scale
+            scales = [float(s) for s in scales] if isinstance(scales, (list, tuple)) else [float(scales)] * k
+            if len(scales) != k:
+                raise ValueError(f"`adapter_conditioning_scale` has {len(scales)} entries for {k} adapters")
+        elif isinstance(adapter_conditioning_scale, (list, tuple)):
+            raise IHError("a list of adapter_conditioning_scale values needs a MultiAdapter (a list of adapters)")
+        height, width = self._default_height_width(height, width, image)
+        inputs = [preprocess_adapter_image(im, height, width) for im in (image if multi else [image])]
+        c_in = self.adapter.config.in_channels
+        for x in inputs:
+            if x.dim() != 4 or x.shape[1] != c_in or tuple(x.shape[2:]) != (height, width):
+                raise IHError(f"adapter image {tuple(x.shape)}: expected [B, {c_in}, {height}, {width}] (a tensor is "
+                              "not resized; a PIL image's mode must give the adapter's in_channels)")
+        if any(x.shape[0] != inputs[0].shape[0] for x in inputs):
+            raise IHError(f"MultiAdapter: the adapter images' batches differ: {[x.shape[0] for x in inputs]}")
+        height, width = self._checked_size(height, width)
+        require_image_size(self.adapter.config, height, width)
+        self._check_callback_steps(callback, callback_steps)
+        nipp = num_images_per_prompt or 1
+        if prompt_embeds is not None:
+            batch = prompt_embeds.shape[0]
+        elif prompt is not None:
+            batch = (1 if isinstance(prompt, str) else len(prompt)) * nipp
+        else:
+            raise ValueError("Provide either `prompt` or `prompt_embeds`")
+        fb = inputs[0].shape[0] * nipp
+        if fb != batch and not (guidance_scale <= 1.0 and fb == 1):
+            raise IHError(f"an adapter-image batch of {inputs[0].shape[0]} repeated {nipp} times does not broadcast "
+                          f"against the prompt batch of {batch} (diffusers adds the features without repeating them "
+                          "per prompt: pass one adapter image per prompt)")
+        embeds, sizes = self._embeds_and_sizes(locals(), height, width)
+        dev = self.device
+        self.scheduler.set_timesteps(num_inference_steps)
+        lat = self.prepare_latents(batch, self.unet.config.in_channels, height, width, torch.float16, dev,
+                                   generator, latents)
+        if multi:
+            feats = self.adapter([x.to(dev) for x in inputs], scales)
+            scale = 1.0
+        else:
+            feats = self.adapter(inputs[0].to(dev))
+            scale = float(adapter_conditioning_scale)
+        feats = [f.repeat(nipp, 1, 1, 1) for f in feats]                    # [3P] v.repeat(num_images_per_prompt, ...)
+        feats = [f.expand(batch, -1, -1, -1).contiguous() if f.shape[0] != batch else f for f in feats]  # broadcast
+        loop_end = self._loop_end(num_inference_steps, denoising_end)
+        call = AdapterCall(feats, scale, adapter_keep(num_inference_steps, loop_end, adapter_conditioning_factor))
+        out = self._denoise_from(lat, num_inference_steps=num_inference_steps, embeds=embeds, sizes=sizes,
+                                 guidance_scale=guidance_scale, guidance_rescale=guidance_rescale,
+                                 denoising_end=denoising_end, control_guidance_start=control_guidance_start,
+                                 control_guidance_end=control_guidance_end, callback=callback,
+                                 callback_steps=callback_steps, generator=generator, adapter=call)
         return self._output(out, output_type, return_dict)

@@ -84,7 +84,7 @@ def measure(strength: float, K: int, res: int, rounds: int, replays: int) -> dic
     args = (latents, pos, neg, pooled, npooled, tid, K)
     eng.run(*args, guidance_scale=5.0, ip_scale=1.0)
     eng.run(*args, guidance_scale=5.0, ip_scale=1.0, inpaint=(image_latents, noise, mask))
-    graphs = {kind: next(g for key, (g, _) in eng._graphs.items() if key[-2] == (kind == "inpaint"))  # the ib flag
+    graphs = {kind: next(g for key, (g, _) in eng._graphs.items() if key.ib == (kind == "inpaint"))
               for kind in ("t2i", "inpaint")}
     a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     times = {"t2i": [], "inpaint": []}
