@@ -31,14 +31,19 @@ REGISTRY = {
     "ih_conv2d_scaled_f16": ["test_kernel_edges_gpu::test_conv2d_scaled_stride2_residual",
                              "test_kernel_edges_gpu::test_relu_epilogue_propagates_nan_and_inf"],
     "ih_conv2d_down_f16": ["test_img2img_gpu::test_conv_down_kernel"],
-    "ih_attention_workspace_bytes": ["test_kernels_gpu::test_attention_kv_split"],
+    "ih_attention_workspace_bytes": ["test_kernels_gpu::test_attention_kv_split",
+                                     "test_planted_gpu::test_attention_planted"],
     "ih_attention_ws_f16": ["test_kernels_gpu::test_attention", "test_kernels_gpu::test_attention_kv_split",
-                            "test_kernel_edges_gpu::test_attention_ws_f16_without_workspace"],
+                            "test_kernel_edges_gpu::test_attention_ws_f16_without_workspace",
+                            "test_planted_gpu::test_attention_planted",
+                            "test_planted_gpu::test_attention_two_segment_planted"],
     "ih_groupnorm_workspace_bytes": ["test_kernel_edges_gpu::test_groupnorm_workspace_reuse_and_graph_replay"],
     "ih_groupnorm_f16": ["test_kernel_edges_gpu::test_groupnorm_group_counts",
                          "test_kernel_edges_gpu::test_groupnorm_large_group_means",
-                         "test_kernel_edges_gpu::test_groupnorm_workspace_reuse_and_graph_replay"],
-    "ih_layernorm_f16": ["test_kernels_gpu::test_layernorm", "test_kernel_edges_gpu::test_layernorm_large_mean"],
+                         "test_kernel_edges_gpu::test_groupnorm_workspace_reuse_and_graph_replay",
+                         "test_planted_gpu::test_groupnorm_planted"],
+    "ih_layernorm_f16": ["test_kernels_gpu::test_layernorm", "test_kernel_edges_gpu::test_layernorm_large_mean",
+                         "test_planted_gpu::test_layernorm_planted"],
     "ih_linear_small_f16": ["test_kernel_edges_gpu::test_linear_small_edges"],
     "ih_attention_small_f16": ["test_kernel_edges_gpu::test_attention_small_key_tails",
                                "test_kernel_edges_gpu::test_attention_small_rejects_ragged_warp_count"],
@@ -46,7 +51,8 @@ REGISTRY = {
     "ih_add_bcast_f16": ["test_kernel_edges_gpu::test_add_bcast"],
     "ih_mean_tokens_f16": ["test_kernel_edges_gpu::test_mean_tokens"],
     "ih_softmax_rows_masked_f16": ["test_vae_gpu::test_softmax_rows_kernel",
-                                   "test_vae_gpu::test_softmax_rows_masked_kernel"],
+                                   "test_vae_gpu::test_softmax_rows_masked_kernel",
+                                   "test_planted_gpu::test_softmax_rows_masked_planted"],
     "ih_upsample2x_f16": ["test_kernels_gpu::test_upsample", "test_kernel_edges_gpu::test_upsample2x_odd"],
     "ih_concat_f16": ["test_kernel_edges_gpu::test_concat_channels"],
     "ih_im2col3x3_nchw_f16": ["test_inpaint9_gpu::test_im2col_cat_kernel_equals_im2col_of_the_concatenation"],
@@ -54,10 +60,13 @@ REGISTRY = {
     "ih_nhwc_to_nchw_f16": ["test_kernel_edges_gpu::test_nhwc_to_nchw"],
     "ih_vae_posterior_noise_f16": ["test_img2img_gpu::test_posterior_noise_kernel"],
     "ih_euler_cfg_step": ["test_kernels_gpu::test_euler_cfg_step"],
-    "ih_euler_step_ex": ["test_kernels_gpu::test_euler_step_ex"],
-    "ih_euler_inpaint_step": ["test_inpaint_gpu::test_euler_inpaint_step_kernel"],
-    "ih_dpm_solver_step": ["test_dpm_gpu::test_dpm_solver_step_kernel"],
-    "ih_euler_ancestral_step": ["test_euler_a_gpu::test_euler_ancestral_step_kernel"],
+    "ih_euler_step_ex": ["test_kernels_gpu::test_euler_step_ex", "test_planted_gpu::test_step_kernels_rescale_planted"],
+    "ih_euler_inpaint_step": ["test_inpaint_gpu::test_euler_inpaint_step_kernel",
+                              "test_planted_gpu::test_step_kernels_rescale_planted"],
+    "ih_dpm_solver_step": ["test_dpm_gpu::test_dpm_solver_step_kernel",
+                           "test_planted_gpu::test_step_kernels_rescale_planted"],
+    "ih_euler_ancestral_step": ["test_euler_a_gpu::test_euler_ancestral_step_kernel",
+                                "test_planted_gpu::test_step_kernels_rescale_planted"],
     "ih_euler_ancestral_scale_input": ["test_euler_a_gpu::test_first_input_equals_torch_scale_model_input"],
     "ih_scale_model_input_ex": ["test_kernels_gpu::test_euler_cfg_step",
                                 "test_kernel_edges_gpu::test_scale_model_input_entry"],
