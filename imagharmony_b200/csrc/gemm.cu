@@ -554,21 +554,36 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_f16_kernel(const __grid_
 //
 // In gemm_f16_kernel both MMA warpgroups share every tile, so the tensor cores idle through each epilogue; with the
 // 10-20 k-blocks of a transformer GEMM that is about half of a multi-round launch.  Here each MMA warpgroup owns WHOLE
-// 128 x 128 tiles (two m64n128 blocks, 128 accumulator registers): CTA c walks tiles c, c + grid, ... and hands them to
-// warpgroup 1, 2, 1, 2, ..., so one warpgroup's epilogue runs under the other's main loop.  Each MMA warpgroup has its
-// own stage ring, filled by its own producer warp (warp 0 for warpgroup 1, warp 2 for warpgroup 2): every ring has
-// one producer and one consumer, as in gemm_f16_kernel.  The main loops take turns through two named barriers (as
-// CUTLASS's ping-pong does), so that the two warpgroups' epilogues do not fall together.
+// 128 x 128 tiles (two m64n128 blocks, 128 accumulator registers): CTA c walks tiles c, c + grid, ... (numbered as in
+// pp_tile_coords) and hands them to warpgroup 1, 2, 1, 2, ..., so one warpgroup's epilogue runs under the other's main
+// loop.  One producer warp fills one stage ring with the k-blocks of all the CTA's tiles in that order, and the two MMA
+// warpgroups consume it in turn (as CUTLASS's ping-pong does): the running main loop has the whole ring of loads in
+// flight ahead of it, instead of half of it while the idle warpgroup's half sits full.  The main loops take turns
+// through two named barriers, so the two warpgroups' epilogues do not fall together.
 // The epilogue is gemm_f16_kernel's expressions in the same order -- the LayerNorm statistics summed in slab order,
 // fmaf(rstd, acc, bias), gelu_erf_f on the gate, pack_half2 -- so the outputs are bitwise equal to it.  The LayerNorm
 // statistics of the tile's rows and its bias columns are fetched during the main loop.
 // ------------------------------------------------------------------------------------------------
-constexpr int PP_STAGES = 3;      // per MMA warpgroup
+constexpr int PP_STAGES = 6;      // one ring, shared by both MMA warpgroups
 constexpr int PP_BN = 128;        // B-tile rows (GEGLU: 64 value + 64 gate rows, 64 outputs)
 // named barriers (gemm_f16_kernel uses 1 and 2): 3 + wg lets warpgroup wg start its next main loop, 5 + wg is its
 // epilogue barrier
 constexpr int PP_BAR_ORDER = 3;
 constexpr int PP_BAR_EPI = 5;
+
+// Tile order: bands of PP_BAND row tiles, M fastest inside a band.  The 132 tiles in flight then share 16 A row
+// blocks and about 8 weight column blocks, instead of (N fastest) reading the whole weight -- 26 MB for a 1024^2
+// GEGLU-in -- for every 1.6 rows of tiles, or (M fastest) the whole of a tall A for every column.  A permutation of
+// whole tiles: each output element is computed as before.  The last band may be narrower.
+constexpr int PP_BAND = 16;
+
+__device__ __forceinline__ void pp_tile_coords(int tile, int n_tiles, int m_tiles, int& m_tile, int& n_tile) {
+  const int first = tile / (PP_BAND * n_tiles) * PP_BAND;
+  const int rows = min(PP_BAND, m_tiles - first);
+  const int r = tile - first * n_tiles;
+  m_tile = first + r % rows;
+  n_tile = r / rows;
+}
 
 struct PpOperands {   // one MMA warpgroup's epilogue operands of its current tile
   float rstd[BM];      // alpha (LayerNorm folded: alpha / std) of every tile row
@@ -579,14 +594,13 @@ template <bool GEGLU>
 struct PpSmem {
   static constexpr int STAGE_BYTES = A_STAGE_BYTES + PP_BN * BK * 2;   // 32 KiB
   static constexpr int RING_BYTES = PP_STAGES * STAGE_BYTES;
-  static constexpr int TILE_BYTES = 2 * RING_BYTES;
   static constexpr int BN_OUT = GEGLU ? PP_BN / 2 : PP_BN;
   static constexpr int SLABS = BN_OUT / 64;
   static constexpr int SLAB_BYTES = BM * 64 * 2;
   static constexpr int STG_BYTES = 2 * SLAB_BYTES;   // one staging slab per MMA warpgroup
-  static constexpr int BAR_BYTES = 128;              // full and empty barriers of both rings
-  static constexpr int TOTAL = TILE_BYTES + STG_BYTES + BAR_BYTES + 2 * sizeof(PpOperands) + 1024;   // + alignment slack
-  static_assert(4 * PP_STAGES * 8 <= BAR_BYTES, "ping-pong GEMM barriers");
+  static constexpr int BAR_BYTES = 128;              // full and empty barriers of the ring
+  static constexpr int TOTAL = RING_BYTES + STG_BYTES + BAR_BYTES + 2 * sizeof(PpOperands) + 1024;   // + alignment slack
+  static_assert(2 * PP_STAGES * 8 <= BAR_BYTES, "ping-pong GEMM barriers");
   static_assert(TOTAL <= GemmSmem<128, 6, false>::SMEM_LIMIT, "ping-pong GEMM shared-memory budget exceeded");
 };
 
@@ -598,9 +612,9 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_pp_f16_kernel(const __gr
   using S = PpSmem<GEGLU>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* stg = smem + S::TILE_BYTES;
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + S::TILE_BYTES + S::STG_BYTES);   // [ring][stage]
-  uint64_t* empty_bar = full_bar + 2 * PP_STAGES;
+  uint8_t* stg = smem + S::RING_BYTES;
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + S::RING_BYTES + S::STG_BYTES);
+  uint64_t* empty_bar = full_bar + PP_STAGES;
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -620,9 +634,9 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_pp_f16_kernel(const __gr
     tma_prefetch_desc(&amap);
     tma_prefetch_desc(&bmap);
     tma_prefetch_desc(&omap);
-    for (int s = 0; s < 2 * PP_STAGES; ++s) {
+    for (int s = 0; s < PP_STAGES; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 4);   // lane 0 of the four warps of the ring's MMA warpgroup
+      mbar_init(&empty_bar[s], 4);   // lane 0 of the four warps of the MMA warpgroup that consumed the stage
     }
     fence_barrier_init();
   }
@@ -635,26 +649,24 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_pp_f16_kernel(const __gr
   if (warp < 4) {
     // ------------------------------ producer warpgroup ------------------------------
     setmaxnreg_dec<40>();
-    if (warp == 0 || warp == 2) {
-      // the ring of MMA warpgroup `ring`, which takes every other tile of the CTA
-      const int ring = warp >> 1;
-      uint8_t* ring_smem = smem + ring * S::RING_BYTES;
-      uint64_t* ring_full = full_bar + ring * PP_STAGES;
-      uint64_t* ring_empty = empty_bar + ring * PP_STAGES;
+    if (warp == 0) {
+      // every k-block of the CTA's tiles, in the order the two MMA warpgroups take them
       int stage = 0;
       uint32_t phase = 0;
-      for (int tile = blockIdx.x + ring * gridDim.x; tile < num_tiles; tile += 2 * gridDim.x) {
-        const int n0 = (tile % n_tiles) * BN_OUT;
-        const int m0 = (tile / n_tiles) * BM;
+      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+        int m_tile, n_tile;
+        pp_tile_coords(tile, n_tiles, p.m_tiles, m_tile, n_tile);
+        const int n0 = n_tile * BN_OUT;
+        const int m0 = m_tile * BM;
         for (int kb = 0; kb < p.num_kb; ++kb) {
-          mbar_wait(&ring_empty[stage], phase ^ 1);
-          uint8_t* sA = ring_smem + stage * S::STAGE_BYTES;
+          mbar_wait(&empty_bar[stage], phase ^ 1);
+          uint8_t* sA = smem + stage * S::STAGE_BYTES;
           uint8_t* sB = sA + A_STAGE_BYTES;
           if (elect_one()) {
-            mbar_arrive_expect_tx(&ring_full[stage], S::STAGE_BYTES);
-            tma_load_2d(sA, &amap, &ring_full[stage], kb * BK, m0);
-            tma_load_2d(sB, &bmap, &ring_full[stage], kb * BK, n0);
-            if (GEGLU) tma_load_2d(sB + (PP_BN / 2) * BK * 2, &bmap, &ring_full[stage], kb * BK, p.gate_row_off + n0);
+            mbar_arrive_expect_tx(&full_bar[stage], S::STAGE_BYTES);
+            tma_load_2d(sA, &amap, &full_bar[stage], kb * BK, m0);
+            tma_load_2d(sB, &bmap, &full_bar[stage], kb * BK, n0);
+            if (GEGLU) tma_load_2d(sB + (PP_BN / 2) * BK * 2, &bmap, &full_bar[stage], kb * BK, p.gate_row_off + n0);
           }
           __syncwarp();
           if (++stage == PP_STAGES) {
@@ -682,19 +694,15 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_pp_f16_kernel(const __gr
     const int t = threadIdx.x & 127;
     const bool issuer = t == 0;
     uint8_t* my_stg = stg + wg * S::SLAB_BYTES;
-    uint8_t* ring_smem = smem + wg * S::RING_BYTES;
-    uint64_t* ring_full = full_bar + wg * PP_STAGES;
-    uint64_t* ring_empty = empty_bar + wg * PP_STAGES;
-    PpOperands* my_ops = reinterpret_cast<PpOperands*>(smem + S::TILE_BYTES + S::STG_BYTES + S::BAR_BYTES) + wg;
+    PpOperands* my_ops = reinterpret_cast<PpOperands*>(smem + S::RING_BYTES + S::STG_BYTES + S::BAR_BYTES) + wg;
     const int ln_n = p.ln_stats ? p.ln_slabs : 0;
     const float2* ln_st = reinterpret_cast<const float2*>(p.ln_stats);   // [slab][row]
-    int stage = 0;
-    uint32_t phase = 0;
     float acc[2][PP_BN / 2];
     int j = wg;   // index of the tile among this CTA's tiles
     for (int tile = blockIdx.x + wg * gridDim.x; tile < num_tiles; tile += 2 * gridDim.x, j += 2) {
-      const int n0 = (tile % n_tiles) * BN_OUT;
-      const int m_tile = tile / n_tiles;
+      int m_tile, n_tile;
+      pp_tile_coords(tile, n_tiles, p.m_tiles, m_tile, n_tile);
+      const int n0 = n_tile * BN_OUT;
       // epilogue operands, fetched behind the main loop and handed over in shared memory: the warpgroup's thread t
       // sums the LayerNorm statistics of tile row t, the load of slab kb + 1 in flight behind k-block kb, and threads
       // 0..63 fetch one bias pair each (GEGLU: 32 value pairs, then 32 gate pairs)
@@ -719,11 +727,21 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_pp_f16_kernel(const __gr
 
       // ---- main loop, after the other warpgroup has issued all of the CTA's previous tile
       if (j > 0) named_bar_sync(PP_BAR_ORDER + wg, 256);
+      // The tile's k-blocks are the ring's k-blocks g = j num_kb, j num_kb + 1, ...; k-block g fills stage g % STAGES in
+      // the stage's phase g / STAGES.  A parity wait cannot tell phase n from phase n - 2, so it is only sound if the
+      // stage's full barrier has completed at least g / STAGES phases when the wait starts, i.e. if k-block g - STAGES
+      // has landed.  The turn-taking above gives that: every k-block before g belongs to an earlier tile of this CTA,
+      // and the main loop of that tile (this warpgroup's, or the other's, which passed the named barrier only after its
+      // last wait) has waited for it.  Nor can the barrier be a phase further on: the producer refills a stage only
+      // after the warpgroup that waits on it has freed it.
+      const int g = j * p.num_kb;
+      int stage = g % PP_STAGES;
+      uint32_t phase = (g / PP_STAGES) & 1;
       int prev = -1;
       for (int kb = 0; kb < p.num_kb; ++kb) {
-        mbar_wait(&ring_full[stage], phase);
+        mbar_wait(&full_bar[stage], phase);
         if (issuer && j == 0 && kb == 0) stamp(3);
-        const uint32_t a_addr = smem_u32(ring_smem + stage * S::STAGE_BYTES);
+        const uint32_t a_addr = smem_u32(smem + stage * S::STAGE_BYTES);
         const uint64_t a_desc0 = wgmma_desc_sw128(a_addr);
         const uint64_t a_desc1 = wgmma_desc_sw128(a_addr + 64 * 128);
         const uint64_t b_desc = wgmma_desc_sw128(a_addr + A_STAGE_BYTES);
@@ -736,7 +754,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_pp_f16_kernel(const __gr
         wgmma_commit();
         if (prev >= 0) {
           wgmma_wait<1>();
-          if (lane == 0) mbar_arrive(&ring_empty[prev]);
+          if (lane == 0) mbar_arrive(&empty_bar[prev]);
         }
         prev = stage;
         if (++stage == PP_STAGES) {
@@ -751,7 +769,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_pp_f16_kernel(const __gr
       wgmma_wait<0>();
       fence_regs(acc[0]);
       fence_regs(acc[1]);
-      if (lane == 0) mbar_arrive(&ring_empty[prev]);
+      if (lane == 0) mbar_arrive(&empty_bar[prev]);
       if (issuer) stamp(4 + (j < 3 ? j : 3));
 
       // ---- epilogue: the same expressions in the same order as gemm_f16_kernel
@@ -911,24 +929,24 @@ static int pick_bn(long long m_tiles, int N, int num_kb, bool allow160, double* 
 // Whether the ping-pong kernel beats gemm_f16_kernel's choice.  Both are linear models of the launch time in us, fitted
 // to tools/ab_probe.py pp (the LayerNorm-folded q|k|v and GEGLU launches of the SDXL base and refiner UNets at 512^2 -
 // 1024^2, 1 and 4 images; H100 80GB HBM3 at a 700 W power limit; DESIGN section 3), in the rounds R of tiles per SM:
-//   ping-pong, plain  0.461 R kb + 0.898 R + 3.21     (128 x 128 tiles; within 8 % of the table)
-//   ping-pong, GEGLU  0.650 R kb - 1.03 R + 5.81      (64 outputs per tile; within 13 %)
-//   old, plain        0.627 (pick_bn's cost) + 1.33   (within 17 %)
-//   old, GEGLU        0.969 R kb + 6.95 R - 1.28      (the 256-row tile, 128 outputs; within 7 %)
-// The ping-pong GEGLU tile spends more per k-block (its epilogue is as long as the main loop) and nothing per round, so
-// it wins up to about 20 k-blocks (K = 1280).  The GEGLU per-k-block coefficient is the least-squares one lowered from
-// 0.674 to 0.650, which minimises the time lost to wrong picks over the table (12.6 us in all, at K = 1536).
+//   ping-pong, plain  0.491 R kb + 0.515 R + 1.88     (128 x 128 tiles; within 12 % of the table)
+//   ping-pong, GEGLU  0.479 R kb + 1.49 R - 1.18      (64 outputs per tile; within 17 %)
+//   old, plain        0.620 (pick_bn's cost) + 2.35   (within 18 %)
+//   old, GEGLU        0.972 R kb + 7.03 R - 1.73      (the 256-row tile, 128 outputs; within 10 %)
+// These least-squares fits pick the faster kernel at every shape of the table.  The ping-pong GEGLU tile costs half as
+// much per k-block of output as the 256-row tile and little per round, so it wins at every GEGLU shape of the table,
+// the refiner's K = 1536 included.
 static bool pick_pp(long long m_tiles, int N, int num_kb, bool geglu) {
   const int sms = num_sms();
   auto rounds = [&](int cols) { return (double)((m_tiles * ((N + cols - 1) / cols) + sms - 1) / sms); };
   if (geglu) {
-    const double pp = rounds(64) * (0.650 * num_kb - 1.03) + 5.81;
-    const double old = rounds(128) * (0.969 * num_kb + 6.95) - 1.28;
+    const double pp = rounds(64) * (0.479 * num_kb + 1.49) - 1.18;
+    const double old = rounds(128) * (0.972 * num_kb + 7.03) - 1.73;
     return pp < old;
   }
   double cost;
   if (pick_bn(m_tiles, N, num_kb, true, &cost) == 64) return false;   // one round of narrow tiles: not in the table
-  return rounds(128) * (0.461 * num_kb + 0.898) + 3.21 < 0.627 * cost + 1.33;
+  return rounds(128) * (0.491 * num_kb + 0.515) + 1.88 < 0.620 * cost + 2.35;
 }
 
 static int dispatch(const TmapSet4& amaps, const OutView& ov, const void* w, int ldw_rows, long long K, GemmParams& p,

@@ -1,4 +1,5 @@
-"""Ramp breakdown of one GEMM launch inside a dependent chain (globaltimer stamps of CTA 0)."""
+"""Ramp breakdown of one GEMM launch inside a dependent chain (globaltimer stamps of CTA 0).  `python
+tools/gemm_trace.py pp` traces the ping-pong kernel at the q|k|v and GEGLU launches of a 1024^2 step."""
 import os
 import sys
 
@@ -39,6 +40,45 @@ def run(label, M, N, K, geglu=False, tn=0, full=False):
     print(label, f"event {s.elapsed_time(e) * 1e3:.1f} us |", ", ".join(f"{n}={v:.2f}" for n, v in zip(names, rel) if v is not None))
     buf.zero_()
 
+
+def run_pp(label, M, C, geglu):
+    """One LayerNorm-folded q|k|v (N = 3C) or GEGLU (N = 8C) launch with bias on the ping-pong kernel.  CTA 0's stamps
+    give the accumulator-ready times of its first three tiles (warpgroups 1, 2, 1) and of its last; from the second tile
+    on the main loops run back to back, so the gap between consecutive ready stamps is one tile's main loop."""
+    N = 8 * C if geglu else 3 * C
+    x = torch.randn(M, C, device="cuda").half()
+    w = (torch.randn(N, C, device="cuda") * C ** -0.5).half()
+    b = torch.randn(N, device="cuda").half()
+    st = torch.rand((C // 64, M, 2), device="cuda")
+    st[..., 1] += 64.0
+    for _ in range(3):
+        ops.linear(x, w, b, geglu=geglu, ln=(st, 1e-5), tile_n=ops.TILE_PINGPONG)
+    torch.cuda.synchronize()
+    lib.ih_gemm_set_trace(buf.data_ptr())
+    s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    s.record()
+    ops.linear(x, w, b, geglu=geglu, ln=(st, 1e-5), tile_n=ops.TILE_PINGPONG)
+    e.record()
+    torch.cuda.synchronize()
+    lib.ih_gemm_set_trace(None)
+    t = [(v - buf[0].item()) / 1e3 for v in buf.cpu().tolist()[:9]]
+    buf.zero_()
+    kb = C // 64
+    sms = torch.cuda.get_device_properties(0).multi_processor_count
+    tiles = -(-M // 128) * -(-(N // 2 if geglu else N) // (64 if geglu else 128))
+    loops = [t[5] - t[4], t[6] - t[5]]
+    print(f"{label} M{M} N{N} K{C}: kb {kb}, tiles/SM {tiles / sms:.2f}, event {s.elapsed_time(e) * 1e3:.1f} us | "
+          f"first stage {t[3]:.2f}, tile 0 ready {t[4]:.2f}, main loops of tiles 1, 2 "
+          f"{loops[0]:.2f}, {loops[1]:.2f} us ({sum(loops) / (2 * kb):.3f} us per k-block), last tile ready {t[7]:.2f}, "
+          f"cta done {t[8]:.2f}", flush=True)
+
+
+if len(sys.argv) > 1 and sys.argv[1] == "pp":
+    # the ping-pong launches of a 1024^2 step with CFG (batch 2): level 1 (res / 16, C 640), level 2 (res / 32, C 1280)
+    for lvl, (M, C) in enumerate([(2 * 64 * 64, 640), (2 * 32 * 32, 1280)], 1):
+        for geglu in (False, True):
+            run_pp(f"level {lvl} {'GEGLU' if geglu else 'q|k|v'}", M, C, geglu)
+    sys.exit(0)
 
 run("1 tile 128x256x64      ", 128, 256, 64, tn=256)
 run("1280^2 (80 tiles)      ", 2048, 1280, 1280, tn=256)
