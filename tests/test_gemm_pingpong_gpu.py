@@ -1,9 +1,13 @@
 """GPU tests of the ping-pong GEMM kernel (gemm_pp_f16_kernel, forced with tile_n = TILE_PINGPONG): its outputs must be
 bitwise equal to gemm_f16_kernel's -- the 256-row tile for GEGLU, the plain tiles for q|k|v -- because the automatic
-choice switches between the two kernels by shape."""
+choice switches between the two kernels by shape; and, with exact small-integer operands (tests/exact_gemm.py), equal
+to the fp64 reference, bit for bit or within 1 ulp behind the LayerNorm fold, so that a defect both kernels share
+fails too."""
 import pytest
 import torch
 import torch.nn.functional as F
+
+import exact_gemm as E
 
 pytestmark = pytest.mark.gpu
 
@@ -52,7 +56,25 @@ def check_equal(ops, m, n, k, geglu, bias=True, ln=True, seed=0):
         y = x.float() @ w.float().t() + (0 if b is None else b.float())
         want = y[:, :n // 2] * F.gelu(y[:, n // 2:]) if geglu else y
         torch.testing.assert_close(pp.float(), want, rtol=2e-3, atol=2e-3)
+    check_exact(ops, m, n, k, geglu, bias, ln, seed)
     return pp
+
+
+def check_exact(ops, m, n, k, geglu, bias, ln, seed):
+    """The same launch shape with exact integer operands against the fp64 reference: bit for bit, or with the
+    LayerNorm fold within 1 fp16 ulp.  GEGLU always takes its gate bias here (it keeps the gates saturated, which makes
+    GEGLU exact)."""
+    c = E.gemm_case(m, n, k, seed=seed + 101, bias=bias or geglu, geglu=geglu, ln=ln, device="cuda")
+    ref, pre = E.gemm_ref(c)
+    E.gemm_check_bounds(c, ref, pre)
+    st = c["ln_stats"] if ln else None
+    pp = launch(ops, c["a"], c["w"], c.get("bias"), geglu, st, ops.TILE_PINGPONG)
+    assert torch.equal(pp, launch(ops, c["a"], c["w"], c.get("bias"), geglu, st, old_tile(geglu)))
+    if ln:
+        r = E.ratio(pp, ref, 1.0, c["slack"])
+        assert r <= 1.0, (m, n, k, geglu, bias, "err / 1-ulp bar", r)
+    else:
+        assert E.check_bits(pp, ref) == 0, (m, n, k, geglu, bias, E.first_mismatch(pp, ref, 64 if geglu else 128))
 
 
 # the LayerNorm-folded q|k|v (N = 3C) and GEGLU (N = 8C) launches of the SDXL base UNet (C 640 / 1280) and refiner

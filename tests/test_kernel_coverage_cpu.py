@@ -21,16 +21,27 @@ EXEMPT = {
 }
 
 REGISTRY = {
-    "ih_gemm_f16": ["test_kernels_gpu::test_gemm_plain", "test_kernel_edges_gpu::test_gemm_epilogue_matrix"],
+    "ih_gemm_f16": ["test_kernels_gpu::test_gemm_plain", "test_kernel_edges_gpu::test_gemm_epilogue_matrix",
+                    "test_exact_gemm_gpu::test_ring_positions", "test_exact_gemm_gpu::test_plain_epilogues",
+                    "test_exact_gemm_gpu::test_geglu_epilogues", "test_exact_gemm_gpu::test_sdxl_shapes_library_choice",
+                    "test_exact_gemm_gpu::test_conv_in_im2col_gemm"],
     "ih_gemm_ln_f16": ["test_kernels_gpu::test_gemm_layernorm_fold", "test_kernel_edges_gpu::test_gemm_epilogue_matrix",
-                       "test_kernel_edges_gpu::test_layernorm_fold_accuracy_envelope"],
+                       "test_kernel_edges_gpu::test_layernorm_fold_accuracy_envelope",
+                       "test_exact_gemm_gpu::test_plain_epilogues", "test_exact_gemm_gpu::test_geglu_epilogues",
+                       "test_exact_gemm_gpu::test_stats_chain_feeds_layernorm_fold"],
     "ih_gemm_scaled_f16": ["test_kernel_edges_gpu::test_gemm_alpha_with_residual_and_gelu",
-                           "test_kernel_edges_gpu::test_relu_epilogue_propagates_nan_and_inf"],
-    "ih_conv2d_f16": ["test_kernels_gpu::test_conv3x3", "test_kernel_edges_gpu::test_conv3x3_rowbias_every_tile"],
-    "ih_conv2d_shortcut_f16": ["test_kernels_gpu::test_conv3x3_fused_shortcut"],
+                           "test_kernel_edges_gpu::test_relu_epilogue_propagates_nan_and_inf",
+                           "test_exact_gemm_gpu::test_scaled_epilogues"],
+    "ih_conv2d_f16": ["test_kernels_gpu::test_conv3x3", "test_kernel_edges_gpu::test_conv3x3_rowbias_every_tile",
+                      "test_exact_gemm_gpu::test_conv_levels", "test_exact_gemm_gpu::test_conv_every_spatial_tile",
+                      "test_exact_gemm_gpu::test_conv_forced_tiles"],
+    "ih_conv2d_shortcut_f16": ["test_kernels_gpu::test_conv3x3_fused_shortcut", "test_exact_gemm_gpu::test_conv_levels"],
     "ih_conv2d_scaled_f16": ["test_kernel_edges_gpu::test_conv2d_scaled_stride2_residual",
-                             "test_kernel_edges_gpu::test_relu_epilogue_propagates_nan_and_inf"],
-    "ih_conv2d_down_f16": ["test_img2img_gpu::test_conv_down_kernel"],
+                             "test_kernel_edges_gpu::test_relu_epilogue_propagates_nan_and_inf",
+                             "test_exact_gemm_gpu::test_conv_levels"],
+    "ih_conv2d_down_f16": ["test_img2img_gpu::test_conv_down_kernel", "test_exact_gemm_gpu::test_conv_levels",
+                           "test_exact_gemm_gpu::test_conv_every_spatial_tile",
+                           "test_exact_gemm_gpu::test_conv_forced_tiles"],
     "ih_attention_workspace_bytes": ["test_kernels_gpu::test_attention_kv_split",
                                      "test_planted_gpu::test_attention_planted"],
     "ih_attention_ws_f16": ["test_kernels_gpu::test_attention", "test_kernels_gpu::test_attention_kv_split",
@@ -55,8 +66,10 @@ REGISTRY = {
                                    "test_planted_gpu::test_softmax_rows_masked_planted"],
     "ih_upsample2x_f16": ["test_kernels_gpu::test_upsample", "test_kernel_edges_gpu::test_upsample2x_odd"],
     "ih_concat_f16": ["test_kernel_edges_gpu::test_concat_channels"],
-    "ih_im2col3x3_nchw_f16": ["test_inpaint9_gpu::test_im2col_cat_kernel_equals_im2col_of_the_concatenation"],
-    "ih_im2col3x3_nchw_cat_f16": ["test_inpaint9_gpu::test_im2col_cat_kernel_equals_im2col_of_the_concatenation"],
+    "ih_im2col3x3_nchw_f16": ["test_inpaint9_gpu::test_im2col_cat_kernel_equals_im2col_of_the_concatenation",
+                              "test_exact_gemm_gpu::test_conv_in_im2col_gemm"],
+    "ih_im2col3x3_nchw_cat_f16": ["test_inpaint9_gpu::test_im2col_cat_kernel_equals_im2col_of_the_concatenation",
+                                  "test_exact_gemm_gpu::test_conv_in_im2col_gemm"],
     "ih_nhwc_to_nchw_f16": ["test_kernel_edges_gpu::test_nhwc_to_nchw"],
     "ih_vae_posterior_noise_f16": ["test_img2img_gpu::test_posterior_noise_kernel"],
     "ih_euler_cfg_step": ["test_kernels_gpu::test_euler_cfg_step"],
