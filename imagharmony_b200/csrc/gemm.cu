@@ -107,6 +107,67 @@ struct GemmSmem {
 constexpr int GEMM_THREADS = 384;   // warpgroup 0 producer, warpgroups 1-2 MMA + epilogue (64 tile rows each)
 constexpr int GEMM_MMA_THREADS = 256;
 
+// ---- device code shared by gemm_f16_kernel and gemm_pp_f16_kernel
+
+// %globaltimer stamp `slot` of CTA 0 (ih_gemm_set_trace)
+__device__ __forceinline__ void trace_stamp(const GemmParams& p, int slot) {
+  if (p.trace && blockIdx.x == 0) {
+    unsigned long long t;
+    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+    p.trace[slot] = t;
+  }
+}
+
+// this CTA's 1/gridDim slice of the next kernel's weights -> L2 (a hint: no completion to wait for)
+__device__ __forceinline__ void prefetch_next_weights(const GemmParams& p) {
+  constexpr unsigned long long CH = 16384;
+  const unsigned long long per = ((p.pf_bytes / gridDim.x) + CH - 1) / CH * CH;
+  unsigned long long off = per * blockIdx.x;
+  const unsigned long long end = off + per < p.pf_bytes ? off + per : p.pf_bytes;
+  for (; off < end; off += CH) {
+    const unsigned long long n = end - off < CH ? ((end - off) & ~15ull) : CH;
+    if (n) l2_prefetch_bulk(p.pf_ptr + off, (uint32_t)n);
+  }
+}
+
+template <int STAGES>
+__device__ __forceinline__ void ring_advance(int& stage, uint32_t& phase) {
+  if (++stage == STAGES) {
+    stage = 0;
+    phase ^= 1;
+  }
+}
+
+// k-block kb of the B tile: BN weight rows from n0, or with GEGLU the value rows n0.. and the gate rows
+// gate_row_off + n0.., BN / 2 each
+template <int BN, bool GEGLU>
+__device__ __forceinline__ void load_weight_tile(uint8_t* sB, const CUtensorMap* bmap, uint64_t* bar, int kb, int n0,
+                                                 int gate_row_off) {
+  tma_load_2d(sB, bmap, bar, kb * BK, n0);
+  if (GEGLU) tma_load_2d(sB + (BN / 2) * BK * 2, bmap, bar, kb * BK, gate_row_off + n0);
+}
+
+// folded LayerNorm: alpha / std of a row from the totals of its statistics slots
+__device__ __forceinline__ float ln_rstd(const GemmParams& p, float ssum, float ssq) {
+  const float ln_mean = ssum * p.ln_inv_c;
+  const float var = fmaxf(ssq * p.ln_inv_c - ln_mean * ln_mean, 0.f);
+  return p.alpha * rsqrtf(var + p.ln_eps);
+}
+
+// One output pair before the optional row bias, activation, residual and ReLU: rstd * acc + bias, with GEGLU times
+// gelu(rstd * gate + gate bias).  acc[v], acc[v + 1] are the pair's accumulators, acc[g], acc[g + 1] its gate's.  Both
+// kernels compute their outputs through this, so the ping-pong kernel's are bitwise equal to gemm_f16_kernel's.
+template <bool GEGLU, int N>
+__device__ __forceinline__ float2 epilogue_pair(const float (&acc)[N], int v, int g, float rstd, const float2& bv,
+                                                const float2& bg) {
+  float2 x = make_float2(fmaf(rstd, acc[v], bv.x), fmaf(rstd, acc[v + 1], bv.y));
+  if (GEGLU) {
+    x.x *= gelu_erf_f(fmaf(rstd, acc[g], bg.x));
+    x.y *= gelu_erf_f(fmaf(rstd, acc[g + 1], bg.y));
+  }
+  return x;
+}
+
 // Persistent kernel: grid = min(#tiles, #SMs); every CTA walks tiles blockIdx.x, +gridDim.x, ...  The stage ring runs
 // continuously across tiles.
 template <int BN, int STAGES, bool GEGLU>
@@ -127,14 +188,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_f16_kernel(const __grid_
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  auto stamp = [&](int slot) {
-    if (p.trace && blockIdx.x == 0) {
-      unsigned long long t;
-      asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-      p.trace[slot] = t;
-    }
-  };
-  if (threadIdx.x == 0) stamp(0);
+  if (threadIdx.x == 0) trace_stamp(p, 0);
   constexpr int BN_OUT = GEGLU ? BN / 2 : BN;
   const int n_tiles = (p.N + BN_OUT - 1) / BN_OUT;
   const int num_tiles = n_tiles * p.m_tiles;
@@ -152,10 +206,10 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_f16_kernel(const __grid_
     fence_barrier_init();
   }
   __syncthreads();
-  if (threadIdx.x == 0) stamp(1);
+  if (threadIdx.x == 0) trace_stamp(p, 1);
   pdl_launch_dependents();  // the next kernel may begin its prologue now ...
   pdl_wait();               // ... and we may not touch global memory before our predecessor has finished
-  if (threadIdx.x == 0) stamp(2);
+  if (threadIdx.x == 0) trace_stamp(p, 2);
 
   if (warp < 4) {
     // ------------------------------ producer warpgroup ------------------------------
@@ -197,30 +251,14 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_f16_kernel(const __grid_
               tma_load_4d(sA, &amaps.m[p.tap_map[tap]], &full_bar[stage], ckb * BK, x0 + p.tap_ox[tap],
                           y0 + p.tap_oy[tap], img);
             }
-            if (GEGLU) {
-              tma_load_2d(sB, &bmap, &full_bar[stage], kb * BK, n0);
-              tma_load_2d(sB + (BN / 2) * BK * 2, &bmap, &full_bar[stage], kb * BK, p.gate_row_off + n0);
-            } else {
-              tma_load_2d(sB, &bmap, &full_bar[stage], kb * BK, n0);
-            }
+            load_weight_tile<BN, GEGLU>(sB, &bmap, &full_bar[stage], kb, n0, p.gate_row_off);
           }
           __syncwarp();
-          if (++stage == STAGES) {
-            stage = 0;
-            phase ^= 1;
-          }
+          ring_advance<STAGES>(stage, phase);
         }
       }
     } else if (warp == 1 && lane == 0 && p.pf_ptr) {
-      // my 1/gridDim slice of the next kernel's weights -> L2 (a hint: no completion to wait for)
-      constexpr unsigned long long CH = 16384;
-      const unsigned long long per = ((p.pf_bytes / gridDim.x) + CH - 1) / CH * CH;
-      unsigned long long off = per * blockIdx.x;
-      const unsigned long long end = off + per < p.pf_bytes ? off + per : p.pf_bytes;
-      for (; off < end; off += CH) {
-        const unsigned long long n = end - off < CH ? ((end - off) & ~15ull) : CH;
-        if (n) l2_prefetch_bulk(p.pf_ptr + off, (uint32_t)n);
-      }
+      prefetch_next_weights(p);
     }
   } else {
     // ------------------------------ MMA + epilogue warpgroups ------------------------------
@@ -283,7 +321,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_f16_kernel(const __grid_
       int prev = -1;
       for (int kb = 0; kb < p.num_kb; ++kb) {
         mbar_wait(&full_bar[stage], phase);
-        if (issuer && it == 0 && kb == 0) stamp(3);
+        if (issuer && it == 0 && kb == 0) trace_stamp(p, 3);
         const uint32_t a_addr = smem_u32(smem + stage * S::STAGE_BYTES) + wg * (64 * 128);
         const uint32_t b_addr = smem_u32(smem + stage * S::STAGE_BYTES + A_STAGE_BYTES);
         const uint64_t a_desc = wgmma_desc_sw128(a_addr);
@@ -298,6 +336,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_f16_kernel(const __grid_
           if (lane == 0) mbar_arrive(&empty_bar[prev]);
         }
         prev = stage;
+        // ring_advance, written out: through the helper ptxas allocates this loop's uniform registers differently
         if (++stage == STAGES) {
           stage = 0;
           phase ^= 1;
@@ -306,7 +345,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_f16_kernel(const __grid_
       wgmma_wait<0>();
       fence_regs(acc);
       if (lane == 0) mbar_arrive(&empty_bar[prev]);
-      if (issuer) stamp(4 + (it < 3 ? it : 3));
+      if (issuer) trace_stamp(p, 4 + (it < 3 ? it : 3));
 
       // ---- epilogue: registers -> bias / LN-fold / activation / GEGLU / residual -> fp16 pairs in the 128B-swizzled
       // staging slab -> TMA store (clipped at the M / N / image edges by the tensor map)
@@ -347,9 +386,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_f16_kernel(const __grid_
               ssq += t[i].y;
             }
           }
-          const float ln_mean = ssum * p.ln_inv_c;
-          const float var = fmaxf(ssq * p.ln_inv_c - ln_mean * ln_mean, 0.f);
-          rstd[h] = p.alpha * rsqrtf(var + p.ln_eps);
+          rstd[h] = ln_rstd(p, ssum, ssq);
         }
       }
       if constexpr (FAST_EPI) {
@@ -376,11 +413,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_f16_kernel(const __grid_
           }
 #pragma unroll
           for (int h = 0; h < 2; ++h) {
-            if (ok[h]) {
-              const float ln_mean = ssum[h] * p.ln_inv_c;
-              const float var = fmaxf(ssq[h] * p.ln_inv_c - ln_mean * ln_mean, 0.f);
-              rstd[h] = p.alpha * rsqrtf(var + p.ln_eps);
-            }
+            if (ok[h]) rstd[h] = ln_rstd(p, ssum[h], ssq[h]);
           }
         }
         // lazy store drain: without a residual nothing writes staging between the last slab of one tile and the first
@@ -445,13 +478,9 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_f16_kernel(const __grid_
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
               const int r = r0 + 8 * h;
-              float x0v = fmaf(rstd[h], acc[4 * i + 2 * h], bv.x);
-              float x1v = fmaf(rstd[h], acc[4 * i + 2 * h + 1], bv.y);
-              if (GEGLU) {
-                constexpr int G = BN / 16;           // the gate columns sit BN / 2 columns (BN / 16 groups) further
-                x0v *= gelu_erf_f(fmaf(rstd[h], acc[4 * (i + G) + 2 * h], bg.x));
-                x1v *= gelu_erf_f(fmaf(rstd[h], acc[4 * (i + G) + 2 * h + 1], bg.y));
-              }
+              constexpr int G = BN / 16;   // GEGLU: the gate columns sit BN / 2 columns (BN / 16 groups) further
+              const float2 x = epilogue_pair<GEGLU>(acc, 4 * i + 2 * h, 4 * (i + G) + 2 * h, rstd[h], bv, bg);
+              float x0v = x.x, x1v = x.y;
               if (rb[h] && col_ok) {
                 const float2 f = FAST_EPI ? __half22float2(rh[h][j])
                                           : __half22float2(*reinterpret_cast<const __half2*>(rb[h] + col));
@@ -546,7 +575,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_f16_kernel(const __grid_
     if (FAST_EPI && issuer) tma_store_wait_read0();   // lazy drain: the last tile's stores read out before exit
   }
   __syncthreads();
-  if (threadIdx.x == 0) stamp(8);
+  if (threadIdx.x == 0) trace_stamp(p, 8);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -560,9 +589,9 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_f16_kernel(const __grid_
 // warpgroups consume it in turn (as CUTLASS's ping-pong does): the running main loop has the whole ring of loads in
 // flight ahead of it, instead of half of it while the idle warpgroup's half sits full.  The main loops take turns
 // through two named barriers, so the two warpgroups' epilogues do not fall together.
-// The epilogue is gemm_f16_kernel's expressions in the same order -- the LayerNorm statistics summed in slab order,
-// fmaf(rstd, acc, bias), gelu_erf_f on the gate, pack_half2 -- so the outputs are bitwise equal to it.  The LayerNorm
-// statistics of the tile's rows and its bias columns are fetched during the main loop.
+// The epilogue sums the LayerNorm statistics in gemm_f16_kernel's slab order and computes each output pair through the
+// same ln_rstd and epilogue_pair, so the outputs are bitwise equal to it.  The LayerNorm statistics of the tile's rows
+// and its bias columns are fetched during the main loop.
 // ------------------------------------------------------------------------------------------------
 constexpr int PP_STAGES = 6;      // one ring, shared by both MMA warpgroups
 constexpr int PP_BN = 128;        // B-tile rows (GEGLU: 64 value + 64 gate rows, 64 outputs)
@@ -618,14 +647,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_pp_f16_kernel(const __gr
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  auto stamp = [&](int slot) {
-    if (p.trace && blockIdx.x == 0) {
-      unsigned long long t;
-      asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-      p.trace[slot] = t;
-    }
-  };
-  if (threadIdx.x == 0) stamp(0);
+  if (threadIdx.x == 0) trace_stamp(p, 0);
   constexpr int BN_OUT = S::BN_OUT;
   const int n_tiles = (p.N + BN_OUT - 1) / BN_OUT;
   const int num_tiles = n_tiles * p.m_tiles;
@@ -641,10 +663,10 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_pp_f16_kernel(const __gr
     fence_barrier_init();
   }
   __syncthreads();
-  if (threadIdx.x == 0) stamp(1);
+  if (threadIdx.x == 0) trace_stamp(p, 1);
   pdl_launch_dependents();
   pdl_wait();
-  if (threadIdx.x == 0) stamp(2);
+  if (threadIdx.x == 0) trace_stamp(p, 2);
 
   if (warp < 4) {
     // ------------------------------ producer warpgroup ------------------------------
@@ -665,25 +687,14 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_pp_f16_kernel(const __gr
           if (elect_one()) {
             mbar_arrive_expect_tx(&full_bar[stage], S::STAGE_BYTES);
             tma_load_2d(sA, &amap, &full_bar[stage], kb * BK, m0);
-            tma_load_2d(sB, &bmap, &full_bar[stage], kb * BK, n0);
-            if (GEGLU) tma_load_2d(sB + (PP_BN / 2) * BK * 2, &bmap, &full_bar[stage], kb * BK, p.gate_row_off + n0);
+            load_weight_tile<PP_BN, GEGLU>(sB, &bmap, &full_bar[stage], kb, n0, p.gate_row_off);
           }
           __syncwarp();
-          if (++stage == PP_STAGES) {
-            stage = 0;
-            phase ^= 1;
-          }
+          ring_advance<PP_STAGES>(stage, phase);
         }
       }
     } else if (warp == 1 && lane == 0 && p.pf_ptr) {
-      constexpr unsigned long long CH = 16384;
-      const unsigned long long per = ((p.pf_bytes / gridDim.x) + CH - 1) / CH * CH;
-      unsigned long long off = per * blockIdx.x;
-      const unsigned long long end = off + per < p.pf_bytes ? off + per : p.pf_bytes;
-      for (; off < end; off += CH) {
-        const unsigned long long n = end - off < CH ? ((end - off) & ~15ull) : CH;
-        if (n) l2_prefetch_bulk(p.pf_ptr + off, (uint32_t)n);
-      }
+      prefetch_next_weights(p);
     }
   } else {
     // ------------------------------ MMA + epilogue warpgroups, one whole tile each ------------------------------
@@ -740,7 +751,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_pp_f16_kernel(const __gr
       int prev = -1;
       for (int kb = 0; kb < p.num_kb; ++kb) {
         mbar_wait(&full_bar[stage], phase);
-        if (issuer && j == 0 && kb == 0) stamp(3);
+        if (issuer && j == 0 && kb == 0) trace_stamp(p, 3);
         const uint32_t a_addr = smem_u32(smem + stage * S::STAGE_BYTES);
         const uint64_t a_desc0 = wgmma_desc_sw128(a_addr);
         const uint64_t a_desc1 = wgmma_desc_sw128(a_addr + 64 * 128);
@@ -757,10 +768,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_pp_f16_kernel(const __gr
           if (lane == 0) mbar_arrive(&empty_bar[prev]);
         }
         prev = stage;
-        if (++stage == PP_STAGES) {
-          stage = 0;
-          phase ^= 1;
-        }
+        ring_advance<PP_STAGES>(stage, phase);
         if (kb == 0 && t < 64) my_ops->bias[t] = bias_pair;
         if (kb < ln_n) ln_step(kb);
       }
@@ -770,17 +778,11 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_pp_f16_kernel(const __gr
       fence_regs(acc[0]);
       fence_regs(acc[1]);
       if (lane == 0) mbar_arrive(&empty_bar[prev]);
-      if (issuer) stamp(4 + (j < 3 ? j : 3));
+      if (issuer) trace_stamp(p, 4 + (j < 3 ? j : 3));
 
-      // ---- epilogue: the same expressions in the same order as gemm_f16_kernel
+      // ---- epilogue: gemm_f16_kernel's ln_rstd and epilogue_pair, the statistics summed in the same slab order
       for (int s = p.num_kb; s < ln_n; ++s) ln_step(s);   // statistics slabs past the k-blocks
-      float rstd = p.alpha;
-      if (ln_n && ln_ok) {
-        const float ln_mean = ssum * p.ln_inv_c;
-        const float var = fmaxf(ssq * p.ln_inv_c - ln_mean * ln_mean, 0.f);
-        rstd = p.alpha * rsqrtf(var + p.ln_eps);
-      }
-      my_ops->rstd[t] = rstd;
+      my_ops->rstd[t] = ln_n && ln_ok ? ln_rstd(p, ssum, ssq) : p.alpha;
       const uint32_t stg_row = smem_u32(my_stg) + rw * 128 + cq * 2;   // rows 64 mb + rw + 8 h: (row & 7) == lane >> 2
       const uint32_t ops_bias = smem_u32(my_ops->bias) + (cq >> 1) * 4;
 #pragma unroll
@@ -797,14 +799,9 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_pp_f16_kernel(const __gr
           for (int c = 0; c < 8; ++c) {
             const int i = sl * 8 + c;   // accumulator 8-column group; its bias pair is 4 i + cq / 2 (GEGLU gate: + 32)
             const float2 bv = unpack_half2(ld_shared_u32(ops_bias + 16 * i));
-            float x0v = fmaf(rs, acc[mb][4 * i + 2 * h], bv.x);
-            float x1v = fmaf(rs, acc[mb][4 * i + 2 * h + 1], bv.y);
-            if (GEGLU) {
-              const float2 bg = unpack_half2(ld_shared_u32(ops_bias + 128 + 16 * i));
-              x0v *= gelu_erf_f(fmaf(rs, acc[mb][4 * (i + 8) + 2 * h], bg.x));
-              x1v *= gelu_erf_f(fmaf(rs, acc[mb][4 * (i + 8) + 2 * h + 1], bg.y));
-            }
-            st_shared_u32(stg_row + (64 * mb + 8 * h) * 128 + ((c ^ (lane >> 2)) << 4), pack_half2(x0v, x1v));
+            const float2 bg = GEGLU ? unpack_half2(ld_shared_u32(ops_bias + 128 + 16 * i)) : make_float2(0.f, 0.f);
+            const float2 x = epilogue_pair<GEGLU>(acc[mb], 4 * i + 2 * h, 4 * (i + 8) + 2 * h, rs, bv, bg);
+            st_shared_u32(stg_row + (64 * mb + 8 * h) * 128 + ((c ^ (lane >> 2)) << 4), pack_half2(x.x, x.y));
           }
         }
         fence_proxy_async_smem();
@@ -818,7 +815,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_pp_f16_kernel(const __gr
     if (issuer) tma_store_wait_read0();   // staging stays valid until the last stores have read it
   }
   __syncthreads();
-  if (threadIdx.x == 0) stamp(8);
+  if (threadIdx.x == 0) trace_stamp(p, 8);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -854,32 +851,11 @@ static int out_maps(const OutView& v, bool narrow_slab, OutMaps& m) {
   return 0;
 }
 
-template <int BN, int STAGES, bool GEGLU>
-static int launch_gemm(const TmapSet4& amaps, const CUtensorMap& bmap, const OutMaps& om, GemmParams& p, int m_tiles,
-                       cudaStream_t stream) {
-  using S = GemmSmem<BN, STAGES, GEGLU>;
+// Launches a persistent GEMM kernel whose shared-memory layout is S (GemmSmem or PpSmem, one type per kernel): grid =
+// min(#tiles, #SMs).  `args` are the kernel's arguments before the GemmParams.
+template <typename S, typename... KArgs, typename... Args>
+static int launch_gemm(void (*kern)(KArgs...), GemmParams& p, int m_tiles, cudaStream_t stream, const Args&... args) {
   static bool configured = false;
-  auto kern = gemm_f16_kernel<BN, STAGES, GEGLU>;
-  if (!configured) {
-    IH_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, S::TOTAL));
-    configured = true;
-  }
-  constexpr int BN_OUT = GEGLU ? BN / 2 : BN;
-  p.m_tiles = m_tiles;
-  const long long n_tiles = (p.N + BN_OUT - 1) / BN_OUT;
-  const long long tiles = n_tiles * m_tiles;
-  const int grid = (int)(tiles < num_sms() ? tiles : num_sms());
-  IH_CUDA(launch_kernel(kern, dim3(grid), dim3(GEMM_THREADS), (size_t)(S::TOTAL), stream, amaps, bmap, om.o, om.r,
-                        om.o32, om.r32, p));
-  return 0;
-}
-
-template <bool GEGLU>
-static int launch_gemm_pp(const TmapSet4& amaps, const CUtensorMap& bmap, const OutMaps& om, GemmParams& p, int m_tiles,
-                          cudaStream_t stream) {
-  using S = PpSmem<GEGLU>;
-  static bool configured = false;
-  auto kern = gemm_pp_f16_kernel<GEGLU>;
   if (!configured) {
     IH_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, S::TOTAL));
     configured = true;
@@ -887,7 +863,7 @@ static int launch_gemm_pp(const TmapSet4& amaps, const CUtensorMap& bmap, const 
   p.m_tiles = m_tiles;
   const long long tiles = (long long)((p.N + S::BN_OUT - 1) / S::BN_OUT) * m_tiles;
   const int grid = (int)(tiles < num_sms() ? tiles : num_sms());
-  IH_CUDA(launch_kernel(kern, dim3(grid), dim3(GEMM_THREADS), (size_t)(S::TOTAL), stream, amaps.m[0], bmap, om.o, p));
+  IH_CUDA(launch_kernel(kern, dim3(grid), dim3(GEMM_THREADS), (size_t)(S::TOTAL), stream, args..., p));
   return 0;
 }
 
@@ -984,23 +960,29 @@ static int dispatch(const TmapSet4& amaps, const OutView& ov, const void* w, int
   if (rc) return rc;
   OutMaps om;
   if ((rc = out_maps(ov, bn_out % 64 == 32, om))) return rc;
-  if (pp) return geglu ? launch_gemm_pp<true>(amaps, bmap, om, p, m_tiles, stream)
-                       : launch_gemm_pp<false>(amaps, bmap, om, p, m_tiles, stream);
+  if (pp) {
+    if (geglu) return launch_gemm<PpSmem<true>>(gemm_pp_f16_kernel<true>, p, m_tiles, stream, amaps.m[0], bmap, om.o);
+    return launch_gemm<PpSmem<false>>(gemm_pp_f16_kernel<false>, p, m_tiles, stream, amaps.m[0], bmap, om.o);
+  }
+#define IH_LAUNCH_F16(BN, STAGES, GEGLU)                                                                           \
+  launch_gemm<GemmSmem<BN, STAGES, GEGLU>>(gemm_f16_kernel<BN, STAGES, GEGLU>, p, m_tiles, stream, amaps, bmap, om.o, \
+                                           om.r, om.o32, om.r32)
   if (geglu) {
     switch (bn) {
-      case 256: return launch_gemm<256, 4, true>(amaps, bmap, om, p, m_tiles, stream);
-      case 192: return launch_gemm<192, 5, true>(amaps, bmap, om, p, m_tiles, stream);
-      default: return launch_gemm<128, 6, true>(amaps, bmap, om, p, m_tiles, stream);
+      case 256: return IH_LAUNCH_F16(256, 4, true);
+      case 192: return IH_LAUNCH_F16(192, 5, true);
+      default: return IH_LAUNCH_F16(128, 6, true);
     }
   }
   switch (bn) {
-    case 256: return launch_gemm<256, 4, false>(amaps, bmap, om, p, m_tiles, stream);
-    case 192: return launch_gemm<192, 4, false>(amaps, bmap, om, p, m_tiles, stream);
-    case 160: return launch_gemm<160, 5, false>(amaps, bmap, om, p, m_tiles, stream);
-    case 128: return launch_gemm<128, 6, false>(amaps, bmap, om, p, m_tiles, stream);
-    case 64: return launch_gemm<64, 8, false>(amaps, bmap, om, p, m_tiles, stream);
+    case 256: return IH_LAUNCH_F16(256, 4, false);
+    case 192: return IH_LAUNCH_F16(192, 4, false);
+    case 160: return IH_LAUNCH_F16(160, 5, false);
+    case 128: return IH_LAUNCH_F16(128, 6, false);
+    case 64: return IH_LAUNCH_F16(64, 8, false);
     default: return set_error(IH_ERR_ARG, "unsupported BN %d", bn);
   }
+#undef IH_LAUNCH_F16
 }
 
 static unsigned long long* g_trace = nullptr;
@@ -1019,6 +1001,23 @@ static PrefetchHint take_prefetch_hint() {
   g_pf_bytes = 0;
   return h;
 }
+
+// The epilogue fields that GEMM and conv launches set alike; the caller sets the rest.
+static GemmParams epilogue_params(const PrefetchHint& hint, const void* bias, const void* rowbias, long long ld_rowbias,
+                                  const void* residual, void* out, float alpha, int epilogue) {
+  GemmParams p{};
+  p.bias = (const __half*)bias;
+  p.rowbias = (const __half*)rowbias;
+  p.ld_rowbias = ld_rowbias;
+  p.residual = (const __half*)residual;
+  p.out = (__half*)out;
+  p.trace = g_trace;
+  p.pf_ptr = hint.ptr;
+  p.pf_bytes = hint.bytes;
+  p.alpha = alpha;
+  p.relu = epilogue == IH_EPI_RELU;
+  return p;
+}
 }  // namespace ih
 
 using namespace ih;
@@ -1031,33 +1030,6 @@ extern "C" void ih_gemm_set_trace(void* device_buffer) { ih::g_trace = (unsigned
 extern "C" void ih_gemm_prefetch_next(const void* weights, long long bytes) {
   ih::g_pf_ptr = (weights && bytes >= 16 && ((uintptr_t)weights & 15) == 0) ? weights : nullptr;
   ih::g_pf_bytes = ih::g_pf_ptr ? (unsigned long long)bytes : 0;
-}
-
-static int gemm_impl(const void* a, long long lda, const void* w, const void* bias, const void* rowbias,
-                     int rows_per_group, long long ld_rowbias, const void* residual, long long ldr, void* out,
-                     long long ldo, int M, int N, int K, int epilogue, int tile_n, const void* ln_stats,
-                     int ln_slabs, float ln_eps, void* stats_out, float alpha, void* stream);
-
-extern "C" int ih_gemm_f16(const void* a, long long lda, const void* w, const void* bias, const void* rowbias,
-                           int rows_per_group, long long ld_rowbias, const void* residual, long long ldr, void* out,
-                           long long ldo, int M, int N, int K, int epilogue, int tile_n, void* stream) {
-  return gemm_impl(a, lda, w, bias, rowbias, rows_per_group, ld_rowbias, residual, ldr, out, ldo, M, N, K, epilogue,
-                   tile_n, nullptr, 0, 0.f, nullptr, 1.f, stream);
-}
-
-extern "C" int ih_gemm_scaled_f16(const void* a, long long lda, const void* w, const void* bias, const void* residual,
-                                  long long ldr, void* out, long long ldo, int M, int N, int K, int epilogue, float alpha,
-                                  void* stream) {
-  return gemm_impl(a, lda, w, bias, nullptr, 0, 0, residual, ldr, out, ldo, M, N, K, epilogue, 0, nullptr, 0, 0.f,
-                   nullptr, alpha, stream);
-}
-
-extern "C" int ih_gemm_ln_f16(const void* a, long long lda, const void* w, const void* bias, const void* rowbias,
-                              int rows_per_group, long long ld_rowbias, const void* residual, long long ldr, void* out,
-                              long long ldo, int M, int N, int K, int epilogue, int tile_n, const void* ln_stats,
-                              int ln_slabs, float ln_eps, void* stats_out, void* stream) {
-  return gemm_impl(a, lda, w, bias, rowbias, rows_per_group, ld_rowbias, residual, ldr, out, ldo, M, N, K, epilogue,
-                   tile_n, ln_stats, ln_slabs, ln_eps, stats_out, 1.f, stream);
 }
 
 static int gemm_impl(const void* a, long long lda, const void* w, const void* bias, const void* rowbias,
@@ -1085,25 +1057,16 @@ static int gemm_impl(const void* a, long long lda, const void* w, const void* bi
   if (rc) return rc;
   amaps.m[1] = amaps.m[2] = amaps.m[3] = amaps.m[0];
 
-  GemmParams p{};
+  GemmParams p = epilogue_params(hint, bias, rowbias, ld_rowbias, residual, out, alpha, epilogue);
   p.M = M;
   p.N = geglu ? N / 2 : N;
   p.num_kb = (K + BK - 1) / BK;
   p.mode = 0;
   p.gate_row_off = geglu ? N / 2 : 0;
-  p.bias = (const __half*)bias;
-  p.rowbias = (const __half*)rowbias;
   p.rows_per_group = rows_per_group > 0 ? rows_per_group : 1;
-  p.ld_rowbias = ld_rowbias;
-  p.residual = (const __half*)residual;
   p.ldr = ldr;
-  p.out = (__half*)out;
   p.ldo = ldo;
   p.act = (epilogue & IH_EPI_SILU) ? 1 : ((epilogue & IH_EPI_GELU) ? 2 : ((epilogue & IH_EPI_QUICK_GELU) ? 3 : 0));
-  p.relu = epilogue == IH_EPI_RELU;
-  p.trace = g_trace;
-  p.pf_ptr = hint.ptr;
-  p.pf_bytes = hint.bytes;
   IH_CHECK(!ln_stats || ln_slabs > 0, IH_ERR_ARG, "ih_gemm_ln_f16: ln_stats needs ln_slabs > 0");
   IH_CHECK(!stats_out || N % 64 == 0 || geglu, IH_ERR_SHAPE, "ih_gemm_ln_f16: stats_out needs N %% 64 == 0");
   p.stats_out = (float*)stats_out;
@@ -1111,46 +1074,32 @@ static int gemm_impl(const void* a, long long lda, const void* w, const void* bi
   p.ln_slabs = ln_slabs;
   p.ln_inv_c = 1.0f / (float)K;
   p.ln_eps = ln_eps;
-  p.alpha = alpha;
   const int m_tiles = (M + BM - 1) / BM;
   const OutView ov{out, residual, 2, {(uint64_t)p.N, (uint64_t)M}, {(uint64_t)ldo * 2}, {(uint64_t)ldr * 2},
                    {64u, (uint32_t)BM}};
   return dispatch(amaps, ov, w, N, K, p, m_tiles, geglu, tile_n, (cudaStream_t)stream);
 }
 
-static int conv_impl(const void* x, const void* w, const void* bias, const void* rowbias, long long ld_rowbias,
-                     const void* residual, void* out, int B, int Hin, int Win, int Cin, int Cout, int ksize, int stride,
-                     int tile_n, float alpha, void* stream, const void* sc0 = nullptr, int Csc0 = 0,
-                     const void* sc1 = nullptr, int Csc1 = 0, bool pad_bottom_right = false,
-                     int epilogue = IH_EPI_NONE);
-
-extern "C" int ih_conv2d_f16(const void* x, const void* w, const void* bias, const void* rowbias,
-                             long long ld_rowbias, const void* residual, void* out, int B, int Hin, int Win, int Cin,
-                             int Cout, int ksize, int stride, int tile_n, void* stream) {
-  return conv_impl(x, w, bias, rowbias, ld_rowbias, residual, out, B, Hin, Win, Cin, Cout, ksize, stride, tile_n, 1.f,
-                   stream);
+extern "C" int ih_gemm_f16(const void* a, long long lda, const void* w, const void* bias, const void* rowbias,
+                           int rows_per_group, long long ld_rowbias, const void* residual, long long ldr, void* out,
+                           long long ldo, int M, int N, int K, int epilogue, int tile_n, void* stream) {
+  return gemm_impl(a, lda, w, bias, rowbias, rows_per_group, ld_rowbias, residual, ldr, out, ldo, M, N, K, epilogue,
+                   tile_n, nullptr, 0, 0.f, nullptr, 1.f, stream);
 }
 
-extern "C" int ih_conv2d_scaled_f16(const void* x, const void* w, const void* bias, const void* residual, void* out,
-                                    int B, int Hin, int Win, int Cin, int Cout, int stride, float alpha, void* stream,
-                                    int epilogue) {
-  return conv_impl(x, w, bias, nullptr, 0, residual, out, B, Hin, Win, Cin, Cout, 3, stride, 0, alpha, stream, nullptr, 0,
-                   nullptr, 0, false, epilogue);
+extern "C" int ih_gemm_scaled_f16(const void* a, long long lda, const void* w, const void* bias, const void* residual,
+                                  long long ldr, void* out, long long ldo, int M, int N, int K, int epilogue, float alpha,
+                                  void* stream) {
+  return gemm_impl(a, lda, w, bias, nullptr, 0, 0, residual, ldr, out, ldo, M, N, K, epilogue, 0, nullptr, 0, 0.f,
+                   nullptr, alpha, stream);
 }
 
-extern "C" int ih_conv2d_shortcut_f16(const void* x, const void* w, const void* bias, const void* rowbias,
-                                      long long ld_rowbias, const void* sc0, int Csc0, const void* sc1, int Csc1, void* out,
-                                      int B, int H, int W, int Cin, int Cout, void* stream) {
-  IH_CHECK(sc0 && Csc0 > 0 && Csc0 % BK == 0 && (!sc1 || (Csc1 > 0 && Csc1 % BK == 0)), IH_ERR_SHAPE,
-           "ih_conv2d_shortcut_f16: shortcut sources need channel counts that are multiples of 64");
-  return conv_impl(x, w, bias, rowbias, ld_rowbias, nullptr, out, B, H, W, Cin, Cout, 3, 1, 0, 1.f, stream, sc0, Csc0,
-                   sc1 ? sc1 : nullptr, sc1 ? Csc1 : 0);
-}
-
-extern "C" int ih_conv2d_down_f16(const void* x, const void* w, const void* bias, void* out, int B, int Hin, int Win,
-                                  int Cin, int Cout, int tile_n, float alpha, void* stream) {
-  return conv_impl(x, w, bias, nullptr, 0, nullptr, out, B, Hin, Win, Cin, Cout, 3, 2, tile_n, alpha, stream, nullptr, 0,
-                   nullptr, 0, true);
+extern "C" int ih_gemm_ln_f16(const void* a, long long lda, const void* w, const void* bias, const void* rowbias,
+                              int rows_per_group, long long ld_rowbias, const void* residual, long long ldr, void* out,
+                              long long ldo, int M, int N, int K, int epilogue, int tile_n, const void* ln_stats,
+                              int ln_slabs, float ln_eps, void* stats_out, void* stream) {
+  return gemm_impl(a, lda, w, bias, rowbias, rows_per_group, ld_rowbias, residual, ldr, out, ldo, M, N, K, epilogue,
+                   tile_n, ln_stats, ln_slabs, ln_eps, stats_out, 1.f, stream);
 }
 
 static int conv_impl(const void* x, const void* w, const void* bias, const void* rowbias, long long ld_rowbias,
@@ -1178,7 +1127,7 @@ static int conv_impl(const void* x, const void* w, const void* bias, const void*
       best_bw = bw;
     }
   }
-  GemmParams p{};
+  GemmParams p = epilogue_params(hint, bias, rowbias, ld_rowbias, residual, out, alpha, epilogue);
   p.bw = best_bw;
   p.bh = 128 / best_bw;
   p.tiles_x = (Wo + p.bw - 1) / p.bw;
@@ -1201,19 +1150,9 @@ static int conv_impl(const void* x, const void* w, const void* bias, const void*
   p.num_kb = p.tap_kb_end[p.n_taps - 1];
   p.M = B * Ho * Wo;
   p.N = Cout;
-  p.bias = (const __half*)bias;
-  p.rowbias = (const __half*)rowbias;
   p.rows_per_group = Ho * Wo;
-  p.ld_rowbias = ld_rowbias;
-  p.residual = (const __half*)residual;
   p.ldr = Cout;
-  p.out = (__half*)out;
   p.ldo = Cout;
-  p.trace = g_trace;
-  p.pf_ptr = hint.ptr;
-  p.pf_bytes = hint.bytes;
-  p.alpha = alpha;
-  p.relu = epilogue == IH_EPI_RELU;
 
   TmapSet4 amaps;
   const uint32_t abox[4] = {(uint32_t)BK, (uint32_t)p.bw, (uint32_t)p.bh, 1u};
@@ -1267,4 +1206,33 @@ static int conv_impl(const void* x, const void* w, const void* bias, const void*
   const OutView ov{out, residual, 4, {(uint64_t)Cout, (uint64_t)Wo, (uint64_t)Ho, (uint64_t)B}, {ostr[0], ostr[1], ostr[2]},
                    {ostr[0], ostr[1], ostr[2]}, {64u, (uint32_t)p.bw, (uint32_t)p.bh, 1u}};
   return dispatch(amaps, ov, w, Cout, (long long)9 * Cin + Csc0 + Csc1, p, m_tiles, 0, tile_n, (cudaStream_t)stream);
+}
+
+extern "C" int ih_conv2d_f16(const void* x, const void* w, const void* bias, const void* rowbias,
+                             long long ld_rowbias, const void* residual, void* out, int B, int Hin, int Win, int Cin,
+                             int Cout, int ksize, int stride, int tile_n, void* stream) {
+  return conv_impl(x, w, bias, rowbias, ld_rowbias, residual, out, B, Hin, Win, Cin, Cout, ksize, stride, tile_n, 1.f,
+                   stream, nullptr, 0, nullptr, 0, false, IH_EPI_NONE);
+}
+
+extern "C" int ih_conv2d_scaled_f16(const void* x, const void* w, const void* bias, const void* residual, void* out,
+                                    int B, int Hin, int Win, int Cin, int Cout, int stride, float alpha, void* stream,
+                                    int epilogue) {
+  return conv_impl(x, w, bias, nullptr, 0, residual, out, B, Hin, Win, Cin, Cout, 3, stride, 0, alpha, stream, nullptr, 0,
+                   nullptr, 0, false, epilogue);
+}
+
+extern "C" int ih_conv2d_shortcut_f16(const void* x, const void* w, const void* bias, const void* rowbias,
+                                      long long ld_rowbias, const void* sc0, int Csc0, const void* sc1, int Csc1, void* out,
+                                      int B, int H, int W, int Cin, int Cout, void* stream) {
+  IH_CHECK(sc0 && Csc0 > 0 && Csc0 % BK == 0 && (!sc1 || (Csc1 > 0 && Csc1 % BK == 0)), IH_ERR_SHAPE,
+           "ih_conv2d_shortcut_f16: shortcut sources need channel counts that are multiples of 64");
+  return conv_impl(x, w, bias, rowbias, ld_rowbias, nullptr, out, B, H, W, Cin, Cout, 3, 1, 0, 1.f, stream, sc0, Csc0,
+                   sc1, sc1 ? Csc1 : 0, false, IH_EPI_NONE);
+}
+
+extern "C" int ih_conv2d_down_f16(const void* x, const void* w, const void* bias, void* out, int B, int Hin, int Win,
+                                  int Cin, int Cout, int tile_n, float alpha, void* stream) {
+  return conv_impl(x, w, bias, nullptr, 0, nullptr, out, B, Hin, Win, Cin, Cout, 3, 2, tile_n, alpha, stream, nullptr, 0,
+                   nullptr, 0, true, IH_EPI_NONE);
 }
