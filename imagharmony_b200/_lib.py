@@ -29,6 +29,9 @@ class IhCnResidual(ctypes.Structure):
 
 
 IH_CN_MAX_NETS = 8      # include/ih_api.h
+IH_SOLVER_DPMPP_2M = 0  # include/ih_api.h: ih_dpm_solver_step's solver
+IH_SOLVER_UNIPC_BH2 = 1
+IH_UNIPC_COEFFS = 16
 
 
 class IhCnMultiResidual(ctypes.Structure):
@@ -131,7 +134,7 @@ SIGNATURES = {
     "ih_euler_inpaint_step": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_float, c_float, c_longlong,
                                       c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "ih_dpm_solver_step": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_float,
-                                   c_float, c_longlong, c_int, c_int, c_void_p]),
+                                   c_float, c_longlong, c_int, c_int, c_void_p, c_int, c_void_p, c_void_p]),
     "ih_euler_ancestral_step": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_float, c_float,
                                         c_longlong, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "ih_euler_ancestral_scale_input": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_longlong, c_int, c_void_p]),

@@ -478,6 +478,136 @@ __global__ void __launch_bounds__(1024) dpm_solver_kernel(const __half* __restri
 }
 
 // ---------------------------------------------------------------------------------------------------------------
+// UniPC step ([3P] diffusers==0.30.0 UniPCMultistepScheduler: bh2, solver_order 2, predict_x0, epsilon).  The guided
+// prediction and its rescale are those of dpm_solver_kernel; every per-step scalar comes from the host table
+// coeffs[i, IH_UNIPC_COEFFS] (torch fp32 0-dim arithmetic, the diffusers expressions; rho0 / rho1 already rounded to
+// fp16).  With x the fp16 latents, m1 = prev_x0 = x0_{i-1}, m2 = prev_x0_2 = x0_{i-2}, ls = last_sample:
+//   x0  = fp16(fp16(x - fp16(sigma_s * eps)) * inv_alpha_s)                          convert_model_output
+//   corrector (order c >= 1), D1_t = fp16(x0 - m1):
+//     xt_ = fp16(fp16(c_ratio * ls) - fp16(c_c * m1))
+//     res = c == 1 ? fp16(fp16(rho1 * D1_t) + 0)
+//                  : fp16(fp16(rho0 * fp16(c_inv_rk * fp16(m2 - m1))) + fp16(rho1 * D1_t))
+//     x   = fp16(xt_ - fp16(c_c * res))                                                (bh2: B_h = h_phi_1)
+//   prev_x0_2 <- m1, prev_x0 <- x0, last_sample <- x
+//   predictor (order p): xt_ = fp16(fp16(p_ratio * x) - fp16(p_c * x0))
+//     p == 2: latents = fp16(xt_ - fp16(p_c * fp16(0.5 * fp16(p_inv_rk * fp16(m1 - x0)))))
+//     p == 1: latents = fp16(xt_ - p_c * 0)
+// Orders: p = min(table p, i - b + 1), c = i > b ? min(table c, i - b) : 0 with b = *loop_begin, so a loop that starts
+// at b has no history at b; a corrector of order 1 uses rho1 = 0.5 whatever the table's order.  A step reads only the
+// history its orders use (the buffers hold stale data at a loop's first steps, and 0 * NaN is NaN); prev_x0 is always
+// moved to prev_x0_2 unread by arithmetic.  Explicit _rn intrinsics: no FMA that torch does not form.
+// ---------------------------------------------------------------------------------------------------------------
+struct UniPCCoeffs {
+  float sigma_s, inv_alpha_s, p_ratio, p_c, p_inv_rk, c_ratio, c_c, c_inv_rk, rho0, rho1;
+  int p, c;
+};
+
+__device__ __forceinline__ void unipc_elem(long long idx, float eps, const UniPCCoeffs& k, long long total, int cfg,
+                                           __half* __restrict__ latents, __half* __restrict__ model_in,
+                                           __half* __restrict__ last_sample, __half* __restrict__ prev_x0,
+                                           __half* __restrict__ prev_x0_2) {
+  const float x = __half2float(latents[idx]);
+  const float x0 = h16(__fmul_rn(h16(__fsub_rn(x, h16(__fmul_rn(k.sigma_s, eps)))), k.inv_alpha_s));
+  const __half m1h = prev_x0[idx];
+  const float m1 = __half2float(m1h);
+  float xc = x;
+  if (k.c > 0) {
+    const float xt = h16(__fsub_rn(h16(__fmul_rn(k.c_ratio, __half2float(last_sample[idx]))), h16(__fmul_rn(k.c_c, m1))));
+    float res = h16(__fmul_rn(k.rho1, h16(__fsub_rn(x0, m1))));
+    if (k.c == 2) {
+      const float d1 = h16(__fmul_rn(k.c_inv_rk, h16(__fsub_rn(__half2float(prev_x0_2[idx]), m1))));
+      res = h16(__fadd_rn(h16(__fmul_rn(k.rho0, d1)), res));
+    } else {
+      res = __fadd_rn(res, 0.f);                 // corr_res is the integer 0 at order 1
+    }
+    xc = h16(__fsub_rn(xt, h16(__fmul_rn(k.c_c, res))));
+  }
+  prev_x0_2[idx] = m1h;
+  prev_x0[idx] = __float2half_rn(x0);
+  last_sample[idx] = __float2half_rn(xc);
+  const float xt = h16(__fsub_rn(h16(__fmul_rn(k.p_ratio, xc)), h16(__fmul_rn(k.p_c, x0))));
+  float out;
+  if (k.p == 2) {
+    const float d1 = h16(__fmul_rn(k.p_inv_rk, h16(__fsub_rn(m1, x0))));
+    out = __fsub_rn(xt, h16(__fmul_rn(k.p_c, h16(__fmul_rn(0.5f, d1)))));
+  } else {
+    out = __fsub_rn(xt, __fmul_rn(k.p_c, 0.f));   // pred_res is the integer 0 at order 1
+  }
+  const __half xh = __float2half_rn(out);
+  latents[idx] = xh;
+  model_in[idx] = xh;                            // scale_model_input is the identity for this scheduler
+  if (cfg) model_in[total + idx] = xh;
+}
+
+// Without guidance_rescale: grid-stride over all elements.  With it: one block per image, the std ratio reduced in the
+// order of euler_ex_kernel (the reduction of dpm_solver_kernel; a shared helper changed that kernel's register
+// allocation, so each step kernel keeps its own copy).
+__global__ void __launch_bounds__(1024) unipc_kernel(const __half* __restrict__ noise, __half* __restrict__ latents,
+                                                     __half* __restrict__ model_in, __half* __restrict__ last_sample,
+                                                     __half* __restrict__ prev_x0, __half* __restrict__ prev_x0_2,
+                                                     const float* __restrict__ coeffs, const int* __restrict__ step,
+                                                     const int* __restrict__ loop_begin, float guidance, float rescale,
+                                                     long long per_image, int n_images, int cfg) {
+  pdl_launch_dependents();
+  pdl_wait();
+  const int i = *step;
+  const int b = *loop_begin;
+  const float* row = coeffs + (long long)i * IH_UNIPC_COEFFS;
+  const int p = min((int)row[5], i - b + 1);
+  const int c = i > b ? min((int)row[11], i - b) : 0;
+  const UniPCCoeffs k{row[0], row[1], row[2], row[3], row[4], row[6], row[7], row[8], row[9],
+                      c == 1 ? 0.5f : row[10], p, c};
+  const long long total = per_image * n_images;
+  if (!(cfg && rescale > 0.f)) {
+    for (long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x; idx < total;
+         idx += (long long)gridDim.x * blockDim.x) {
+      float cv;
+      unipc_elem(idx, cfg_guided(noise, idx, total, cfg, guidance, cv), k, total, cfg, latents, model_in, last_sample,
+                 prev_x0, prev_x0_2);
+    }
+    return;
+  }
+  const long long base = (long long)blockIdx.x * per_image;
+  double s_t = 0.0, q_t = 0.0, s_g = 0.0, q_g = 0.0;
+  for (long long e = threadIdx.x; e < per_image; e += blockDim.x) {
+    float cv;
+    const float g = cfg_guided(noise, base + e, total, cfg, guidance, cv);
+    s_t += cv;
+    q_t += (double)cv * cv;
+    s_g += g;
+    q_g += (double)g * g;
+  }
+  __shared__ double red[4][32];
+  __shared__ float s_factor;
+  double v[4] = {s_t, q_t, s_g, q_g};
+#pragma unroll
+  for (int q = 0; q < 4; ++q) {
+    for (int o = 16; o > 0; o >>= 1) v[q] += __shfl_xor_sync(0xffffffffu, v[q], o);
+    if ((threadIdx.x & 31) == 0) red[q][threadIdx.x >> 5] = v[q];
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double t[4] = {0, 0, 0, 0};
+    const int nw = (blockDim.x + 31) >> 5;
+    for (int q = 0; q < 4; ++q)
+      for (int w = 0; w < nw; ++w) t[q] += red[q][w];
+    const double n = (double)per_image;
+    const double var_t = fmax((t[1] - t[0] * t[0] / n) / (n - 1.0), 0.0);
+    const double var_g = fmax((t[3] - t[2] * t[2] / n) / (n - 1.0), 0.0);
+    s_factor = h16(h16((float)sqrt(var_t)) / h16((float)sqrt(var_g)));
+  }
+  __syncthreads();
+  const float factor = s_factor;
+  for (long long e = threadIdx.x; e < per_image; e += blockDim.x) {
+    float cv;
+    const float eps = cfg_guided(noise, base + e, total, cfg, guidance, cv);
+    const float a = h16(rescale * h16(eps * factor));
+    const float r = h16((1.f - rescale) * eps);
+    unipc_elem(base + e, h16(a + r), k, total, cfg, latents, model_in, last_sample, prev_x0, prev_x0_2);
+  }
+}
+
+// ---------------------------------------------------------------------------------------------------------------
 // Euler Ancestral step ([3P] diffusers==0.30.0 EulerAncestralDiscreteScheduler, epsilon).  The guided prediction is
 // formed as in euler_cfg_kernel / euler_ex_kernel; the per-step scalars come from the host table
 // coeffs[i, IH_EULER_A_COEFFS] (torch fp32 0-dim arithmetic) and the step's Gaussian noise from row i of a buffer the
@@ -1109,20 +1239,31 @@ extern "C" int ih_euler_inpaint_step(const void* noise_pred, void* latents, void
 extern "C" int ih_dpm_solver_step(const void* noise_pred, void* latents, void* model_in, void* prev_x0,
                                   const void* coeffs, void* step, const void* loop_begin, float guidance,
                                   float guidance_rescale, long long n_per_image, int n_images, int use_cfg,
-                                  void* stream_) {
+                                  void* stream_, int solver, void* last_sample, void* prev_x0_2) {
   cudaStream_t stream = (cudaStream_t)stream_;
   IH_CHECK(noise_pred && latents && model_in && prev_x0 && coeffs && step && loop_begin, IH_ERR_ARG,
            "ih_dpm_solver_step: null pointer");
+  IH_CHECK(solver == IH_SOLVER_DPMPP_2M || solver == IH_SOLVER_UNIPC_BH2, IH_ERR_ARG,
+           "ih_dpm_solver_step: solver %d is neither IH_SOLVER_DPMPP_2M nor IH_SOLVER_UNIPC_BH2", solver);
+  IH_CHECK(solver == IH_SOLVER_UNIPC_BH2 ? (last_sample && prev_x0_2) : (!last_sample && !prev_x0_2), IH_ERR_ARG,
+           "ih_dpm_solver_step: last_sample and prev_x0_2 are required by IH_SOLVER_UNIPC_BH2 and must be null for "
+           "IH_SOLVER_DPMPP_2M");
   IH_CHECK(n_per_image > 1 && n_images > 0, IH_ERR_SHAPE, "ih_dpm_solver_step: bad shape");
   IH_CHECK(guidance_rescale >= 0.f && guidance_rescale <= 1.f, IH_ERR_ARG,
            "ih_dpm_solver_step: guidance_rescale outside [0, 1]");
   const int cfg = use_cfg ? 1 : 0;
   const bool per_image = cfg && guidance_rescale > 0.f;
   const long long total = n_per_image * n_images;
-  IH_CUDA(launch_kernel(dpm_solver_kernel, dim3(per_image ? n_images : grid_for(total, 256)), dim3(per_image ? 1024 : 256),
-                        (size_t)(0), stream, (const __half*)noise_pred, (__half*)latents, (__half*)model_in,
-                        (__half*)prev_x0, (const float*)coeffs, (const int*)step, (const int*)loop_begin, guidance,
-                        guidance_rescale, n_per_image, n_images, cfg));
+  const dim3 grid(per_image ? n_images : grid_for(total, 256)), block(per_image ? 1024 : 256);
+  if (solver == IH_SOLVER_DPMPP_2M)
+    IH_CUDA(launch_kernel(dpm_solver_kernel, grid, block, (size_t)(0), stream, (const __half*)noise_pred,
+                          (__half*)latents, (__half*)model_in, (__half*)prev_x0, (const float*)coeffs, (const int*)step,
+                          (const int*)loop_begin, guidance, guidance_rescale, n_per_image, n_images, cfg));
+  else
+    IH_CUDA(launch_kernel(unipc_kernel, grid, block, (size_t)(0), stream, (const __half*)noise_pred, (__half*)latents,
+                          (__half*)model_in, (__half*)last_sample, (__half*)prev_x0, (__half*)prev_x0_2,
+                          (const float*)coeffs, (const int*)step, (const int*)loop_begin, guidance, guidance_rescale,
+                          n_per_image, n_images, cfg));
   IH_CUDA(launch_kernel(step_inc_kernel, dim3(1), dim3(1), (size_t)(0), stream, (int*)step));
   return 0;
 }

@@ -10,10 +10,12 @@ not the graph): classifier-free guidance on or off (`guidance_scale <= 1`, :223,
 (:352-354), `denoising_end` (:307-316, via `num_loop_steps`), `callback` / `callback_steps` (:359-363),
 `control_guidance_start/end` IP-scale gating (:326-329), negative micro-conditioning time ids (:286-300).
 
-Schedulers: EulerDiscreteScheduler (the reference's), EulerAncestralDiscreteScheduler (SURVEY A.6) and
-DPMSolverMultistepScheduler (DPM-Solver++ 2M, SURVEY A.5), chosen by the engine's scheduler object in one place of `run`.
-The DPM step reads its per-step scalars from a coefficient table and the previous step's data prediction from a static
-`prev_x0` buffer, both device-resident, so it too is one graph per shape.  The Euler Ancestral step reads its scalars
+Schedulers: EulerDiscreteScheduler (the reference's), EulerAncestralDiscreteScheduler (SURVEY A.6),
+DPMSolverMultistepScheduler (DPM-Solver++ 2M, SURVEY A.5) and UniPCMultistepScheduler (UniPC bh2, SURVEY A.9), chosen
+by the engine's scheduler object in one place of `run`.  The DPM step reads its per-step scalars from a coefficient
+table and the previous step's data prediction from a static `prev_x0` buffer, both device-resident, so it too is one
+graph per shape; the UniPC step also keeps the corrected sample (`last_sample`) and the data prediction before that
+(`prev_x0_2`) in static buffers.  The Euler Ancestral step reads its scalars
 from a coefficient table and its Gaussian noise from row `step` of a static [T, n, 4, h, w] buffer that `run` fills from
 the caller's generator(s) before the replays, outside any capture: the draws are torch's, in diffusers' order, so a seed
 gives diffusers' noise (a Philox stream inside the kernel would not reproduce torch's generator).
@@ -53,13 +55,16 @@ from . import ops
 from ._lib import IH_CN_MAX_NETS, IHError
 from .controlnet import controlnet_scales
 from .scheduler import (DPMSolverMultistepScheduler, EulerAncestralDiscreteScheduler, EulerDiscreteScheduler,
-                        randn_tensor)
+                        UniPCMultistepScheduler, randn_tensor)
 from .t2i_adapter import AdapterCall
 from .unet import UNet2DConditionModel, require_adapter_shapes, require_latent_size
 
 # option -> the options it cannot be combined with, and why
 _EXCLUDES = (
     ("DPMSolverMultistepScheduler", ("begin_step", "inpaint", "unet_cond", "start_step", "stop_after"),
+     "it runs whole text-to-image loops; EulerDiscreteScheduler and EulerAncestralDiscreteScheduler support these "
+     "options"),
+    ("UniPCMultistepScheduler", ("begin_step", "inpaint", "unet_cond", "start_step", "stop_after"),
      "it runs whole text-to-image loops; EulerDiscreteScheduler and EulerAncestralDiscreteScheduler support these "
      "options"),
     ("unet_cond", ("inpaint", "start_step", "stop_after"), "the 9-channel UNet is not blended and resumes nothing"),
@@ -103,8 +108,9 @@ class _Loop:
     rescale: float
     shape: Tuple[int, int, int, int, int]     # (n, h, w, L, T)
     kind: str                                 # the scheduler's
-    coeffs: Optional[torch.Tensor] = None     # DPM-Solver++ / Euler Ancestral coefficient table
-    dpm: Optional[dict] = None                # DPM-Solver++: prev_x0, loop_begin
+    coeffs: Optional[torch.Tensor] = None     # DPM-Solver++ / UniPC / Euler Ancestral coefficient table
+    dpm: Optional[dict] = None                # DPM-Solver++ and UniPC: prev_x0, loop_begin
+    unipc: Optional[tuple] = None             # UniPC: its further history (last_sample, prev_x0_2)
     noise: Optional[torch.Tensor] = None      # Euler Ancestral step noise [T, n, C, h, w]
     ib: Optional[dict] = None                 # 4-channel inpainting: image_latents, noise, mask, blend_end
     cond: Optional[torch.Tensor] = None       # 9-channel UNet: mask | masked-image latents
@@ -121,7 +127,7 @@ class _Loop:
 class DenoiseEngine:
     def __init__(self, unet: UNet2DConditionModel, use_cuda_graph: bool = True,
                  scheduler: Optional[Union[EulerDiscreteScheduler, EulerAncestralDiscreteScheduler,
-                                           DPMSolverMultistepScheduler]] = None):
+                                           DPMSolverMultistepScheduler, UniPCMultistepScheduler]] = None):
         self.unet = unet
         self.device = unet.conv_in.weight.device
         self.scheduler = scheduler or EulerDiscreteScheduler()      # the pipeline's own scheduler object when given
@@ -156,7 +162,7 @@ class DenoiseEngine:
         return self._schedule(num_steps)[:3]
 
     def coeffs(self, num_steps: int) -> torch.Tensor:
-        """The DPM-Solver++ / Euler Ancestral coefficient table on the device."""
+        """The DPM-Solver++ / UniPC / Euler Ancestral coefficient table on the device."""
         return self._schedule(num_steps)[3]
 
     def set_scale(self, scale: float) -> None:
@@ -204,7 +210,7 @@ class DenoiseEngine:
                                             duplicate=loop.use_cfg)
         elif loop.dpm is None:
             ops.scale_model_input(st["latents"], st["model_in"], loop.sigmas, st["step"], duplicate=loop.use_cfg)
-        else:                                        # DPM-Solver++: scale_model_input is the identity
+        else:                                        # DPM-Solver++ / UniPC: scale_model_input is the identity
             n = st["latents"].shape[0]
             st["model_in"][:n].copy_(st["latents"])
             if loop.use_cfg:
@@ -228,7 +234,11 @@ class DenoiseEngine:
                           cond=loop.cond, controlnet_residuals=residuals,
                           adapter_residuals=loop.adapter if adapter else None)
         ib = loop.ib
-        if loop.dpm is not None:
+        if loop.unipc is not None:
+            ops.dpm_solver_step(noise, st["latents"], st["model_in"], loop.dpm["prev_x0"], loop.coeffs, st["step"],
+                                loop.dpm["loop_begin"], loop.guidance, use_cfg=loop.use_cfg,
+                                guidance_rescale=loop.rescale, unipc=loop.unipc)
+        elif loop.dpm is not None:
             ops.dpm_solver_step(noise, st["latents"], st["model_in"], loop.dpm["prev_x0"], loop.coeffs, st["step"],
                                 loop.dpm["loop_begin"], loop.guidance, use_cfg=loop.use_cfg,
                                 guidance_rescale=loop.rescale)
@@ -284,6 +294,11 @@ class DenoiseEngine:
         text-to-image loops, with every option above except begin_step, inpaint, start_step and stop_after (IHError):
         they would need the VP-form add_noise, or the history of another call.
 
+        With a UniPCMultistepScheduler the loop is UniPC (bh2, order 2): the first model input is the latents
+        themselves, and every step first corrects the latents with the new data prediction, then predicts the next
+        latents; the corrected sample and the data predictions of the two previous steps stay on the device.  It has
+        the scope and the refusals of DPM-Solver++.
+
         `unet_cond` = (mask [n,1,h,w], masked_image_latents [n,4,h,w]) is inpainting with the 9-channel inpainting UNet
         ([3P] StableDiffusionXLInpaintPipeline with unet.config.in_channels == 9): every step's UNet input is the scaled
         latents followed by the mask and the masked-image latents (their CFG halves equal), and there is no blend.  It
@@ -319,6 +334,7 @@ class DenoiseEngine:
         draws no random numbers."""
         use_cfg = guidance_scale > 1.0                                            # :223
         is_dpm = isinstance(self.scheduler, DPMSolverMultistepScheduler)         # the one scheduler dispatch
+        is_unipc = isinstance(self.scheduler, UniPCMultistepScheduler)
         is_ancestral = isinstance(self.scheduler, EulerAncestralDiscreteScheduler)
         ucfg = self.unet.config
         n, _, h, w = latents.shape
@@ -326,9 +342,10 @@ class DenoiseEngine:
         # ---- every refusal comes before any allocation, copy or launch
         if use_cfg and (negative_prompt_embeds is None or negative_pooled is None):
             raise IHError("classifier-free guidance needs negative_prompt_embeds / negative_pooled")
-        given = {"DPMSolverMultistepScheduler": is_dpm, "begin_step": bool(begin_step), "inpaint": inpaint is not None,
-                 "unet_cond": unet_cond is not None, "controlnet": controlnet is not None,
-                 "start_step": bool(start_step), "stop_after": stop_after is not None, "adapter": adapter is not None}
+        given = {"DPMSolverMultistepScheduler": is_dpm, "UniPCMultistepScheduler": is_unipc,
+                 "begin_step": bool(begin_step), "inpaint": inpaint is not None, "unet_cond": unet_cond is not None,
+                 "controlnet": controlnet is not None, "start_step": bool(start_step), "stop_after": stop_after is not None,
+                 "adapter": adapter is not None}
         for option, excluded, why in _EXCLUDES:
             clash = [o for o in excluded if given[o]]
             if given[option] and clash:
@@ -407,11 +424,14 @@ class DenoiseEngine:
             st["text_embeds"].copy_(pooled, non_blocking=True)
             st["time_ids"].copy_(time_ids, non_blocking=True)
         C = ucfg.out_channels
-        if is_dpm:      # the previous step's data prediction and the schedule index the loop starts at (first order)
+        if is_dpm or is_unipc:  # the previous steps' data predictions and the index the loop starts at (no history)
             loop.coeffs = coeffs
             loop.dpm = {"prev_x0": self._buf("prev_x0", (n, h, w), (n, C, h, w)),
                         "loop_begin": self._buf("loop_begin", (n, h, w), (1,), torch.int32, zero=True)}
             loop.dpm["loop_begin"].fill_(start_step)
+            if is_unipc:    # the corrected sample and the data prediction of the step before the previous one
+                loop.unipc = (self._buf("last_sample", (n, h, w), (n, C, h, w)),
+                              self._buf("prev_x0_2", (n, h, w), (n, C, h, w)))
         elif is_ancestral:
             loop.coeffs = coeffs
             loop.noise = self._buf("step_noise", (n, h, w, T), (T, n, C, h, w), zero=True)

@@ -11,7 +11,7 @@ from typing import Optional, Tuple
 import torch
 
 from . import _lib
-from ._lib import IHError, check
+from ._lib import IH_SOLVER_DPMPP_2M, IH_SOLVER_UNIPC_BH2, IH_UNIPC_COEFFS, IHError, check
 
 EPI_NONE, EPI_GEGLU, EPI_SILU, EPI_GELU, EPI_QUICK_GELU, EPI_RELU = 0, 1, 2, 4, 8, 16
 TILE_PINGPONG = 1   # IH_TILE_PINGPONG: linear(tile_n=TILE_PINGPONG) forces the ping-pong GEMM kernel
@@ -628,11 +628,19 @@ def euler_inpaint_step(noise_pred: torch.Tensor, latents: torch.Tensor, model_in
 
 def dpm_solver_step(noise_pred: torch.Tensor, latents: torch.Tensor, model_in: torch.Tensor, prev_x0: torch.Tensor,
                     coeffs: torch.Tensor, step: torch.Tensor, loop_begin: torch.Tensor, guidance: float, *,
-                    use_cfg: bool = True, guidance_rescale: float = 0.0) -> None:
-    """One DPM-Solver++ 2M transition (ih_dpm_solver_step) with the loop options of euler_step: the guided prediction's
-    data estimate x0 goes to `prev_x0` for the next step, the new latents to `latents` and, unscaled, to `model_in`.
-    coeffs: fp32 [T, 8] (DPMSolverMultistepScheduler.coeffs) indexed by the device step counter; loop_begin: device
-    int32, the schedule index whose step is first order because it has no history."""
+                    use_cfg: bool = True, guidance_rescale: float = 0.0,
+                    unipc: Optional[Tuple[torch.Tensor, torch.Tensor]] = None) -> None:
+    """One multistep-solver transition (ih_dpm_solver_step) with the loop options of euler_step.  loop_begin: device
+    int32, the schedule index whose step has no history; coeffs is indexed by the device step counter.
+
+    DPM-Solver++ 2M (`unipc` None): the guided prediction's data estimate x0 goes to `prev_x0` for the next step, the
+    new latents to `latents` and, unscaled, to `model_in`; coeffs: fp32 [T, 8] (DPMSolverMultistepScheduler.coeffs).
+
+    UniPC (`unipc` = (last_sample, prev_x0_2)): the corrector rewrites the latents from `last_sample` and the data
+    predictions of the two previous steps (`prev_x0`, `prev_x0_2`), the history shifts, and the predictor writes the
+    new latents to `latents` and, unscaled, to `model_in`; coeffs: fp32 [T, 16] (UniPCMultistepScheduler.coeffs).
+    Its bit-exact kernel test is tests/test_unipc_gpu.py::test_unipc_step_kernel (the op census lists the DPM-Solver++
+    test for this op)."""
     lib = _lib.load()
     _req(noise_pred, "noise_pred"); _req(latents, "latents"); _req(model_in, "model_in"); _req(prev_x0, "prev_x0")
     _req(coeffs, "coeffs", torch.float32); _req(step, "step", torch.int32); _req(loop_begin, "loop_begin", torch.int32)
@@ -641,13 +649,21 @@ def dpm_solver_step(noise_pred: torch.Tensor, latents: torch.Tensor, model_in: t
     want = (2 * n if use_cfg else n) * per
     if noise_pred.numel() != want or model_in.numel() != want:
         raise IHError(f"dpm_solver_step: noise_pred / model_in must hold {want} elements (use_cfg={use_cfg})")
-    if prev_x0.shape != latents.shape or not (latents.is_contiguous() and prev_x0.is_contiguous()):
-        raise IHError("dpm_solver_step: contiguous latents and prev_x0 of one shape required")
-    if coeffs.dim() != 2 or coeffs.shape[1] != 8 or not coeffs.is_contiguous():
-        raise IHError("dpm_solver_step: coeffs must be a contiguous [T, 8] table")
+    hist = (prev_x0,)
+    if unipc is not None:
+        _req(unipc[0], "last_sample"); _req(unipc[1], "prev_x0_2")
+        hist += tuple(unipc)
+    if any(t.shape != latents.shape for t in hist) or not all(t.is_contiguous() for t in (latents,) + hist):
+        raise IHError("dpm_solver_step: contiguous latents, prev_x0 (and last_sample, prev_x0_2) of one shape required")
+    width = 8 if unipc is None else IH_UNIPC_COEFFS
+    if coeffs.dim() != 2 or coeffs.shape[1] != width or not coeffs.is_contiguous():
+        raise IHError(f"dpm_solver_step: coeffs must be a contiguous [T, {width}] table")
+    solver, extra = ((IH_SOLVER_DPMPP_2M, (None, None)) if unipc is None
+                     else (IH_SOLVER_UNIPC_BH2, (unipc[0].data_ptr(), unipc[1].data_ptr())))
     check(lib.ih_dpm_solver_step(noise_pred.data_ptr(), latents.data_ptr(), model_in.data_ptr(), prev_x0.data_ptr(),
                                  coeffs.data_ptr(), step.data_ptr(), loop_begin.data_ptr(), float(guidance),
-                                 float(guidance_rescale), per, n, int(use_cfg), _stream()), "ih_dpm_solver_step")
+                                 float(guidance_rescale), per, n, int(use_cfg), _stream(), solver, *extra),
+          "ih_dpm_solver_step")
 
 
 def euler_ancestral_step(noise_pred: torch.Tensor, latents: torch.Tensor, model_in: torch.Tensor, coeffs: torch.Tensor,

@@ -259,20 +259,37 @@ int ih_euler_inpaint_step(const void* noise_pred, void* latents, void* model_in,
                           const void* image_latents, const void* noise, const void* mask, const void* blend_end,
                           void* stream);
 
-/* DPM-Solver++ 2M transition ([3P] diffusers DPMSolverMultistepScheduler: dpmsolver++, midpoint, epsilon prediction)
- * with the use_cfg / guidance_rescale options and CFG rounding points of ih_euler_step_ex.  Step i = *step reads row i
- * of coeffs, fp32 [T, IH_DPM_COEFFS] computed on the host:
+/* Multistep-solver transition with the use_cfg / guidance_rescale options and CFG rounding points of ih_euler_step_ex.
+ * `solver` picks the scheduler; step i = *step reads row i of its coefficient table `coeffs`, computed on the host
+ * with torch fp32 0-dim arithmetic.  Both write latents and model_in <- latents (unscaled, duplicated with CFG) and
+ * advance the step counter; loop_begin is a device int32, the first schedule index of the loop (only read), whose step
+ * has no history.  prev_x0, last_sample, prev_x0_2: [n,C,H,W] fp16 buffers the solver keeps between steps.
+ *
+ * IH_SOLVER_DPMPP_2M ([3P] diffusers DPMSolverMultistepScheduler: dpmsolver++, midpoint, epsilon prediction):
+ * coeffs fp32 [T, IH_DPM_COEFFS]
  *   {sigma_s, 1/alpha_s, sigma_t/sigma_s, c = alpha_t*(exp(-h)-1), 0.5*c, 1/r0, first, 0}
  * (VP sigmas, h = lambda_t - lambda_s, r0 = h_prev / h).  With eps the guided prediction and x the fp16 latents:
  *   x0 = fp16(fp16(x - fp16(sigma_s*eps)) * (1/alpha_s));
  *   x  <- fp16(fp32(ratio*x) - fp16(c*x0) [- fp16(0.5c * fp16(1/r0 * fp16(x0 - prev_x0)))])
- * where the bracket (second order) is dropped iff i == *loop_begin or first != 0.  Writes latents, prev_x0 <- x0 and
- * model_in <- x (unscaled, duplicated with CFG); step counter i += 1.  prev_x0: [n,C,H,W] fp16; loop_begin: device
- * int32, the first schedule index of the loop (only read). */
+ * where the bracket (second order) is dropped iff i == *loop_begin or first != 0.  prev_x0 <- x0.  last_sample and
+ * prev_x0_2 must be null.
+ *
+ * IH_SOLVER_UNIPC_BH2 ([3P] diffusers UniPCMultistepScheduler: bh2, solver_order 2, predict_x0, epsilon prediction):
+ * coeffs fp32 [T, IH_UNIPC_COEFFS]
+ *   {sigma_s, 1/alpha_s, p_ratio, p_c, 1/rk_p, p, c_ratio, c_c, 1/rk_c, rho0, rho1, c, 0, 0, 0, 0}
+ * with the predictor's scalars from sigma_i -> sigma_{i+1} and the corrector's from sigma_{i-1} -> sigma_i (ratio =
+ * sigma_t/sigma_s0 of VP sigmas, c = alpha_t*expm1(-h), rk = (lambda_{s_k} - lambda_s0)/h, rho = fp16 rhos_c) and the
+ * orders p = min(2, T-i, i+1), c = p(i-1) (0 at i = 0).  The corrector of order c rewrites x from last_sample,
+ * prev_x0 (and prev_x0_2 when c == 2) and x0; then prev_x0_2 <- prev_x0 <- x0, last_sample <- x, and the predictor
+ * of order p steps x to the latents (SURVEY A.9).  A loop starting at b = *loop_begin lowers the orders to
+ * p <= i - b + 1 and c <= i - b.  last_sample and prev_x0_2 are required. */
+#define IH_SOLVER_DPMPP_2M 0
+#define IH_SOLVER_UNIPC_BH2 1
 #define IH_DPM_COEFFS 8
+#define IH_UNIPC_COEFFS 16
 int ih_dpm_solver_step(const void* noise_pred, void* latents, void* model_in, void* prev_x0, const void* coeffs,
                        void* step, const void* loop_begin, float guidance, float guidance_rescale, long long n_per_image,
-                       int n_images, int use_cfg, void* stream);
+                       int n_images, int use_cfg, void* stream, int solver, void* last_sample, void* prev_x0_2);
 
 /* Euler Ancestral transition ([3P] diffusers EulerAncestralDiscreteScheduler, epsilon prediction) with the use_cfg /
  * guidance_rescale options and CFG rounding points of ih_euler_step_ex.  Step i = *step reads row i of coeffs, fp32

@@ -8,7 +8,8 @@ a dependency here, so the pieces the reference touches are provided directly:
 Denoise loop semantics follow custom_pipelines.py:188-363 (CFG batch [negative, positive], per-step IP-scale gating
 by control_guidance_start/end, Euler update); the loop itself runs as replayed CUDA graphs (imagharmony_b200/denoise.py).
 Text-to-image also runs DPM-Solver++ 2M: pass `scheduler=DPMSolverMultistepScheduler.from_config(pipe.scheduler.config,
-use_karras_sigmas=True)` or assign it to `pipe.scheduler`, as with diffusers.  Text-to-image, image-to-image and
+use_karras_sigmas=True)` or assign it to `pipe.scheduler`, as with diffusers, and UniPC likewise:
+`pipe.scheduler = UniPCMultistepScheduler.from_config(pipe.scheduler.config)`.  Text-to-image, image-to-image and
 inpainting run Euler Ancestral (`EulerAncestralDiscreteScheduler.from_config(pipe.scheduler.config)`), whose per-step
 noise comes from the call's `generator` in diffusers' order.
 VAE decode / PIL post-processing (:365-386, scope row f1) runs on the native decoder `imagharmony_b200.vae` when the
@@ -32,7 +33,7 @@ from imagharmony_b200._lib import IHError
 from imagharmony_b200.config import SDXL_BASE, SDXL_CONTROLNET, ControlNetConfig, UNetConfig, config_from_diffusers
 from imagharmony_b200.denoise import DenoiseEngine
 from imagharmony_b200.scheduler import (DPMSolverMultistepScheduler, EulerAncestralDiscreteScheduler,
-                                        EulerDiscreteScheduler, randn_tensor)
+                                        EulerDiscreteScheduler, UniPCMultistepScheduler, randn_tensor)
 from imagharmony_b200.unet import UNet2DConditionModel, require_latent_size
 from imagharmony_b200.weights import random_module
 
@@ -151,7 +152,8 @@ class StableDiffusionXLCustomPipeline:
 
     def __init__(self, unet: UNet2DConditionModel, prompt_encoder: Optional[Callable] = None,
                  vae_decode: Optional[Callable] = None,
-                 scheduler: Optional[Union[EulerDiscreteScheduler, DPMSolverMultistepScheduler]] = None, vae=None):
+                 scheduler: Optional[Union[EulerDiscreteScheduler, DPMSolverMultistepScheduler,
+                                            UniPCMultistepScheduler]] = None, vae=None):
         if unet.config.num_time_ids not in self.TIME_IDS:
             raise IHError(f"{type(self).__name__} needs a UNet with {' or '.join(map(str, self.TIME_IDS))} "
                           f"micro-conditioning ids; this one has {unet.config.num_time_ids} (a UNet that requires an "
@@ -664,7 +666,8 @@ class StableDiffusionXLImg2ImgPipeline(StableDiffusionXLCustomPipeline):
 
     def __init__(self, unet: UNet2DConditionModel, prompt_encoder: Optional[Callable] = None,
                  vae_decode: Optional[Callable] = None,
-                 scheduler: Optional[Union[EulerDiscreteScheduler, DPMSolverMultistepScheduler]] = None, vae=None,
+                 scheduler: Optional[Union[EulerDiscreteScheduler, DPMSolverMultistepScheduler,
+                                            UniPCMultistepScheduler]] = None, vae=None,
                  vae_encoder=None):
         super().__init__(unet, prompt_encoder=prompt_encoder, vae_decode=vae_decode, scheduler=scheduler, vae=vae)
         self.vae_encoder = vae_encoder      # imagharmony_b200.vae.AutoencoderKLEncoder or None
@@ -812,10 +815,11 @@ class StableDiffusionXLImg2ImgPipeline(StableDiffusionXLCustomPipeline):
 
     def _require_euler(self) -> None:
         """Image-to-image and inpainting noise the image latents with Euler's add_noise (x + sigma * noise) inside the
-        posterior kernel; DPM-Solver++ noises in VP form (alpha * x + sigma_vp * noise), which it does not compute."""
-        if isinstance(self.scheduler, DPMSolverMultistepScheduler):
+        posterior kernel; DPM-Solver++ and UniPC noise in VP form (alpha * x + sigma_vp * noise), which it does not
+        compute."""
+        if isinstance(self.scheduler, (DPMSolverMultistepScheduler, UniPCMultistepScheduler)):
             raise IHError(f"{type(self).__name__} supports EulerDiscreteScheduler and EulerAncestralDiscreteScheduler; "
-                          "DPMSolverMultistepScheduler runs text-to-image (StableDiffusionXLCustomPipeline)")
+                          f"{type(self.scheduler).__name__} runs text-to-image (StableDiffusionXLCustomPipeline)")
 
     def _begin_index(self, num_inference_steps: int, strength: float) -> int:
         """[3P] check_inputs and get_timesteps: the schedule index t_start a run of `strength` begins at."""
